@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native SimpleTuner training step.
+"""bench.py — headline benchmark of the SimpleTuner training step on H100 (sm_90a kernels of libstb200).
 
 Workload (BASELINE.json configs[1]): Flux.1-dev (19 double + 38 single MMDiT blocks, D=3072, 24x128 heads,
 guidance-distilled) LoRA rank 16 on all attention projections, bf16, 1024x1024 images as cached latents
-[B,16,128,128] + cached T5 embeds [B,512,4096] + pooled CLIP [B,768], batch 4 per GPU.  Weights are
+[B,16,128,128] + cached T5 embeds [B,512,4096] + pooled CLIP [B,768], batch 1 per GPU (80 GB H100).  Weights are
 random-init of that architecture and data is synthetic (no network): said in `data`.
 
 One "step" = prepare_batch (noise + sigma sampling + noisy latents + patchify) -> model_predict
@@ -31,6 +31,7 @@ ROOT = Path(__file__).resolve().parent
 if str(ROOT) not in sys.path:
     sys.path.insert(0, str(ROOT))
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 METRIC = "images/sec Flux.1-dev LoRA bf16 1024^2"
@@ -49,8 +50,9 @@ def measured_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return d, "MEASURED_PEAKS.json"
+    # NVIDIA H100 SXM data sheet (dense, 700 W); a card at a lower power limit does not reach it
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet, dense bf16 at 700 W"
 
 
 # ------------------------------------------------------------------------------------------------ clocks
@@ -176,7 +178,7 @@ def synth_batch(B, device, pinned=False, seed=0, hw=128, s_txt=S_TXT, joint=4096
     return {k: v.to(device) for k, v in b.items()}
 
 
-# SD3.5-medium geometry (BASELINE configs[2]: "SD3-medium MMDiT full fine-tune bf16, 512^2 aspect buckets, batch=8, 8xB200 DDP")
+# SD3.5-medium geometry (BASELINE configs[2]: "SD3-medium MMDiT full fine-tune bf16, 512^2 aspect buckets, batch=8, 8xH100 DDP")
 SD35_MEDIUM = dict(sample_size=128, patch_size=2, in_channels=16, num_layers=24, attention_head_dim=64, num_attention_heads=24,
                    joint_attention_dim=4096, caption_projection_dim=1536, pooled_projection_dim=2048, out_channels=16,
                    pos_embed_max_size=384, dual_attention_layers=tuple(range(13)), qk_norm="rms_norm")
@@ -236,7 +238,7 @@ def synth_batch_sd3(B, device, hw, pinned=False, seed=0, s_txt=SD3_S_TXT, joint=
     return {k: v.to(device) for k, v in b.items()}
 
 
-# PixArt-Sigma XL (BASELINE configs[4]: "PixArt-Sigma DiT LoRA rank=32, mixed aspect buckets 512-1536, grad-accum=4, 8xB200")
+# PixArt-Sigma XL (BASELINE configs[4]: "PixArt-Sigma DiT LoRA rank=32, mixed aspect buckets 512-1536, grad-accum=4, 8xH100")
 PIXART_SIGMA = dict(num_attention_heads=16, attention_head_dim=72, in_channels=4, out_channels=8, num_layers=28, cross_attention_dim=1152,
                     sample_size=128, caption_channels=4096)
 PIXART_BUCKETS = [(64, 64), (96, 128), (128, 128), (112, 144), (160, 160), (192, 192), (128, 96), (144, 112)]   # latent (h, w): 512^2 .. 1536^2 px
@@ -377,7 +379,7 @@ def run_vae(args):
                         "d2h_bytes_per_step": out_host.numel() * 2, "ms_per_step": ms_e2e / args.steps},
                 "gpu_launches": int(launches), "clocks": clocks,
                 "roofline": {"bound": "tensor", "kernel": "whole encode (implicit-GEMM 3x3 convs dominate)", "achieved": round(ach, 1), "peak": peak_tf,
-                             "unit": "TFLOP/s", "frac": round(ach / peak_tf, 4), "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peak_src})",
+                             "unit": "TFLOP/s", "frac": round(ach / peak_tf, 4), "peak_source": peak_src,
                              "traffic": None},
                 "model_tflops": {"algorithmic_tf_per_image": round(tf_img, 2), "achieved_tflops_per_gpu": round(ach, 1)},
                 "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1)}
@@ -482,7 +484,7 @@ def run_text(args):
                 "gpu_launches": int(launches), "clocks": clocks,
                 "roofline": {"bound": "tensor", "kernel": "whole encode (T5 projections / feed-forward GEMMs dominate)", "achieved": round(ach, 1),
                              "peak": peak_tf, "unit": "TFLOP/s", "frac": round(ach / peak_tf, 4),
-                             "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peak_src})", "traffic": None},
+                             "peak_source": peak_src, "traffic": None},
                 "model_tflops": {"algorithmic_tf_per_prompt": round(tf_prompt, 3), "achieved_tflops_per_gpu": round(ach, 1)},
                 "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2 ** 30, 1)}
         print(json.dumps(line))
@@ -667,7 +669,7 @@ def eager_gpu_step_fn(wrapper, device):
     """What the reference's DEFAULT path costs on this box (informational): the dtype-agnostic oracle restatement of the
     diffusers modules run as eager bf16 torch ops on the GPU, attention through `F.scaled_dot_product_attention`
     (attention_mechanism="diffusers"), PEFT-style un-fused LoRA matmuls, every block under torch.utils.checkpoint
-    (gradient_checkpointing=true is the reference default), sharing the B200 model's own parameter tensors."""
+    (gradient_checkpointing=true is the reference default), sharing the libstb200 model's own parameter tensors."""
     import torch.nn.functional as F
     from torch.utils.checkpoint import checkpoint
 
@@ -742,6 +744,24 @@ def time_eager_gpu(wrapper, device, batches, opt, steps=3, warmup=2):
     return e0.elapsed_time(e1) / steps
 
 
+DUMP_PARAM_SAMPLES = 1 << 22   # 16 MB of float32
+
+
+def dump_outputs(out_dir, loss, params):
+    """What the timed training step hands back to its caller after the last timed step: the loss of that step and the
+    trainable parameters it updated.  The parameters are written as a fixed, seeded sample (the same element indices for
+    the same configuration) of their concatenation in `parameters()` order, in float32."""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    np.save(out / "loss.npy", loss.detach().float().reshape(1).cpu().numpy())
+    flat = torch.cat([p.detach().reshape(-1) for p in params])
+    if flat.numel() > DUMP_PARAM_SAMPLES:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randint(0, flat.numel(), (DUMP_PARAM_SAMPLES,), generator=g).sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(out / "params_sample.npy", flat.float().cpu().numpy())
+
+
 def run_b200(args):
     import torch.distributed as dist
 
@@ -758,7 +778,11 @@ def run_b200(args):
     sd3 = args.config == "sd3_fullft"
     pix = args.config == "pixart_lora"
     lokr = args.config == "flux_lokr"
-    B = args.batch if args.batch else (8 if sd3 else (2 if lokr else 4))
+    # torch seeds its default generators randomly per process; the adapter initialisation (PEFT's kaiming_uniform_ on
+    # lora_A, LoKr factors) draws from them, so seed before the model is built, as the reference's set_seed does
+    torch.manual_seed(42 + rank)
+    # Flux.1-dev at 1024^2 without gradient checkpointing: one sample per step fits an 80 GB H100
+    B = args.batch if args.batch else (8 if sd3 else (4 if pix else 1))
     cfg_over = None
     hw, s_txt = 128, S_TXT
     if args.tiny:  # plumbing check only (never a bench value)
@@ -840,12 +864,6 @@ def run_b200(args):
     nbat = len(dev_batches)
     if use_graph:      # every bucket shape must be captured BEFORE the timed region
         args.warmup = max(args.warmup, nbat)
-    if (sd3 or pix) and not args.tiny:
-        # every rank must time the SAME multiset of buckets (ranks only start at different offsets): round the step count up so
-        # that the timed micro-batches are whole cycles of the bucket list
-        import math
-        cyc = nbat // math.gcd(nbat, accum)
-        args.steps = ((args.steps + cyc - 1) // cyc) * cyc
 
     def barrier():
         if world > 1:
@@ -869,16 +887,17 @@ def run_b200(args):
         return float(ms.item())
 
     per_rank_ms = []
+    last_loss = [None]
     # ---- device-resident arm
     def dev_step(i):
         for a_ in range(accum):
-            step({k: v for k, v in dev_batches[(i * accum + a_) % nbat].items()})
+            last_loss[0] = step({k: v for k, v in dev_batches[(i * accum + a_) % nbat].items()})
 
     for i in range(args.warmup):
         dev_step(i)
     if os.environ.get("STB_NCU_RANGE"):
-        # `ncu --profile-from-start off ...`: exactly ONE device-resident step inside the profiler range (launch list for
-        # profiles/); numbers printed under a profiler are never bench values, so nothing is printed
+        # a profiler started with collection off: exactly ONE device-resident step inside the profiler range (launch list);
+        # numbers printed under a profiler are never bench values, so nothing is printed
         torch.cuda.synchronize()
         torch.cuda.profiler.start()
         dev_step(args.warmup)
@@ -893,6 +912,8 @@ def run_b200(args):
     launches = ops.launch_count()
     clocks = sampler.stop() if rank == 0 else None
     step.check_finite()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss[0], params)
 
     # ---- end-to-end arm: pinned host batch -> H2D -> step -> D2H loss, every step
     loss_host = torch.empty((), dtype=torch.float32).pin_memory()
@@ -924,16 +945,10 @@ def run_b200(args):
         roof = None
         if kern and "gemm_big" in kern:
             gb = kern["gemm_big"]
-            traffic = None
-            tp = ROOT / "profiles" / "r01" / "gemm_traffic.json"
-            if tp.exists():  # dram__bytes_read+write of one ncu --set full capture of this kernel (committed summary)
-                tj = json.loads(tp.read_text())
-                traffic = {"dram_bytes_per_launch": tj["dram_bytes_total"], "algorithmic_bytes": tj["algorithmic_bytes"],
-                           "shape": tj["shape"], "source": tj["source"]}
-            roof = {"bound": "tensor", "kernel": "gemm_bf16_tn_kernel (tcgen05, all >=0.1 TFLOP launches of one step)",
+            traffic = None   # not measured on H100
+            roof = {"bound": "tensor", "kernel": "gemm_bf16_tn_kernel (wgmma, all >=0.1 TFLOP launches of one step)",
                     "achieved": gb["tflops"], "peak": peak_tf, "unit": "TFLOP/s", "frac": round(gb["tflops"] / peak_tf, 4),
-                    "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peak_src}): cuBLAS bf16 back to back for 4 s, "
-                                   "the right denominator for a kernel timed inside a long power-capped step",
+                    "peak_source": peak_src,
                     "peak_burst": float(peaks.get("bf16_tflops", 0.0)),
                     "frac_of_burst": round(gb["tflops"] / float(peaks.get("bf16_tflops", peak_tf)), 4), "traffic": traffic,
                     "avg_launch_ms": gb["avg_ms"], "tflop_per_launch": gb["tflop_per_launch"], "launches_per_step": gb["launches"]}
@@ -1000,7 +1015,7 @@ def run_b200(args):
         if (sd3 or pix) and roof is None:
             ach = tf_sample * B * accum / (ms_step * 1e-3)
             roof = {"bound": "tensor", "kernel": "whole step, algorithmic FLOPs (SURVEY 8d counting)", "achieved": round(ach, 1),
-                    "peak": peak_tf, "unit": "TFLOP/s", "frac": round(ach / peak_tf, 4), "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peak_src})",
+                    "peak": peak_tf, "unit": "TFLOP/s", "frac": round(ach / peak_tf, 4), "peak_source": peak_src,
                     "traffic": None}
             line["roofline"] = roof
         if world == 1 and not args.no_eager_baseline and not args.tiny and not (sd3 or pix):
@@ -1032,9 +1047,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=8)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last timed step's outputs (loss, updated trainable parameters) as DIR/<name>.npy")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--batch", type=int, default=0, help="per-GPU batch (default: 4 for flux_lora, 8 for sd3_fullft)")
+    ap.add_argument("--batch", type=int, default=0, help="per-GPU batch (default: 1 for flux_lora / flux_lokr, 8 for sd3_fullft, 4 for pixart_lora)")
     ap.add_argument("--config", default="flux_lora", choices=["flux_lora", "sd3_fullft", "pixart_lora", "vae_encode", "flux_lokr", "text_encode"],
                     help="flux_lora = BASELINE configs[1] (the headline metric); sd3_fullft = configs[2] (SD3.5-medium full fine-tune); "
                          "pixart_lora = configs[4] (PixArt-Sigma LoRA r32, mixed buckets, grad-accum 4); vae_encode = the VAE cache path")
@@ -1057,6 +1074,8 @@ def main():
         args.dp = "flat"
     if args.warmup < 3 and args.impl == "b200" and not args.tiny:
         args.warmup = 3
+    if args.dump_outputs and (args.impl == "reference" or args.config in ("vae_encode", "text_encode")):
+        ap.error("--dump-outputs is supported for the training-step configurations of --impl b200")
     if args.impl == "reference":
         run_reference(args)
     elif args.config == "vae_encode":

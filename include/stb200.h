@@ -1,9 +1,9 @@
-/* stb200.h — C ABI of libstb200.so: the sm_100a kernels of the SimpleTuner diffusion training step.
+/* stb200.h — C ABI of libstb200.so: the sm_90a (H100) kernels of the SimpleTuner diffusion training step.
  *
  * Plain pointers, sizes and element strides only; every pointer is a CUDA device pointer unless
  * noted, every tensor is bf16 unless noted, `stream` is a cudaStream_t.  All functions return 0 on
  * success and a negative code on failure; stb_last_error() returns the message of the last failure
- * on the calling thread.  There is no CPU fallback: without an sm_100 device every launch fails.
+ * on the calling thread.  There is no CPU fallback: without an sm_90 (H100) device every launch fails.
  *
  * The reference (bghira/SimpleTuner) has no FFI for this path — its seams are Python-level
  * (SURVEY.md §8b).  Each entry point below names the reference call site it replaces; the Python
@@ -75,7 +75,8 @@ typedef struct {
   long long res_batch_stride, res_row_stride;
   void* aux;
   long long aux_batch_stride, aux_row_stride;
-  int tile_mt, tile_bn; /* 0 = pick automatically; else MT in {1,2}, BN in {64,128,256} */
+  int tile_mt, tile_bn; /* 0 = pick automatically; else BN in {64,128,256}.  MT (0..3) is accepted for compatibility;
+                           every tile is 128 rows */
 } stb_gemm_args;
 
 int stb_gemm_bf16(const stb_gemm_args* args, void* stream);
@@ -172,7 +173,8 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
  *                        (common.py:4610-4611, 6286, 6426-6429) with pred in packed layout
  *                        (layout 0: Flux unpack_latents order, flux/__init__.py:33-44; layout 1: SD3
  *                        unpatchify order "nhwpqc->nchpwq", sd3/transformer.py:894); optional d loss/d pred.
- * latents/noise: bf16 [B, C, Hh, Ww] contiguous; sigmas fp32 [B]; loss_out fp32 [1] (zeroed here).
+ * latents/noise: bf16 [B, C, Hh, Ww] contiguous; sigmas fp32 [B]; loss_out fp32 [1] (written; the reduction has a fixed
+ * order, so the loss is the same bit for bit from run to run).
  * loss_type (both loss entry points): 0 = l2, 1 = huber, 2 = smooth_l1 as `conditional_loss` defines them
  * (common.py:6132-6166): huber = 2c(sqrt(d^2+c^2)-c), smooth_l1 = 2(sqrt(d^2+c^2)-c); huber_c = fp32 [B]
  * per-sample c (constant or the scheduled value of common.py:6168-6215), may be NULL for l2.
@@ -301,7 +303,7 @@ int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm
 /* ---------------------------------------------------------------------------------------------
  * VAE latent encode (diffusers AutoencoderKL.encode as called at reference common.py:2766-2772 from
  * caching/vae.py:1311; sampling caching/vae.py:1337; scaling foundation_mixins.py:68-81).
- * Activations are NHWC bf16; every 3x3 conv is a tcgen05 implicit GEMM (9 shifted K-segments, the halo
+ * Activations are NHWC bf16; every 3x3 conv is a wgmma implicit GEMM (9 shifted K-segments, the halo
  * is zero-filled by TMA); 1x1 convs / attention projections are stb_gemm_bf16 over pixels.
  *   stb_conv3x3_nhwc : out[B,Ho,Wo,Co] = conv3x3(x[B,H,W,Ci]; w[Co, 9*Ci] tap-major (dy,dx,ci)) + bias (+ res)
  *                      stride 1: padding 1;  stride 2: F.pad(x,(0,1,0,1)) then stride-2 (Downsample2D)

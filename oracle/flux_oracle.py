@@ -11,7 +11,7 @@ function, of the arithmetic that SimpleTuner's Flux training step performs:
   * Flux._model_predict_single               reference flux/model.py:707-864
   * flow-matching batch prep / target / loss reference common.py:4975-4992, 4610-4611, 6286, 6426-6429
 The layer classes that the reference imports from the third-party `diffusers` package
-(diffusers>=0.36.0, reference setup.py:287 — NOT vendored under /root/reference and not installed
+(diffusers>=0.36.0, reference setup.py:287 — NOT vendored in the reference and not installed
 here) are restated from their published semantics: Attention + RMSNorm, AdaLayerNormZero /
 ZeroSingle / Continuous, FeedForward("gelu-approximate"), FluxPosEmbed (get_1d_rotary_pos_embed),
 CombinedTimestep(Guidance)TextProjEmbeddings, PEFT lora.Linear.

@@ -4,7 +4,7 @@
 targets = modules of class `Attention` and `FeedForward`).
 
 PARITY UNPINNED: the algorithm lives in the third-party package `lycoris-lora` (setup.py:319 pins `>=3.4.0`), which is not
-vendored under /root/reference and not installed in this image, so it is restated here from its published definition
+vendored in the reference and not installed in this image, so it is restated here from its published definition
 (lycoris/modules/lokr.py, lycoris/functional/general.py::factorization, lycoris/functional/lokr.py::make_kron) and anchored on
 the reference's own use of the module's attributes (`lokr_w1`, `lokr_w2`, `org_weight`: helpers/training/peft_init.py:34-38):
 

@@ -1,5 +1,5 @@
 """Generate tests/golden/flux_step_golden.pt by running the reference's own functions
-(via oracle/ref_extract.py, /root/reference mounted) on seeded inputs.  TEST INFRASTRUCTURE ONLY.
+(via oracle/ref_extract.py, with $SIMPLETUNER_SRC naming a SimpleTuner checkout) on seeded inputs.  TEST INFRASTRUCTURE ONLY.
 
 Run in the build container:   python -m oracle.make_golden
 """
@@ -16,7 +16,7 @@ OUT = Path(__file__).resolve().parent.parent / "tests" / "golden" / "flux_step_g
 
 
 def main():
-    assert rx.available(), "/root/reference is not mounted here"
+    assert rx.available(), "set SIMPLETUNER_SRC to a SimpleTuner checkout"
     g = {}
     gen = torch.Generator().manual_seed(1234)
 

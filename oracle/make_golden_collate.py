@@ -15,7 +15,7 @@ OUT = Path(__file__).resolve().parent.parent / "tests" / "golden" / "collate_gol
 
 
 def main():
-    assert rx.available(), "/root/reference is not mounted here"
+    assert rx.available(), "set SIMPLETUNER_SRC to a SimpleTuner checkout"
     g = {}
     tracker = SimpleNamespace(is_sdxl_refiner=lambda: False, get_args=lambda: SimpleNamespace(data_aesthetic_score=7.0),
                               get_accelerator=lambda: SimpleNamespace(device="cpu"))

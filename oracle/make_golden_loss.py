@@ -44,7 +44,7 @@ def lifted(prediction_type, alphas_cumprod=None, **cfg):
 
 
 def main():
-    assert rx.available(), "/root/reference is not mounted here"
+    assert rx.available(), "set SIMPLETUNER_SRC to a SimpleTuner checkout"
     gen = torch.Generator().manual_seed(4321)
     B, C, H, W = 3, 4, 8, 12
     g = {"pred": torch.randn(B, C, H, W, generator=gen).bfloat16(),

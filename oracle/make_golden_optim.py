@@ -31,7 +31,7 @@ class _TorchProxy:
 
 
 def main():
-    assert rx.available(), "/root/reference is not mounted here"
+    assert rx.available(), "set SIMPLETUNER_SRC to a SimpleTuner checkout"
     gen = torch.Generator().manual_seed(2024)
     proxy = _TorchProxy(gen)
     st = rx.functions("helpers/training/optimizers/adamw_bfloat16/stochastic/__init__.py",

@@ -3,15 +3,16 @@
 The reference package cannot be imported in this container (diffusers / accelerate / peft are not
 installed, SURVEY.md §8c) but its pure-torch helpers can be lifted out of the source files with
 `ast` and exec'ed with only torch/math/random in scope.  Nothing is copied into this repository:
-the source text is read from /root/reference at run time, so this module only works where that
-mount exists (the build container), and is used by oracle/make_golden.py to produce the committed
-fixtures under tests/golden/.
+the source text is read at run time from a SimpleTuner checkout named by the SIMPLETUNER_SRC environment
+variable (the directory holding the `simpletuner` package), so this module only works where that checkout
+exists, and is used by the oracle/make_golden*.py scripts to produce the committed fixtures under tests/golden/.
 """
 from __future__ import annotations
 
 import ast
 import logging
 import math
+import os
 import random
 import types
 from pathlib import Path
@@ -20,11 +21,14 @@ from typing import Dict, Iterable
 import torch
 import torch.nn.functional as F
 
-REF_ROOT = Path("/root/reference/simpletuner")
+REF_ROOT = Path(os.environ.get("SIMPLETUNER_SRC", "")) / "simpletuner"
 
 
 def available() -> bool:
-    return REF_ROOT.exists()
+    try:
+        return bool(os.environ.get("SIMPLETUNER_SRC")) and REF_ROOT.is_dir()
+    except OSError:
+        return False
 
 
 def _namespace() -> Dict[str, object]:

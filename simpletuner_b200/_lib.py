@@ -1,7 +1,7 @@
 """ctypes binding of libstb200.so (C ABI declared in include/stb200.h).
 
-The shared library is built in-tree by :func:`build` (nvcc, sm_100a only) and loaded lazily by
-:func:`lib`.  There is no fallback: if the library is missing or the device is not sm_100 the
+The shared library is built in-tree by :func:`build` (nvcc, sm_90a only) and loaded lazily by
+:func:`lib`.  There is no fallback: if the library is missing or the device is not sm_90 (H100) the
 product path raises.
 """
 from __future__ import annotations
@@ -19,7 +19,7 @@ LIB_PATH = Path(os.environ["STB200_LIB"]) if os.environ.get("STB200_LIB") else L
 INCLUDE = _HERE.parent / "include" / "stb200.h"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--shared", "-Xcompiler", "-fPIC",
 ]

@@ -18,9 +18,7 @@
 #include <climits>
 #include "../../include/stb200.h"
 #include "attn_bwd.cuh"
-#include "attn_bwd128.cuh"
 #include "attn_fwd.cuh"
-#include "attn_fwd_pair.cuh"
 #include "optim.cuh"
 #include "elementwise.cuh"
 #include "gemm.cuh"
@@ -73,9 +71,11 @@ int check_device() {
     int dev = 0, major = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return 0;
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-    return major == 10 ? 1 : 0;
+    int minor = 0;
+    if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+    return major == 9 && minor == 0 ? 1 : 0;
   }();
-  if (!ok) return fail(STB_ERR_UNSUPPORTED, "libstb200 needs an sm_100 (B200) device; there is no CPU or other-arch fallback");
+  if (!ok) return fail(STB_ERR_UNSUPPORTED, "libstb200 needs an sm_90 (H100) device; there is no CPU or other-arch fallback");
   return 0;
 }
 
@@ -189,9 +189,9 @@ int set_smem(K kernel, int bytes) {
 }
 
 // ---------------------------------------------------------------- GEMM
-template <int MT, int BN, bool PAIR = false>
+template <int BN>
 int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
-  using Cfg = typename std::conditional<PAIR, stb::GemmPairCfg<BN>, stb::GemmCfg<MT, BN>>::type;
+  using Cfg = stb::GemmCfg<BN>;
   stb::GemmMaps maps;
   std::memset(&maps, 0, sizeof maps);
   stb::GemmParams p;
@@ -213,13 +213,11 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
     } else {
       unsigned long long wd[2] = {(unsigned long long)g.K, (unsigned long long)a->N};
       unsigned long long ws[1] = {(unsigned long long)g.w_row_stride * 2ull};
-      unsigned wb[2] = {64, (unsigned)(PAIR ? BN / 2 : BN)};   // pair: each CTA stages half of the W rows
+      unsigned wb[2] = {64, (unsigned)BN};
       if (int r = make_map(&maps.w[s], g.w, 2, wd, ws, wb)) return r;
     }
     p.w_kn[s] = g.w_kn ? 1 : 0;
     p.kblocks[s] = (g.K + 63) / 64;
-    int rem = g.K - (p.kblocks[s] - 1) * 64;
-    p.kmmas_last[s] = (rem + 15) / 16;
   }
   p.rows_per_batch = a->rows_per_batch;
   p.num_batches = a->num_batches;
@@ -240,40 +238,17 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   p.aux_batch_stride = a->aux_batch_stride;
   p.aux_row_stride = a->aux_row_stride;
 
-  auto kernel = stb::gemm_bf16_tn_kernel<MT, BN, false, PAIR>;
+  auto kernel = stb::gemm_bf16_tn_kernel<BN, false>;
   static bool configured = false;
   if (!configured) {
     if (int r = set_smem(kernel, Cfg::SMEM_BYTES)) return r;
     configured = true;
   }
-  const int tiles_m = ((a->rows_per_batch + Cfg::BM - 1) / Cfg::BM) * a->num_batches;
-  const int tiles_n = (a->N + BN - 1) / BN;
-  const long long tiles = (long long)tiles_m * tiles_n;
-  if constexpr (PAIR) {
-    // one 2-CTA cluster (a TPC's two SMs) per 256 x BN tile stream
-    const int clusters = (int)std::min<long long>(tiles, num_sms() / 2);
-    cudaLaunchConfig_t cfg;
-    std::memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3(2 * clusters);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    STB_CUDA(cudaLaunchKernelEx(&cfg, kernel, maps, p));
-    g_launches.fetch_add(1);
-    return 0;
-  } else {
-    const int grid = (int)std::min<long long>(tiles, num_sms());
-    kernel<<<grid, 256, Cfg::SMEM_BYTES, st>>>(maps, p);
-    STB_LAUNCH_CHECK("gemm_bf16_tn");
-    return 0;
-  }
+  const long long tiles = (long long)((a->rows_per_batch + Cfg::BM - 1) / Cfg::BM) * a->num_batches * ((a->N + BN - 1) / BN);
+  const int grid = (int)std::min<long long>(tiles, num_sms());
+  kernel<<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
+  STB_LAUNCH_CHECK("gemm_bf16_tn");
+  return 0;
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -290,31 +265,18 @@ static int launch_attn_bwd(const stb_attn_bwd_args* a, const stb::AttnBwdMaps& m
         static_cast<const __nv_bfloat16*>(a->d_o), a->do_b, a->do_s, a->do_h, a->delta, a->B, a->H, a->Sq);
     STB_LAUNCH_CHECK("attn_bwd_delta");
   }
-  // Kernel selection: the 128-wide phase-split kernels (attn_bwd128.cuh) are the default; the 64-wide double-buffered ones
-  // (attn_bwd.cuh) remain for the fused q / k pre-processing epilogue (qk_prep) and for A/B timing
-  // (STB_ATTN_BWD_DKDV=64 / STB_ATTN_BWD_DQ=64, read once per process).
-  static const bool old_dkdv = [] { const char* e = std::getenv("STB_ATTN_BWD_DKDV"); return e && e[0] == '6'; }();
-  static const bool old_dq = [] { const char* e = std::getenv("STB_ATTN_BWD_DQ"); return e && e[0] == '6'; }();
   constexpr int SMEM = stb::AttnBwdCfg<HD>::SMEM_BYTES;
-  constexpr int SMEM_DKDV = stb::AttnBwd128Cfg<HD>::SMEM_DKDV;
-  constexpr int SMEM_DQ = stb::AttnBwd128Cfg<HD>::SMEM_DQ;
   auto k1 = stb::attn_bwd_dkdv_kernel<HD>;
   auto k2 = stb::attn_bwd_dq_kernel<HD>;
-  auto n1 = stb::attn_bwd_dkdv128_kernel<HD>;
-  auto n2 = stb::attn_bwd_dq128_kernel<HD>;
   static bool configured = false;
   if (!configured) {
     if (int r = set_smem(k1, SMEM)) return r;
     if (int r = set_smem(k2, SMEM)) return r;
-    if (int r = set_smem(n1, SMEM_DKDV)) return r;
-    if (int r = set_smem(n2, SMEM_DQ)) return r;
     configured = true;
   }
-  if (p.fuse_prep || old_dkdv) k1<<<dim3((a->Sk + 127) / 128, a->H, a->B), 384, SMEM, st>>>(maps, p);
-  else n1<<<dim3((a->Sk + 127) / 128, a->H, a->B), 384, SMEM_DKDV, st>>>(maps, p);
+  k1<<<dim3((a->Sk + 127) / 128, a->H, a->B), 384, SMEM, st>>>(maps, p);
   STB_LAUNCH_CHECK("attn_bwd_dkdv");
-  if (p.fuse_prep || old_dq) k2<<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM, st>>>(maps, p);
-  else n2<<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM_DQ, st>>>(maps, p);
+  k2<<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM, st>>>(maps, p);
   STB_LAUNCH_CHECK("attn_bwd_dq");
   return 0;
 }
@@ -344,45 +306,20 @@ int stb_gemm_bf16(const stb_gemm_args* a, void* stream) {
     return fail(STB_ERR_ARG, "aux must be 16-byte aligned, strides multiple of 8");
   if (a->epi < 0 || a->epi > 6) return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int bn = a->tile_bn, mt = a->tile_mt;
+  // every sm_90a tile is 128 rows (two 64-row consumer warpgroups); the row-tile request tile_mt is accepted and ignored
+  if (a->tile_mt < 0 || a->tile_mt > 3) return fail(STB_ERR_ARG, "unsupported tile config MT=%d", a->tile_mt);
+  int bn = a->tile_bn;
   if (bn == 0) {
     bn = a->N > 128 ? 256 : (a->N > 64 ? 128 : 64);
-    // skinny-M problems (conditioning / modulation GEMMs, M = batch): spread the weight stream over more SMs
+    // skinny-M problems (conditioning / modulation GEMMs, M = batch) and short grids: spread the weight stream over
+    // more SMs with narrower tiles while 256-wide tiles would leave SMs idle
     const long long t256 = (long long)((a->rows_per_batch + 127) / 128) * a->num_batches * ((a->N + 255) / 256);
     if (bn == 256 && t256 < num_sms()) bn = 128;
   }
-  if (mt == 0) {
-    // 256-row CTA tiles halve the per-FLOP L2->SMEM traffic; use them once there are >= 2 waves of them
-    // ... but the persistent grid pays for a partial last wave: pick the variant with the better wave fill
-    // (measured: both variants run the mainloop at about the same rate, profiles/r01).
-    auto fill = [&](int m) {
-      const long long t = (long long)((a->rows_per_batch + 128 * m - 1) / (128 * m)) * a->num_batches * ((a->N + bn - 1) / bn);
-      const long long waves = (t + num_sms() - 1) / num_sms();
-      return double(t) / double(waves * num_sms());
-    };
-    const long long t2 = (long long)((a->rows_per_batch + 255) / 256) * a->num_batches * ((a->N + bn - 1) / bn);
-    mt = (bn >= 128 && t2 >= 2ll * num_sms() && fill(2) >= 0.98 * fill(1)) ? 2 : 1;
-    // CTA-pair kernel (cta_group::2, one 256 x 256 tile per TPC): operand fetch per SM drops from 12 KB to 8 KB per
-    // k-step, which lifts the MMA rate from ~75 % to ~100 % of the tensor-pipe floor (profiles/r01/mma_probe.log);
-    // measured 1.49-1.57 PFLOP/s vs 1.28-1.41 for the single-CTA tiles.  Needs enough tiles to occupy every TPC.
-    if (bn == 256) {
-      const int clusters = num_sms() / 2;
-      const long long waves2 = (t2 + clusters - 1) / clusters;
-      const double fill_pair = double(t2) / double(waves2 * clusters);
-      // rows a 256-row pair tile actually uses, against the 128-row tiling (many short batches would leave one CTA of
-      // every pair idle)
-      const double u2 = double(a->rows_per_batch) / (256.0 * ((a->rows_per_batch + 255) / 256));
-      const double u1 = double(a->rows_per_batch) / (128.0 * ((a->rows_per_batch + 127) / 128));
-      if (t2 >= clusters && fill_pair >= 0.85 * std::max(fill(1), fill(2)) && u2 >= 0.85 * u1) mt = 3;
-    }
-  }
-  if (mt == 3 && bn == 256) return launch_gemm<1, 256, true>(a, st);   // CTA-pair (cta_group::2) 256 x 256 tile
-  if (mt == 1 && bn == 256) return launch_gemm<1, 256>(a, st);
-  if (mt == 2 && bn == 256) return launch_gemm<2, 256>(a, st);
-  if (mt == 1 && bn == 128) return launch_gemm<1, 128>(a, st);
-  if (mt == 2 && bn == 128) return launch_gemm<2, 128>(a, st);
-  if (mt == 1 && bn == 64) return launch_gemm<1, 64>(a, st);
-  return fail(STB_ERR_ARG, "unsupported tile config MT=%d BN=%d", mt, bn);
+  if (bn == 256) return launch_gemm<256>(a, st);
+  if (bn == 128) return launch_gemm<128>(a, st);
+  if (bn == 64) return launch_gemm<64>(a, st);
+  return fail(STB_ERR_ARG, "unsupported tile config BN=%d", bn);
 }
 
 int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
@@ -411,7 +348,7 @@ int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
   p.bias = static_cast<const __nv_bfloat16*>(a->bias);
   p.bias_h = a->bias_h; p.bias_q = a->bias_q;
   p.inv_scale = a->scale != 0.f ? 1.f / a->scale : 0.f;
-  dim3 grid((a->Sq + 255) / 256, a->H, a->B);
+  dim3 grid((a->Sq + 127) / 128, a->H, a->B);
   if (a->bias) {   // text-encoder instantiation (additive bias / mask); never taken by the training step
     if (a->scale == 0.f || a->bias_q < a->Sk) return fail(STB_ERR_ARG, "attn_fwd bias: scale must be non-zero and bias_q >= Sk");
     if (a->HD == 128) {
@@ -432,47 +369,6 @@ int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
       kernel<<<grid, 384, stb::AttnFwdCfg<64>::SMEM_BYTES, st>>>(maps, p);
     }
     STB_LAUNCH_CHECK("attn_fwd_bias");
-    return 0;
-  }
-  // opt-in (STB_ATTN_FWD_PAIR=1) until it has been measured faster inside the full step
-  static const bool use_pair = [] { const char* e = std::getenv("STB_ATTN_FWD_PAIR"); return e && e[0] == '1'; }();
-  if (a->HD == 128 && use_pair) {
-    // CTA-pair kernel (cta_group::2): Q in TMEM, K split by rows / V by columns across the two SMs of a TPC
-    stb::AttnFwdPairMaps pm;
-    {
-      unsigned long long d[4] = {(unsigned long long)a->HD, (unsigned long long)a->H, (unsigned long long)a->Sk, (unsigned long long)a->B};
-      unsigned long long sk[3] = {(unsigned long long)a->k_h * 2ull, (unsigned long long)a->k_s * 2ull, (unsigned long long)a->k_b * 2ull};
-      unsigned long long sv[3] = {(unsigned long long)a->v_h * 2ull, (unsigned long long)a->v_s * 2ull, (unsigned long long)a->v_b * 2ull};
-      unsigned bk[4] = {64, 1, 64, 1}, bv[4] = {64, 1, 128, 1};
-      if (int r = make_map(&pm.k64, a->k, 4, d, sk, bk)) return r;
-      if (int r = make_map(&pm.v128, a->v, 4, d, sv, bv)) return r;
-      unsigned long long dq[4] = {(unsigned long long)a->HD, (unsigned long long)a->H, (unsigned long long)a->Sq, (unsigned long long)a->B};
-      unsigned long long sq[3] = {(unsigned long long)a->q_h * 2ull, (unsigned long long)a->q_s * 2ull, (unsigned long long)a->q_b * 2ull};
-      if (int r = make_map(&pm.q128, a->q, 4, dq, sq, bv)) return r;
-    }
-    stb::AttnFwdPairParams pp;
-    pp.base = p;
-    auto kernel = stb::attn_fwd_pair_kernel;
-    static bool configured = false;
-    if (!configured) {
-      if (int r = set_smem(kernel, stb::AttnFwdPairCfg::SMEM_BYTES)) return r;
-      configured = true;
-    }
-    cudaLaunchConfig_t cfg;
-    std::memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3(2 * ((a->Sq + 255) / 256), a->H, a->B);
-    cfg.blockDim = dim3(384);
-    cfg.dynamicSmemBytes = stb::AttnFwdPairCfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    STB_CUDA(cudaLaunchKernelEx(&cfg, kernel, pm, pp));
-    g_launches.fetch_add(1);
     return 0;
   }
   if (a->HD == 128) {
@@ -683,6 +579,20 @@ int stb_flow_prep_pack(const void* latents, const void* noise, const float* sigm
   return 0;
 }
 
+// the loss kernels run as one fixed cluster (deterministic reduction, elementwise.cuh loss_cluster_store)
+static void loss_cluster_config(cudaLaunchConfig_t& cfg, cudaLaunchAttribute (&attr)[1], cudaStream_t st) {
+  std::memset(&cfg, 0, sizeof cfg);
+  cfg.gridDim = dim3(stb::LOSS_CTAS);
+  cfg.blockDim = dim3(stb::LOSS_THREADS);
+  cfg.stream = st;
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = stb::LOSS_CTAS;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+}
+
 static int check_loss_type(int loss_type, const float* huber_c) {
   if (loss_type < 0 || loss_type > 2) return fail(STB_ERR_ARG, "loss_type must be 0 (l2), 1 (huber) or 2 (smooth_l1)");
   if (loss_type != 0 && !huber_c) return fail(STB_ERR_ARG, "huber / smooth_l1 need the per-sample huber_c array");
@@ -696,11 +606,13 @@ int stb_flow_mse_loss(const void* pred_packed, const void* latents, const void* 
   if (int r = check_loss_type(loss_type, huber_c)) return r;
   if (layout < 0 || layout > 2) return fail(STB_ERR_ARG, "flow_mse_loss layout must be 0 (Flux), 1 (SD3) or 2 (NCHW)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  STB_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
-  const long long n = (long long)B * C * Hh * Ww;
-  const int grid = (int)std::min<long long>((n + 255) / 256, (long long)num_sms() * 8);
-  stb::flow_mse_loss_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(pred_packed), static_cast<const __nv_bfloat16*>(latents), static_cast<const __nv_bfloat16*>(noise), loss_out, static_cast<__nv_bfloat16*>(dpred_packed), grad_scale, B, C, Hh, Ww, layout, loss_type, huber_c);
-  STB_LAUNCH_CHECK("flow_mse_loss");
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  loss_cluster_config(cfg, attr, st);
+  STB_CUDA(cudaLaunchKernelEx(&cfg, stb::flow_mse_loss_kernel, static_cast<const __nv_bfloat16*>(pred_packed), static_cast<const __nv_bfloat16*>(latents),
+                              static_cast<const __nv_bfloat16*>(noise), loss_out, static_cast<__nv_bfloat16*>(dpred_packed), grad_scale, B, C, Hh,
+                              Ww, layout, loss_type, huber_c));
+  g_launches.fetch_add(1, std::memory_order_relaxed);
   return 0;
 }
 
@@ -725,11 +637,12 @@ int stb_target_mse_loss(const void* pred_packed, const void* target, const float
   if (layout < 0 || layout > 2) return fail(STB_ERR_ARG, "target_mse_loss layout must be 0 (c,dy,dx), 1 (dy,dx,c) or 2 (NCHW)");
   if (layout != 2 && ((Hh & 1) || (Ww & 1))) return fail(STB_ERR_ARG, "latent H and W must be even for 2x2 patchify");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  STB_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
-  const long long n = (long long)B * C * Hh * Ww;
-  const int grid = (int)std::min<long long>((n + 255) / 256, (long long)num_sms() * 8);
-  stb::target_mse_loss_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(pred_packed), static_cast<const __nv_bfloat16*>(target), weights, loss_out, static_cast<__nv_bfloat16*>(dpred_packed), grad_scale, B, C, Hh, Ww, layout, loss_type, huber_c);
-  STB_LAUNCH_CHECK("target_mse_loss");
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  loss_cluster_config(cfg, attr, st);
+  STB_CUDA(cudaLaunchKernelEx(&cfg, stb::target_mse_loss_kernel, static_cast<const __nv_bfloat16*>(pred_packed), static_cast<const __nv_bfloat16*>(target),
+                              weights, loss_out, static_cast<__nv_bfloat16*>(dpred_packed), grad_scale, B, C, Hh, Ww, layout, loss_type, huber_c));
+  g_launches.fetch_add(1, std::memory_order_relaxed);
   return 0;
 }
 
@@ -846,7 +759,7 @@ int stb_dropout_expand(const void* x, long long x_b, long long x_s, void* out, i
   if (int r = dropout_args(x, out, members, B, S, K, p)) return r;
   if ((x_b & 7) || (x_s & 7)) return fail(STB_ERR_ARG, "dropout_expand: strides must be multiples of 8 elements");
   const long long total = (long long)B * S * (K >> 3);
-  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)num_sms() * 16);
   const uint32_t thresh = (uint32_t)std::llround(double(p) * 16777216.0);
   stb::dropout_expand_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(x), x_b, x_s, static_cast<__nv_bfloat16*>(out), members, B, S, K, 1.f / (1.f - p), thresh, seed, stream0);
@@ -860,7 +773,7 @@ int stb_dropout_accum(const void* d, void* dx, long long dx_b, long long dx_s, i
   if (int r = dropout_args(d, dx, members, B, S, K, p)) return r;
   if ((dx_b & 7) || (dx_s & 7)) return fail(STB_ERR_ARG, "dropout_accum: strides must be multiples of 8 elements");
   const long long total = (long long)B * S * (K >> 3);
-  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, 148LL * 16);
+  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)num_sms() * 16);
   const uint32_t thresh = (uint32_t)std::llround(double(p) * 16777216.0);
   stb::dropout_accum_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(d), static_cast<__nv_bfloat16*>(dx), dx_b, dx_s, members, B, S, K, 1.f / (1.f - p), thresh, seed, stream0);
@@ -902,14 +815,14 @@ int stb_wgrad_full(const void* dy, long long dy_b, long long dy_s, const void* x
     static bool configured = false;
     if (!configured) { if (int r = set_smem(kern, SMEM)) return r; configured = true; }
     const int tiles = tiles_n * ((K + 255) / 256);
-    kern<<<std::min(tiles, sms), 256, SMEM, st>>>(maps, p);
+    kern<<<std::min(tiles, sms), 384, SMEM, st>>>(maps, p);
   } else {
     auto kern = stb::wgrad_full_kernel<128>;
     constexpr int SMEM = stb::WgradFullCfg<128>::SMEM_BYTES;
     static bool configured = false;
     if (!configured) { if (int r = set_smem(kern, SMEM)) return r; configured = true; }
     const int tiles = tiles_n * ((K + 127) / 128);
-    kern<<<std::min(tiles, sms), 256, SMEM, st>>>(maps, p);
+    kern<<<std::min(tiles, sms), 384, SMEM, st>>>(maps, p);
   }
   STB_LAUNCH_CHECK("wgrad_full");
   return 0;
@@ -924,7 +837,7 @@ int stb_colsum2(const void* dy, long long dy_b, long long dy_s, const void* z, l
     return fail(STB_ERR_ARG, "colsum2: operands must be 16-byte aligned with strides multiple of 8");
   const int vecs = D >> 3;
   const int gx = (vecs + 255) / 256;
-  int rows = std::max(8, (int)(((long long)S * B * gx + 148LL * 8 - 1) / (148LL * 8)));
+  int rows = std::max(8, (int)(((long long)S * B * gx + (long long)num_sms() * 8 - 1) / ((long long)num_sms() * 8)));
   dim3 grid(gx, (S + rows - 1) / rows, B);
   stb::colsum2_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(dy), dy_b, dy_s, static_cast<const __nv_bfloat16*>(z), z_b, z_s, sum, dot, B, S, D, rows);
@@ -987,29 +900,23 @@ int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm
     p.rows_per_split = rows;
     p.splits_per_batch = spb;
     dim3 grid(n_tiles, spb * B);
-    const int rp = (R + 15) / 16 * 16;
-#define STB_WG(RPV)                                                          \
-  {                                                                          \
-    auto kern = stb::wgrad_tn_kernel<RPV>;                                   \
-    constexpr int SMEM = stb::WgradCfg<RPV>::SMEM_BYTES;                     \
-    static bool configured = false;                                          \
-    if (!configured) {                                                       \
-      if (int r = set_smem(kern, SMEM)) return r;                            \
-      configured = true;                                                     \
-    }                                                                        \
-    kern<<<grid, 256, SMEM, st>>>(maps, p);                                  \
-  }
-    switch (rp) {
-      case 16: STB_WG(16) break;
-      case 32: STB_WG(32) break;
-      case 48: STB_WG(48) break;
-      case 64: STB_WG(64) break;
-      case 80: STB_WG(80) break;
-      case 96: STB_WG(96) break;
-      case 112: STB_WG(112) break;
-      default: STB_WG(128) break;
+    if (R <= 64) {
+      auto kern = stb::wgrad_tn_kernel<64>;
+      static bool configured = false;
+      if (!configured) {
+        if (int r = set_smem(kern, stb::WgradCfg<64>::SMEM_BYTES)) return r;
+        configured = true;
+      }
+      kern<<<grid, 384, stb::WgradCfg<64>::SMEM_BYTES, st>>>(maps, p);
+    } else {
+      auto kern = stb::wgrad_tn_kernel<128>;
+      static bool configured = false;
+      if (!configured) {
+        if (int r = set_smem(kern, stb::WgradCfg<128>::SMEM_BYTES)) return r;
+        configured = true;
+      }
+      kern<<<grid, 384, stb::WgradCfg<128>::SMEM_BYTES, st>>>(maps, p);
     }
-#undef STB_WG
     STB_LAUNCH_CHECK("wgrad_tn");
     if (workspace) {
       const long long n = (long long)R * N;
@@ -1043,10 +950,10 @@ int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm
 }  // extern "C"
 
 // ---------------------------------------------------------------- VAE latent encode
-template <int BN, bool PAIR = false>
+template <int BN>
 static int launch_conv3x3(const void* x, const void* w, const void* bias, const void* res, void* out, int B, int H,
                           int W, int C_in, int C_out, int stride, cudaStream_t st) {
-  using Cfg = typename std::conditional<PAIR, stb::GemmPairCfg<BN>, stb::GemmCfg<1, BN>>::type;
+  using Cfg = stb::GemmCfg<BN>;
   const int H_out = stride == 1 ? H : H / 2, W_out = stride == 1 ? W : W / 2;
   stb::GemmMaps maps;
   std::memset(&maps, 0, sizeof maps);
@@ -1061,18 +968,16 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   {
     unsigned long long d[2] = {(unsigned long long)9 * C_in, (unsigned long long)C_out};
     unsigned long long sb[1] = {(unsigned long long)9 * C_in * 2ull};
-    unsigned bx[2] = {64, (unsigned)(PAIR ? BN / 2 : BN)};
+    unsigned bx[2] = {64, (unsigned)BN};
     if (int r = make_map(&maps.w[0], w, 2, d, sb, bx)) return r;
   }
   stb::GemmParams p;
   std::memset(&p, 0, sizeof p);
-  p.conv_pair_rows = W_out > 128 ? 1 : 2;
   p.rows_per_batch = W_out;
   p.num_batches = B * H_out;
   p.N = C_out;
   p.nseg = 1;
   p.kblocks[0] = 9 * (C_in / 64);
-  p.kmmas_last[0] = 4;
   p.epi = res ? stb::EPI_ADD_RES : stb::EPI_STORE;
   p.D = static_cast<__nv_bfloat16*>(out);
   p.d_batch_stride = (long long)W_out * C_out;
@@ -1085,39 +990,17 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   p.conv_stride = stride;
   p.conv_pad = stride == 1 ? 1 : 0;
   p.conv_cblocks = C_in / 64;
-  auto kernel = stb::gemm_bf16_tn_kernel<1, BN, true, PAIR>;
+  auto kernel = stb::gemm_bf16_tn_kernel<BN, true>;
   static bool configured = false;
   if (!configured) {
     if (int r = set_smem(kernel, Cfg::SMEM_BYTES)) return r;
     configured = true;
   }
-  if constexpr (PAIR) {
-    const long long tiles_m = p.conv_pair_rows == 2 ? (p.num_batches + 1) / 2 : (long long)((W_out + 255) / 256) * p.num_batches;
-    const long long tiles = tiles_m * ((C_out + BN - 1) / BN);
-    const int clusters = (int)std::min<long long>(tiles, num_sms() / 2);
-    cudaLaunchConfig_t cfg;
-    std::memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3(2 * clusters);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    STB_CUDA(cudaLaunchKernelEx(&cfg, kernel, maps, p));
-    g_launches.fetch_add(1);
-    return 0;
-  } else {
-    const long long tiles = (long long)((W_out + 127) / 128) * p.num_batches * ((C_out + BN - 1) / BN);
-    const int grid = (int)std::min<long long>(tiles, num_sms());
-    kernel<<<grid, 256, Cfg::SMEM_BYTES, st>>>(maps, p);
-    STB_LAUNCH_CHECK("conv3x3_nhwc");
-    return 0;
-  }
+  const long long tiles = (long long)((W_out + 127) / 128) * p.num_batches * ((C_out + BN - 1) / BN);
+  const int grid = (int)std::min<long long>(tiles, num_sms());
+  kernel<<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
+  STB_LAUNCH_CHECK("conv3x3_nhwc");
+  return 0;
 }
 
 extern "C" {
@@ -1131,17 +1014,6 @@ int stb_conv3x3_nhwc(const void* x, const void* w, const void* bias, const void*
   if (!aligned16(x) || !aligned16(w) || !aligned16(out) || (res && !aligned16(res)) || (bias && !aligned16(bias)))
     return fail(STB_ERR_ARG, "conv3x3_nhwc alignment");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  {
-    // CTA-pair implicit GEMM (two half-rows or two rows of output pixels per TPC) once there is a tile per TPC
-    const int H_out = stride == 1 ? H : H / 2, W_out = stride == 1 ? W : W / 2;
-    const long long rows = (long long)B * H_out;
-    const long long tiles_m = W_out > 128 ? (long long)((W_out + 255) / 256) * rows : (rows + 1) / 2;
-    static const bool no_pair = [] { const char* e = std::getenv("STB_CONV_PAIR"); return e && e[0] == '0'; }();
-    if (!no_pair && C_out >= 128 && (C_out % 16) == 0 && tiles_m * ((C_out + 255) / 256) >= num_sms() / 2) {
-      if (C_out > 128) return launch_conv3x3<256, true>(x, w, bias, res, out, B, H, W, C_in, C_out, stride, st);
-      return launch_conv3x3<128, true>(x, w, bias, res, out, B, H, W, C_in, C_out, stride, st);
-    }
-  }
   if (C_out > 128) return launch_conv3x3<256>(x, w, bias, res, out, B, H, W, C_in, C_out, stride, st);
   if (C_out > 64) return launch_conv3x3<128>(x, w, bias, res, out, B, H, W, C_in, C_out, stride, st);
   return launch_conv3x3<64>(x, w, bias, res, out, B, H, W, C_in, C_out, stride, st);
@@ -1152,20 +1024,25 @@ int stb_conv_in_3ch(const void* pixels, const void* w, const void* bias, void* o
   if (int r = check_device()) return r;
   if (C % 8 || C > 512) return fail(STB_ERR_ARG, "conv_in_3ch: C must be a multiple of 8, <= 512");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static const bool no_mma = [] { const char* e = std::getenv("STB_CONV_IN_MMA"); return e && e[0] == '0'; }();
-  if (!no_mma && C % 16 == 0 && C <= 256 && aligned16(bias) && aligned16(out)) {
+  if ((C == 64 || C == 128 || C == 256) && aligned16(bias) && aligned16(out)) {
     // tensor-core path: im2col tiles built in shared memory, K = 27 padded to 32
-    auto kernel = stb::conv_in_3ch_mma_kernel;
-    constexpr int SMEM = 65536 + 64 + 1024;
+    constexpr int SMEM = 32768 + 16384 + 1024;
+    const long long tiles = (long long)B * H * ((W + 127) / 128);
+    const int grid = (int)std::min<long long>(tiles, 2LL * num_sms());
+    auto px = static_cast<const __nv_bfloat16*>(pixels);
+    auto wt = static_cast<const __nv_bfloat16*>(w);
+    auto bs = static_cast<const __nv_bfloat16*>(bias);
+    auto o = static_cast<__nv_bfloat16*>(out);
     static bool configured = false;
     if (!configured) {
-      if (int r = set_smem(kernel, SMEM)) return r;
+      if (int r = set_smem(stb::conv_in_3ch_mma_kernel<256>, SMEM)) return r;
+      if (int r = set_smem(stb::conv_in_3ch_mma_kernel<128>, SMEM)) return r;
+      if (int r = set_smem(stb::conv_in_3ch_mma_kernel<64>, SMEM)) return r;
       configured = true;
     }
-    const long long tiles = (long long)B * H * ((W + 127) / 128);
-    const int grid = (int)std::min<long long>(tiles, num_sms());
-    kernel<<<grid, 192, SMEM, st>>>(static_cast<const __nv_bfloat16*>(pixels), static_cast<const __nv_bfloat16*>(w),
-                                    static_cast<const __nv_bfloat16*>(bias), static_cast<__nv_bfloat16*>(out), B, H, W, C);
+    if (C == 256) stb::conv_in_3ch_mma_kernel<256><<<grid, 256, SMEM, st>>>(px, wt, bs, o, B, H, W);
+    else if (C == 128) stb::conv_in_3ch_mma_kernel<128><<<grid, 256, SMEM, st>>>(px, wt, bs, o, B, H, W);
+    else stb::conv_in_3ch_mma_kernel<64><<<grid, 256, SMEM, st>>>(px, wt, bs, o, B, H, W);
     STB_LAUNCH_CHECK("conv_in_3ch_mma");
     return 0;
   }

@@ -1,34 +1,23 @@
-// simpletuner_b200 — attention backward on tcgen05, sm_100a (autograd of the SDPA call at reference
+// simpletuner_b200 — attention backward on wgmma, sm_90a (autograd of the SDPA call at reference
 // flux/transformer.py:200-207).
 //
 //   P = exp(S*scale - LSE),  dV = P^T dO,  dP = dO V^T,  dS = P o (dP - Delta) * scale,
 //   dQ = dS K,  dK = dS^T Q,   Delta_i = sum_d dO_id O_id
 //
-// Two deterministic kernels, no atomics:
-//   attn_bwd_dkdv_kernel : one CTA per (b, h, 128-key tile); streams 64-row query tiles.  Transposed
-//       domain (TMEM lane = key): S^T = K Q^T, dP^T = V dO^T; P^T and dS^T are written back to TMEM as
-//       bf16 and fed as the A operand of  dV += P^T dO,  dK += dS^T Q  (dO / Q tiles re-read from the
-//       same smem bytes through MN-major descriptors).
-//   attn_bwd_dq_kernel   : one CTA per (b, h, 128-row query tile); streams 64-key tiles (lane = query
-//       row): S = Q K^T, dP = dO V^T, dS -> TMEM bf16, dQ += dS K.
-//       Q and dO (the resident operands) live in TMEM as bf16 pairs — staged once by the compute warps — and feed
-//       the score MMAs in TS form: 2 KB instead of 6 KB of shared-memory operand fetch per MMA.
-// Both use 64-wide streamed tiles so that the score buffers are DOUBLE-BUFFERED in TMEM
-// (2 x 64 S + 2 x 64 dP + accumulators [+ Q / dO in dq] = 512 columns): while the compute warps turn tile i into
-// P / dS the tensor pipe already works on tile i+1's S / dP.  Both compute warpgroups work on every tile (warpgroup
-// w owns 32 of its 64 columns and packs its bf16 result into the first 16 columns of its own range, PK_COL).
-// What bounds them is the MMA path itself (SS / TS N = 64 instruction rates, tools/probe/mma_probe.cu), not the
-// exp / dS math: see DESIGN.md 3.3.
-// warps 0-3 / 4-7 = compute warpgroups, warp 8 = TMA producer, warp 9 = MMA issuer, warp 10 = TMEM alloc.
+// Two deterministic kernels, no atomics; 384 threads each: warpgroup 0 is the TMA producer, warpgroups 1 and 2
+// own 64 rows each of the CTA's 128 resident rows.
+//   attn_bwd_dkdv_kernel : one CTA per (b, h, 128-key tile); streams 64-row query tiles.  Transposed domain
+//       (accumulator row = key): S^T = K Q^T, dP^T = V dO^T in registers; P^T and dS^T become the register A operand of
+//       dV += P^T dO,  dK += dS^T Q  (dO / Q tiles re-read from the same shared-memory bytes as MN-major operands).
+//   attn_bwd_dq_kernel   : one CTA per (b, h, 128-row query tile); streams 64-key tiles: S = Q K^T, dP = dO V^T,
+//       dS in registers, dQ += dS K.
+// The accumulators are staged through shared memory (fp32) for the store, so that one thread handles contiguous
+// columns of a row — the fused q / k pre-processing backward (qk_prep) needs whole-row sums.
 #pragma once
 #include "../../include/stb200.h"
+#include "attn_fwd.cuh"
 #include "common.cuh"
 #include "elementwise.cuh"
-
-// timing experiments only (never defined in the shipped build): 1 = skip the exp / dS math, 2 = also skip the TMEM traffic
-#ifndef STB_ATTN_DEBUG_SKIP
-#define STB_ATTN_DEBUG_SKIP 0
-#endif
 
 namespace stb {
 
@@ -39,7 +28,7 @@ struct AttnBwdParams {
   const float* delta;  // [B, H, Sq]
   __nv_bfloat16 *dq, *dk, *dv;
   long long dq_b, dq_s, dq_h, dk_b, dk_s, dk_h, dv_b, dv_s, dv_h;
-  // raw views of the operands the dq kernel stages into TMEM itself (everything else goes through the TMA maps)
+  // raw views of q / dO (the operands themselves go through the TMA maps)
   const __nv_bfloat16 *q, *d_o;
   long long q_b, q_s, q_h, do_b, do_s, do_h;
   // optional fused backward of the q / k pre-processing (per-head RMSNorm -> RoPE, qk_rmsnorm_rope_fwd_kernel):
@@ -55,16 +44,8 @@ struct AttnBwdParams {
 };
 
 struct AttnBwdMaps {
-  // 4-D (d, h, s, b) SWIZZLE_128B; box (64, 1, 128, 1) for the resident operand, (64, 1, 64, 1) for the streamed one
+  // 4-D (d, h, s, b) SWIZZLE_128B; box (64, 1, 128, 1) for the resident operands, (64, 1, 64, 1) for the streamed ones
   CUtensorMap q128, k128, v128, do128, q64, k64, v64, do64;
-};
-
-template <int HD>
-struct AttnBwdCfg {
-  static constexpr int BIG = 128 * HD * 2;   // resident 128-row tile
-  static constexpr int SMALL = 64 * HD * 2;  // streamed 64-row tile
-  static constexpr int STAGES = 3;
-  static constexpr int SMEM_BYTES = 2 * BIG + STAGES * 2 * SMALL + 2 * 2 * 128 * 4 + 1024 + 256;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -93,360 +74,243 @@ attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ o, long long o_b, long l
   if (lane == 0) delta[((long long)b * H + h) * S + s] = acc;
 }
 
+template <int HD>
+struct AttnBwdCfg {
+  static constexpr int BIG = 128 * HD * 2;   // resident 128-row tile
+  static constexpr int SMALL = 64 * HD * 2;  // streamed 64-row tile
+  static constexpr int STAGES = 2;
+  static constexpr int SMEM_BYTES = 2 * BIG + STAGES * 2 * SMALL + 1024 + 256;
+};
+
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// store 128 x HD fp32 accumulator rows (this thread's TMEM lane) as bf16 to a global row
+// fp32 accumulator (64 x HD, wgmma layout) of this warpgroup -> shared-memory rows [64][HD + 4] (multiplied by `mul`)
 template <int HD>
-__device__ __forceinline__ void store_acc_row(uint32_t taddr, __nv_bfloat16* grow, bool row_ok, float mul = 1.f) {
-#pragma unroll 1
-  for (int c = 0; c < HD; c += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(taddr + c, v);
-    tc_wait_ld();
-    if (row_ok) {
-      uint4* dp = reinterpret_cast<uint4*>(grow + c);
+__device__ __forceinline__ void stage_acc(float* rows, const float (&acc)[HD / 2], float mul) {
+  const int t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(v[q * 8 + 0]) * mul, __uint_as_float(v[q * 8 + 1]) * mul);
-        u.y = pack_bf16x2(__uint_as_float(v[q * 8 + 2]) * mul, __uint_as_float(v[q * 8 + 3]) * mul);
-        u.z = pack_bf16x2(__uint_as_float(v[q * 8 + 4]) * mul, __uint_as_float(v[q * 8 + 5]) * mul);
-        u.w = pack_bf16x2(__uint_as_float(v[q * 8 + 6]) * mul, __uint_as_float(v[q * 8 + 7]) * mul);
-        dp[q] = u;
+  for (int i = 0; i < HD / 8; ++i)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float* r = rows + (wq * 16 + (lane >> 2) + 8 * hh) * (HD + 4) + 8 * i + 2 * (lane & 3);
+      r[0] = acc[4 * i + 2 * hh] * mul;
+      r[1] = acc[4 * i + 2 * hh + 1] * mul;
+    }
+}
+
+// One staged row (fp32, already multiplied by the softmax scale) -> bf16 global row.  Two threads per row, HD / 2
+// columns each (thread pair = lanes 2k, 2k+1).  With `prep`, the row is the gradient w.r.t. the post-RoPE q or k and
+// is taken back through RoPE and the per-head RMSNorm (same math as qk_rmsnorm_rope_bwd_kernel):
+//   dy = R^T go;  g = dy * w;  dx = rstd * (g - xhat * mean(g * xhat)),  xhat = x * rstd
+template <int HD>
+__device__ __forceinline__ void store_row_half(const float* row, int half, __nv_bfloat16* grow, bool row_ok, bool prep,
+                                               const __nv_bfloat16* xrow, const __nv_bfloat16* w, const float* cs,
+                                               const float* sn, float eps) {
+  constexpr int NC = HD / 2;
+  const int c0 = half * NC;
+  if (!prep) {
+    if (row_ok) {
+#pragma unroll
+      for (int c = 0; c < NC; c += 8) {
+        float o[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) o[i] = row[c0 + c + i];
+        *reinterpret_cast<uint4*>(grow + c0 + c) = pack8(o);
       }
+    }
+    return;
+  }
+  float ss = 0.f, sgx = 0.f;
+  float g[NC];
+#pragma unroll
+  for (int c = 0; c < NC; c += 8) {
+    float x[8], wv[8];
+    unpack8(row_ok ? __ldg(reinterpret_cast<const uint4*>(xrow + c0 + c)) : make_uint4(0u, 0u, 0u, 0u), x);
+    if (w) unpack8(__ldg(reinterpret_cast<const uint4*>(w + c0 + c)), wv);
+#pragma unroll
+    for (int i = 0; i < 8; i += 2) {
+      const int j = c0 + c + i;
+      const float go0 = row[j], go1 = row[j + 1];
+      float dy0 = go0, dy1 = go1;
+      if (cs && row_ok) {
+        const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + j));
+        const float2 s2 = __ldg(reinterpret_cast<const float2*>(sn + j));
+        // o[i] = y[i] c[i] - y[i+1] s[i];  o[i+1] = y[i+1] c[i+1] + y[i] s[i+1]
+        dy0 = go0 * c2.x + go1 * s2.y;
+        dy1 = go1 * c2.y - go0 * s2.x;
+      }
+      const float g0 = w ? dy0 * wv[i] : dy0, g1 = w ? dy1 * wv[i + 1] : dy1;
+      ss += x[i] * x[i] + x[i + 1] * x[i + 1];
+      sgx += g0 * x[i] + g1 * x[i + 1];
+      g[c + i] = g0;
+      g[c + i + 1] = g1;
+    }
+  }
+  ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+  sgx += __shfl_xor_sync(0xffffffffu, sgx, 1);
+  const float rstd = rsqrtf(ss / HD + eps);
+  const float m = sgx * rstd / HD;
+  if (row_ok) {
+#pragma unroll
+    for (int c = 0; c < NC; c += 8) {
+      float x[8], o[8];
+      unpack8(__ldg(reinterpret_cast<const uint4*>(xrow + c0 + c)), x);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) o[i] = rstd * (g[c + i] - (x[i] * rstd) * m);
+      *reinterpret_cast<uint4*>(grow + c0 + c) = pack8(o);
     }
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Fused epilogue: backward of RoPE(RMSNorm(x) * w) for one (token, head) row held in this thread's TMEM lane.
-//   go = acc * scale (gradient w.r.t. the post-RoPE q or k);  dy = R^T go;  g = dy * w;
-//   dx = rstd * (g - xhat * mean(g * xhat)),  xhat = x * rstd        (same math as qk_rmsnorm_rope_bwd_kernel)
-// pass 1 turns the accumulator columns [0, NC) at `taddr` into g in place and returns the partial sums;
-// pass 2 reads g back and writes dx (bf16).  x / w / cos / sin pointers are already offset to the first column.
-// ------------------------------------------------------------------------------------------------
-template <int NC>
-__device__ __forceinline__ void qk_grad_pass1(uint32_t taddr, float scale, bool row_ok, const __nv_bfloat16* xrow,
-                                              const __nv_bfloat16* w, const float* cs, const float* sn, float& ss,
-                                              float& sgx) {
-#pragma unroll 1
-  for (int c = 0; c < NC; c += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(taddr + c, v);
-    tc_wait_ld();
+template <int HD>
+__device__ __forceinline__ void mma_kmajor_n64(float (&d)[32], uint32_t a_tile, uint32_t a_atom, uint32_t b_tile, uint32_t b_atom) {
+  // d (64 x 64) = A (64 rows, K = HD, K-major boxes a_atom bytes apart) . B (64 rows, K-major boxes b_atom apart)^T
 #pragma unroll
-    for (int q4 = 0; q4 < 4; ++q4) {   // 8 columns at a time
-      float x[8], wv[8];
-      const uint4 ux = row_ok ? __ldg(reinterpret_cast<const uint4*>(xrow + c) + q4) : make_uint4(0u, 0u, 0u, 0u);
-      unpack8(ux, x);
-      if (w) unpack8(__ldg(reinterpret_cast<const uint4*>(w + c) + q4), wv);
-#pragma unroll
-      for (int i = 0; i < 8; i += 2) {
-        const int j = q4 * 8 + i;
-        const float go0 = __uint_as_float(v[j]) * scale, go1 = __uint_as_float(v[j + 1]) * scale;
-        float dy0 = go0, dy1 = go1;
-        if (cs && row_ok) {
-          const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + c + j));
-          const float2 s2 = __ldg(reinterpret_cast<const float2*>(sn + c + j));
-          // o[i] = y[i] c[i] - y[i+1] s[i];  o[i+1] = y[i+1] c[i+1] + y[i] s[i+1]
-          dy0 = go0 * c2.x + go1 * s2.y;
-          dy1 = go1 * c2.y - go0 * s2.x;
-        }
-        const float g0 = w ? dy0 * wv[i] : dy0, g1 = w ? dy1 * wv[i + 1] : dy1;
-        ss += x[i] * x[i] + x[i + 1] * x[i + 1];
-        sgx += g0 * x[i] + g1 * x[i + 1];
-        v[j] = __float_as_uint(g0);
-        v[j + 1] = __float_as_uint(g1);
-      }
-    }
-    tmem_st_32x32b_x32(taddr + c, v);
-  }
-  tc_wait_st();
-}
-
-template <int NC>
-__device__ __forceinline__ void qk_grad_pass2(uint32_t taddr, bool row_ok, const __nv_bfloat16* xrow, float rstd, float m,
-                                              __nv_bfloat16* orow) {
-#pragma unroll 1
-  for (int c = 0; c < NC; c += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(taddr + c, v);
-    tc_wait_ld();
-    if (row_ok) {
-#pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4) {
-        float x[8], o[8];
-        unpack8(__ldg(reinterpret_cast<const uint4*>(xrow + c) + q4), x);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = rstd * (__uint_as_float(v[q4 * 8 + i]) - (x[i] * rstd) * m);
-        reinterpret_cast<uint4*>(orow + c)[q4] = pack8(o);
-      }
-    }
-  }
+  for (int kk = 0; kk < HD / 16; ++kk)
+    wgmma_ss_n64<0, 0>(d, sdesc_k(a_tile, (kk / 4) * a_atom + (kk % 4) * 32), sdesc_k(b_tile, (kk / 4) * b_atom + (kk % 4) * 32),
+                       kk > 0 ? 1u : 0u);
 }
 
 // ------------------------------------------------------------------------------------------------
 // dK / dV
 // ------------------------------------------------------------------------------------------------
-// TMEM column (relative to the score buffer) of the packed bf16 operand chunk kk (16 of the 64 streamed rows):
-// chunks 0-1 are written by compute warpgroup 0 at columns 0-15, chunks 2-3 by warpgroup 1 at columns 32-47.
-#define PK_COL(kk) (uint32_t((kk) < 2 ? 8 * (kk) : 32 + 8 * ((kk) - 2)))
-
 template <int HD>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams p) {
   using Cfg = AttnBwdCfg<HD>;
   constexpr int ATOMS = HD / 64;
-  constexpr int BIG = Cfg::BIG, SMALL = Cfg::SMALL, NSTG = Cfg::STAGES;
-  constexpr int ATOM128 = 128 * 64 * 2;  // [128 rows x 64] box
-  constexpr int ATOM64 = 64 * 64 * 2;    // [64 rows x 64] box
-
+  constexpr int BIG_ATOM = 128 * 128, SMALL_ATOM = 64 * 128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t k_smem = smem_base;
-  const uint32_t v_smem = k_smem + BIG;
-  auto q_smem = [&](int s) { return v_smem + BIG + uint32_t(s) * 2 * SMALL; };
-  auto do_smem = [&](int s) { return q_smem(s) + SMALL; };
-  const uint32_t stat_smem = smem_base + 2 * BIG + NSTG * 2 * SMALL;  // [wg][stage 0/1][lse 64 | delta 64]
-  const uint32_t bar_base = stat_smem + 2 * 2 * 128 * 4;
+  const uint32_t k_smem = smem_base, v_smem = smem_base + Cfg::BIG;
+  const uint32_t q_smem = smem_base + 2 * Cfg::BIG;                      // STAGES streamed Q tiles
+  const uint32_t do_smem = q_smem + Cfg::STAGES * Cfg::SMALL;            // STAGES streamed dO tiles
+  const uint32_t bar_base = do_smem + Cfg::STAGES * Cfg::SMALL;
   const uint32_t kv_full = bar_base;
-  auto qdo_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto qdo_empty = [&](int s) { return bar_base + 8u * (4 + s); };
-  auto st_full = [&](int w) { return bar_base + 8u * (7 + w); };
-  auto dpt_full = [&](int w) { return bar_base + 8u * (9 + w); };
-  auto p_full = [&](int w) { return bar_base + 8u * (11 + w); };
-  auto ds_full = [&](int w) { return bar_base + 8u * (13 + w); };
-  const uint32_t acc_done = bar_base + 8u * 15;
-  const uint32_t tmem_slot = bar_base + 8u * 16;
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  float* stat_ptr = reinterpret_cast<float*>(smem_raw + (stat_smem - smem_u32(smem_raw)));
+  auto s_full = [&](int s) { return bar_base + 8u * (1 + s); };
+  auto s_empty = [&](int s) { return bar_base + 8u * (1 + Cfg::STAGES + s); };
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int kv0 = blockIdx.x * 128;
-  const int h = blockIdx.y;
-  const int b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
+  const int kv0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
   const int n_q = (p.Sq + 63) / 64;
 
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&maps.q64);
-    tma_prefetch_desc(&maps.k128);
-    tma_prefetch_desc(&maps.v128);
-    tma_prefetch_desc(&maps.do64);
-  }
-  if (warp == 9 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
-    for (int s = 0; s < NSTG; ++s) {
-      mbar_init(qdo_full(s), 1);
-      mbar_init(qdo_empty(s), 1);
+    for (int s = 0; s < Cfg::STAGES; ++s) {
+      mbar_init(s_full(s), 1);
+      mbar_init(s_empty(s), 8);
     }
-    for (int w = 0; w < 2; ++w) {
-      mbar_init(st_full(w), 1);
-      mbar_init(dpt_full(w), 1);
-      mbar_init(p_full(w), 256);   // both compute warpgroups contribute half the columns of every tile
-      mbar_init(ds_full(w), 128);
-    }
-    mbar_init(acc_done, 1);
     fence_mbar_init();
   }
-  if (warp == 10) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  auto X = [&](int w) { return tmem_base + uint32_t(w) * 64; };        // S^T  (P^T packed in place)
-  auto Y = [&](int w) { return tmem_base + 128 + uint32_t(w) * 64; };  // dP^T (dS^T packed in place)
-  const uint32_t DV = tmem_base + 256;
-  const uint32_t DK = tmem_base + 384;
 
-  // producer / MMA warps: warp-uniform loops, issuing instructions executed by one elected lane
-  if (warp == 8) {
-    if (elect_one()) {
-      mbar_arrive_expect_tx(kv_full, 2 * BIG);
-      for (int a = 0; a < ATOMS; ++a) {
-        tma_load_4d(k_smem + a * ATOM128, &maps.k128, kv_full, a * 64, h, kv0, b);
-        tma_load_4d(v_smem + a * ATOM128, &maps.v128, kv_full, a * 64, h, kv0, b);
-      }
-    }
-    __syncwarp();
-    int stg = 0;
-    uint32_t ph = 0;
-    for (int i = 0; i < n_q; ++i) {
-      mbar_wait(qdo_empty(stg), ph ^ 1u, 40);
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (warp == 0) {
       if (elect_one()) {
-        mbar_arrive_expect_tx(qdo_full(stg), 2 * SMALL);
+        mbar_arrive_expect_tx(kv_full, 2 * Cfg::BIG);
         for (int a = 0; a < ATOMS; ++a) {
-          tma_load_4d(q_smem(stg) + a * ATOM64, &maps.q64, qdo_full(stg), a * 64, h, i * 64, b);
-          tma_load_4d(do_smem(stg) + a * ATOM64, &maps.do64, qdo_full(stg), a * 64, h, i * 64, b);
+          tma_load_4d(k_smem + a * BIG_ATOM, &maps.k128, kv_full, a * 64, h, kv0, b);
+          tma_load_4d(v_smem + a * BIG_ATOM, &maps.v128, kv_full, a * 64, h, kv0, b);
         }
       }
       __syncwarp();
-      if (++stg == NSTG) {
-        stg = 0;
-        ph ^= 1u;
-      }
-    }
-  } else if (warp == 9) {
-    constexpr uint32_t idesc_st = make_idesc_bf16(128, 64, 0, 0);   // [kv x q64] = K-major x K-major
-    constexpr uint32_t idesc_acc = make_idesc_bf16(128, HD, 0, 1);  // [kv x d]   = TMEM x MN-major
-    auto issue_scores = [&](int w, int stg) {
-#pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-        const uint64_t ad = sdesc_k(k_smem, (kk / 4) * ATOM128 + (kk % 4) * 32);
-        const uint64_t bd = sdesc_k(q_smem(stg), (kk / 4) * ATOM64 + (kk % 4) * 32);
-        mma_ss(X(w), ad, bd, idesc_st, kk > 0);
-      }
-      tc_commit(st_full(w));
-#pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-        const uint64_t ad = sdesc_k(v_smem, (kk / 4) * ATOM128 + (kk % 4) * 32);
-        const uint64_t bd = sdesc_k(do_smem(stg), (kk / 4) * ATOM64 + (kk % 4) * 32);
-        mma_ss(Y(w), ad, bd, idesc_st, kk > 0);
-      }
-      tc_commit(dpt_full(w));
-    };
-    mbar_wait(kv_full, 0, 41);
-    mbar_wait(qdo_full(0), 0, 42);
-    tc_fence_after();
-    if (elect_one()) issue_scores(0, 0);
-    __syncwarp();
-    int stg = 0;        // stage of tile i
-    uint32_t ph_n = 0;  // phase of the stage of tile i+1
-    for (int i = 0; i < n_q; ++i) {
-      const int w = i & 1;
-      int stg_n = stg + 1;
-      if (stg_n == NSTG) stg_n = 0;
-      if (i + 1 < n_q) {
-        if (stg_n == 0) ph_n ^= 1u;
-        mbar_wait(qdo_full(stg_n), ph_n, 43);
-        tc_fence_after();
-        if (elect_one()) issue_scores(w ^ 1, stg_n);  // overlaps the compute warpgroup working on tile i
+      for (int j = 0; j < n_q; ++j) {
+        const int stg = j % Cfg::STAGES;
+        mbar_wait(s_empty(stg), ((j / Cfg::STAGES) & 1) ^ 1u, 40);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(s_full(stg), 2 * Cfg::SMALL);
+          for (int a = 0; a < ATOMS; ++a) {
+            tma_load_4d(q_smem + stg * Cfg::SMALL + a * SMALL_ATOM, &maps.q64, s_full(stg), a * 64, h, j * 64, b);
+            tma_load_4d(do_smem + stg * Cfg::SMALL + a * SMALL_ATOM, &maps.do64, s_full(stg), a * 64, h, j * 64, b);
+          }
+        }
         __syncwarp();
       }
-      mbar_wait(p_full(w), (i >> 1) & 1, 44);   // P^T and dS^T of tile i are both in TMEM
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {  // contraction over the 64 query rows of the tile
-          const uint64_t bd = sdesc_mn(do_smem(stg), kk * 2048, ATOM64);
-          mma_ts(DV, X(w) + PK_COL(kk), bd, idesc_acc, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint64_t bd = sdesc_mn(q_smem(stg), kk * 2048, ATOM64);
-          mma_ts(DK, Y(w) + PK_COL(kk), bd, idesc_acc, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        tc_commit(qdo_empty(stg));
-      }
-      __syncwarp();
-      stg = stg_n;
     }
-    if (elect_one()) tc_commit(acc_done);
-    __syncwarp();
-  } else if (warp < 8) {
-    // ===================== compute warpgroups =====================
-    // Warpgroup w owns the 32-column half [32 w, 32 w + 32) of EVERY 64-wide score tile, so one tile's
-    // exp / dS phase is spread over all 8 compute warps (half the latency of a whole tile per warpgroup) and
-    // finishes inside the two MMA groups the tensor pipe has queued behind it.  Each half packs its bf16
-    // P^T / dS^T into the first 16 columns of its own fp32 range (PK_COL), never into the other half's.
-    const int w = warp >> 2;
-    const int r = (warp & 3) * 32 + lane;          // key row within tile == TMEM lane
-    const int wt = threadIdx.x & 127;              // thread within warpgroup
-    const uint32_t lane_off = uint32_t((warp & 3) * 32) << 16;
+  } else {
+    reg_alloc<232>();
+    const int cw = wg - 1;
     const float sl2 = p.scale * 1.4426950408889634f;
-    const float l2e = 1.4426950408889634f;
-    const long long stat_base = ((long long)b * p.H + h) * p.Sq;
-    float* my_stat = stat_ptr + w * 256;           // [2 tile parities][lse 32 | delta 32 | unused 64]
-    auto load_stat = [&](int tile) -> float {      // threads 0-31: lse, 32-63: delta of this warpgroup's 32 queries
-      const int qi = tile * 64 + 32 * w + (wt & 31);
-      const bool ok = qi < p.Sq;
-      return (wt < 32) ? (ok ? p.lse[stat_base + qi] : INFINITY) : (ok ? p.delta[stat_base + qi] : 0.f);
-    };
-    if (wt < 64) {
-      if (0 < n_q) my_stat[wt] = load_stat(0) * (wt < 32 ? l2e : 1.f);
-      if (1 < n_q) my_stat[128 + wt] = load_stat(1) * (wt < 32 ? l2e : 1.f);
-    }
-    named_bar_sync(1 + w, 128);
-    for (int i = 0; i < n_q; ++i) {
-      const int buf = i & 1;
-      const float* lse_s = my_stat + buf * 128;
-      const float* del_s = lse_s + 32;
-      const bool pre = (i + 2 < n_q) && wt < 64;
-      const float nxt = pre ? load_stat(i + 2) : 0.f;   // consumed only after this tile's math (latency hidden)
-      mbar_wait(st_full(buf), (i >> 1) & 1, 46);
-      mbar_wait(dpt_full(buf), (i >> 1) & 1, 47);
-      tc_fence_after();
-      // one pass: P^T = exp2(S^T*sl2 - lse), dS^T = P^T o (dP^T - Delta)  (the softmax scale of dS is
-      // applied once to the dK accumulator in the epilogue)
-#if STB_ATTN_DEBUG_SKIP < 2
-      {
-        uint32_t sv[32], dv[32];
-        tmem_ld_32x32b_x32(X(buf) + lane_off + 32 * w, sv);
-        tmem_ld_32x32b_x32(Y(buf) + lane_off + 32 * w, dv);
-        tc_wait_ld();
-        uint32_t pk[16], dk_[16];
-#if STB_ATTN_DEBUG_SKIP == 1
+    const float* lse_bh = p.lse + ((long long)b * p.H + h) * p.Sq;
+    const float* del_bh = p.delta + ((long long)b * p.H + h) * p.Sq;
+    float dv_acc[HD / 2], dk_acc[HD / 2];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) pk[j] = sv[j] ^ sv[j + 16], dk_[j] = dv[j] ^ dv[j + 16];
-#else
+    for (int i = 0; i < HD / 2; ++i) dv_acc[i] = dk_acc[i] = 0.f;
+    mbar_wait(kv_full, 0, 41);
+    for (int j = 0; j < n_q; ++j) {
+      const int stg = j % Cfg::STAGES;
+      mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 42);
+      const uint32_t qa = q_smem + stg * Cfg::SMALL, da = do_smem + stg * Cfg::SMALL;
+      float st[32], dpt[32];
+      wg_fence();
+      mma_kmajor_n64<HD>(st, k_smem + cw * 8192, BIG_ATOM, qa, SMALL_ATOM);    // S^T  = K Q^T
+      mma_kmajor_n64<HD>(dpt, v_smem + cw * 8192, BIG_ATOM, da, SMALL_ATOM);   // dP^T = V dO^T
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(st);
+      wg_fence_regs(dpt);
+      // st[4 i + 2 hh + e]: key row (16 wq + lane / 4 + 8 hh), query column 8 i + 2 (lane % 4) + e
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 l4 = *reinterpret_cast<const float4*>(lse_s + j);   // smem broadcast
-          const float4 d4 = *reinterpret_cast<const float4*>(del_s + j);
-          const float x0 = ex2f(fmaf(__uint_as_float(sv[j + 0]), sl2, -l4.x));
-          const float x1 = ex2f(fmaf(__uint_as_float(sv[j + 1]), sl2, -l4.y));
-          const float x2 = ex2f(fmaf(__uint_as_float(sv[j + 2]), sl2, -l4.z));
-          const float x3 = ex2f(fmaf(__uint_as_float(sv[j + 3]), sl2, -l4.w));
-          pk[j / 2] = pack_bf16x2(x0, x1);
-          pk[j / 2 + 1] = pack_bf16x2(x2, x3);
-          dk_[j / 2] = pack_bf16x2(x0 * (__uint_as_float(dv[j + 0]) - d4.x), x1 * (__uint_as_float(dv[j + 1]) - d4.y));
-          dk_[j / 2 + 1] = pack_bf16x2(x2 * (__uint_as_float(dv[j + 2]) - d4.z), x3 * (__uint_as_float(dv[j + 3]) - d4.w));
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int q = j * 64 + 8 * i + 2 * (lane & 3) + e;
+          const bool ok = q < p.Sq;
+          const float l2 = ok ? __ldg(lse_bh + q) * 1.4426950408889634f : 0.f;
+          const float dl = ok ? __ldg(del_bh + q) : 0.f;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int x = 4 * i + 2 * hh + e;
+            const float pv = ok ? ex2f(fmaf(st[x], sl2, -l2)) : 0.f;
+            st[x] = pv;                        // P^T
+            dpt[x] = pv * (dpt[x] - dl);       // dS^T (softmax scale applied in the epilogue)
+          }
         }
-#endif
-        tmem_st_32x32b_x16(X(buf) + lane_off + 32 * w, pk);
-        tmem_st_32x32b_x16(Y(buf) + lane_off + 32 * w, dk_);
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {   // 64 queries / 16
+        uint32_t a[4];
+        acc_to_afrag(st, kk, a);
+        wgmma_rs_mn<HD>(dv_acc, a, sdesc_mn(da, kk * 2048, SMALL_ATOM), 1u);
+        acc_to_afrag(dpt, kk, a);
+        wgmma_rs_mn<HD>(dk_acc, a, sdesc_mn(qa, kk * 2048, SMALL_ATOM), 1u);
       }
-#endif
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(p_full(buf));
-      named_bar_sync(1 + w, 128);                      // every thread of the warpgroup is done with this parity's stats
-      if (pre) my_stat[buf * 128 + wt] = nxt * (wt < 32 ? l2e : 1.f);   // tile i + 2 reuses parity buf; read after the next sync
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(dv_acc);
+      wg_fence_regs(dk_acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(s_empty(stg));
     }
-    // ---- epilogue: warpgroup 0 stores dV, warpgroup 1 stores dK
-    mbar_wait(acc_done, 0, 48);
-    tc_fence_after();
-    const int kv = kv0 + r;
+    // ---- epilogue: stage dV and dK rows through the (now idle) K / V tiles, then store row-contiguously
+    named_bar_sync(1, 256);
+    float* stage_rows = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw))) + cw * 64 * (HD + 4);
+    const int t = threadIdx.x & 127;
+    const int r = t >> 1, half = t & 1;
+    const int kv = kv0 + cw * 64 + r;
     const bool row_ok = kv < p.Sk;
-    if (w == 0)
-      store_acc_row<HD>(DV + lane_off, p.dv + (long long)b * p.dv_b + (long long)kv * p.dv_s + (long long)h * p.dv_h, row_ok);
-    else if (!p.fuse_prep)
-      store_acc_row<HD>(DK + lane_off, p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h, row_ok, p.scale);
-    else {
-      // dK row -> gradient of the k projection output (RoPE^T, RMSNorm backward), token index == key index
-      const __nv_bfloat16* xrow = p.src + (long long)b * p.src_b + (long long)kv * p.src_s + p.k_off + h * HD;
-      const __nv_bfloat16* wk = (kv < p.s_split) ? p.wk1 : p.wk0;
-      const float* cs = p.cosT ? p.cosT + (long long)kv * HD : nullptr;
-      const float* sn = p.sinT ? p.sinT + (long long)kv * HD : nullptr;
-      float ss = 0.f, sgx = 0.f;
-      qk_grad_pass1<HD>(DK + lane_off, p.scale, row_ok, xrow, wk, cs, sn, ss, sgx);
-      const float rstd = rsqrtf(ss / HD + p.eps);
-      qk_grad_pass2<HD>(DK + lane_off, row_ok, xrow, rstd, sgx * rstd / HD,
-                        p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h);
+    stage_acc<HD>(stage_rows, dv_acc, 1.f);
+    named_bar_sync(2 + cw, 128);
+    store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dv + (long long)b * p.dv_b + (long long)kv * p.dv_s + (long long)h * p.dv_h,
+                       row_ok, false, nullptr, nullptr, nullptr, nullptr, 0.f);
+    named_bar_sync(2 + cw, 128);
+    stage_acc<HD>(stage_rows, dk_acc, p.scale);
+    named_bar_sync(2 + cw, 128);
+    const __nv_bfloat16* xrow = nullptr;
+    const __nv_bfloat16* wk = nullptr;
+    const float *cs = nullptr, *sn = nullptr;
+    if (p.fuse_prep) {   // dK row -> gradient of the k projection output (token index == key index)
+      xrow = p.src + (long long)b * p.src_b + (long long)min(kv, p.Sk - 1) * p.src_s + p.k_off + h * HD;
+      wk = (kv < p.s_split) ? p.wk1 : p.wk0;
+      cs = p.cosT ? p.cosT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
+      sn = p.sinT ? p.sinT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 10) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h,
+                       row_ok, p.fuse_prep != 0, xrow, wk, cs, sn, p.eps);
   }
 }
 
@@ -458,260 +322,131 @@ __global__ void __launch_bounds__(384, 1)
 attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams p) {
   using Cfg = AttnBwdCfg<HD>;
   constexpr int ATOMS = HD / 64;
-  constexpr int BIG = Cfg::BIG, SMALL = Cfg::SMALL, NSTG = Cfg::STAGES;
-  constexpr int ATOM128 = 128 * 64 * 2;
-  constexpr int ATOM64 = 64 * 64 * 2;
-
+  constexpr int BIG_ATOM = 128 * 128, SMALL_ATOM = 64 * 128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t q_smem = smem_base;
-  const uint32_t do_smem = q_smem + BIG;
-  auto k_smem = [&](int s) { return do_smem + BIG + uint32_t(s) * 2 * SMALL; };
-  auto v_smem = [&](int s) { return k_smem(s) + SMALL; };
-  const uint32_t bar_base = smem_base + 2 * BIG + NSTG * 2 * SMALL + 2 * 2 * 128 * 4;
-  const uint32_t qdo_full = bar_base;
-  auto kv_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bar_base + 8u * (4 + s); };
-  auto s_full = [&](int w) { return bar_base + 8u * (7 + w); };
-  auto dp_full = [&](int w) { return bar_base + 8u * (9 + w); };
-  auto ds_full = [&](int w) { return bar_base + 8u * (11 + w); };
-  const uint32_t dq_done = bar_base + 8u * 13;
-  const uint32_t tmem_slot = bar_base + 8u * 14;
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+  const uint32_t q_smem = smem_base, do_smem = smem_base + Cfg::BIG;
+  const uint32_t k_smem = smem_base + 2 * Cfg::BIG;                      // STAGES streamed K tiles
+  const uint32_t v_smem = k_smem + Cfg::STAGES * Cfg::SMALL;             // STAGES streamed V tiles
+  const uint32_t bar_base = v_smem + Cfg::STAGES * Cfg::SMALL;
+  const uint32_t qd_full = bar_base;
+  auto s_full = [&](int s) { return bar_base + 8u * (1 + s); };
+  auto s_empty = [&](int s) { return bar_base + 8u * (1 + Cfg::STAGES + s); };
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 128;
-  const int h = blockIdx.y;
-  const int b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
+  const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
   const int n_kv = (p.Sk + 63) / 64;
 
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&maps.q128);
-    tma_prefetch_desc(&maps.k64);
-    tma_prefetch_desc(&maps.v64);
-    tma_prefetch_desc(&maps.do128);
-  }
-  if (warp == 9 && lane == 0) {
-    mbar_init(qdo_full, 256);   // Q / dO rows written to TMEM by the 256 compute threads
-    for (int s = 0; s < NSTG; ++s) {
-      mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 1);
+  if (threadIdx.x == 0) {
+    mbar_init(qd_full, 1);
+    for (int s = 0; s < Cfg::STAGES; ++s) {
+      mbar_init(s_full(s), 1);
+      mbar_init(s_empty(s), 8);
     }
-    for (int w = 0; w < 2; ++w) {
-      mbar_init(s_full(w), 1);
-      mbar_init(dp_full(w), 1);
-      mbar_init(ds_full(w), 256);   // both compute warpgroups contribute half the columns of every tile
-    }
-    mbar_init(dq_done, 1);
     fence_mbar_init();
   }
-  if (warp == 10) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  auto Sb = [&](int w) { return tmem_base + uint32_t(w) * 64; };
-  auto Yb = [&](int w) { return tmem_base + 128 + uint32_t(w) * 64; };  // dP (dS packed in place)
-  const uint32_t DQ = tmem_base + 256;
-  // The resident operands live in TMEM (bf16 pairs per column, lane = query row) and feed the score MMAs as the
-  // TS-form A operand: S = Q K^T and dP = dO V^T then fetch only their 64-key B slices from shared memory
-  // (2 KB per MMA instead of 6 KB), which takes the kernel off the shared-memory bandwidth limit.
-  const uint32_t QT = tmem_base + 384;             // Q  [128 x HD] bf16 : HD / 2 columns
-  const uint32_t DOT = tmem_base + 384 + HD / 2;   // dO [128 x HD] bf16
 
-  if (warp == 8) {
-    int stg = 0;
-    uint32_t ph = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      mbar_wait(kv_empty(stg), ph ^ 1u, 50);
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (warp == 0) {
       if (elect_one()) {
-        mbar_arrive_expect_tx(kv_full(stg), 2 * SMALL);
+        mbar_arrive_expect_tx(qd_full, 2 * Cfg::BIG);
         for (int a = 0; a < ATOMS; ++a) {
-          tma_load_4d(k_smem(stg) + a * ATOM64, &maps.k64, kv_full(stg), a * 64, h, j * 64, b);
-          tma_load_4d(v_smem(stg) + a * ATOM64, &maps.v64, kv_full(stg), a * 64, h, j * 64, b);
+          tma_load_4d(q_smem + a * BIG_ATOM, &maps.q128, qd_full, a * 64, h, q0, b);
+          tma_load_4d(do_smem + a * BIG_ATOM, &maps.do128, qd_full, a * 64, h, q0, b);
         }
       }
       __syncwarp();
-      if (++stg == NSTG) {
-        stg = 0;
-        ph ^= 1u;
-      }
-    }
-  } else if (warp == 9) {
-    constexpr uint32_t idesc_s = make_idesc_bf16(128, 64, 0, 0);
-    constexpr uint32_t idesc_dq = make_idesc_bf16(128, HD, 0, 1);
-    auto issue_scores = [&](int w, int stg) {
-#pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-        const uint64_t bd = sdesc_k(k_smem(stg), (kk / 4) * ATOM64 + (kk % 4) * 32);
-        mma_ts(Sb(w), QT + 8 * kk, bd, idesc_s, kk > 0);
-      }
-      tc_commit(s_full(w));
-#pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-        const uint64_t bd = sdesc_k(v_smem(stg), (kk / 4) * ATOM64 + (kk % 4) * 32);
-        mma_ts(Yb(w), DOT + 8 * kk, bd, idesc_s, kk > 0);
-      }
-      tc_commit(dp_full(w));
-    };
-    mbar_wait(qdo_full, 0, 51);
-    mbar_wait(kv_full(0), 0, 52);
-    tc_fence_after();
-    if (elect_one()) issue_scores(0, 0);
-    __syncwarp();
-    int stg = 0;
-    uint32_t ph_n = 0;
-    for (int j = 0; j < n_kv; ++j) {
-      const int w = j & 1;
-      int stg_n = stg + 1;
-      if (stg_n == NSTG) stg_n = 0;
-      if (j + 1 < n_kv) {
-        if (stg_n == 0) ph_n ^= 1u;
-        mbar_wait(kv_full(stg_n), ph_n, 53);
-        tc_fence_after();
-        if (elect_one()) issue_scores(w ^ 1, stg_n);
-        __syncwarp();
-      }
-      mbar_wait(ds_full(w), (j >> 1) & 1, 54);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {  // contraction over the 64 keys of the tile
-          const uint64_t bd = sdesc_mn(k_smem(stg), kk * 2048, ATOM64);
-          mma_ts(DQ, Yb(w) + PK_COL(kk), bd, idesc_dq, (j > 0 || kk > 0) ? 1u : 0u);
-        }
-        tc_commit(kv_empty(stg));
-      }
-      __syncwarp();
-      stg = stg_n;
-    }
-    if (elect_one()) tc_commit(dq_done);
-    __syncwarp();
-  } else if (warp < 8) {
-    const int w = warp >> 2;
-    const int r = (warp & 3) * 32 + lane;  // query row within tile == TMEM lane
-    const uint32_t lane_off = uint32_t((warp & 3) * 32) << 16;
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const int qrow = q0 + r;
-    const bool row_ok = qrow < p.Sq;
-    const long long stat_idx = ((long long)b * p.H + h) * p.Sq + qrow;
-    const float lse2 = row_ok ? p.lse[stat_idx] * 1.4426950408889634f : INFINITY;
-    const float delta = row_ok ? p.delta[stat_idx] : 0.f;
-    {  // warpgroup 0 stages this thread's Q row, warpgroup 1 its dO row (global -> registers -> TMEM)
-      const __nv_bfloat16* src = (w == 0)
-          ? p.q + (long long)b * p.q_b + (long long)qrow * p.q_s + (long long)h * p.q_h
-          : p.d_o + (long long)b * p.do_b + (long long)qrow * p.do_s + (long long)h * p.do_h;
-      const uint32_t dst = (w == 0 ? QT : DOT) + lane_off;
-#pragma unroll
-      for (int c = 0; c < HD / 2; c += 32) {           // 32 columns = 64 bf16 = 128 bytes per chunk
-        uint32_t v[32];
-#pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const uint4 u = row_ok ? __ldg(reinterpret_cast<const uint4*>(src + 2 * c) + q4) : make_uint4(0u, 0u, 0u, 0u);
-          v[4 * q4 + 0] = u.x, v[4 * q4 + 1] = u.y, v[4 * q4 + 2] = u.z, v[4 * q4 + 3] = u.w;
-        }
-        tmem_st_32x32b_x32(dst + c, v);
-      }
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(qdo_full);
-    }
-    // warpgroup w owns key columns [32 w, 32 w + 32) of EVERY 64-key tile (see attn_bwd_dkdv_kernel)
-    for (int j = 0; j < n_kv; ++j) {
-      const int buf = j & 1;
-      const int kv_valid = p.Sk - j * 64 - 32 * w;  // < 32 only on the ragged last tile
-      mbar_wait(s_full(buf), (j >> 1) & 1, 55);
-      mbar_wait(dp_full(buf), (j >> 1) & 1, 56);
-      tc_fence_after();
-#if STB_ATTN_DEBUG_SKIP < 2
-      {
-        uint32_t sv[32], dv[32];
-        tmem_ld_32x32b_x32(Sb(buf) + lane_off + 32 * w, sv);
-        tmem_ld_32x32b_x32(Yb(buf) + lane_off + 32 * w, dv);
-        tc_wait_ld();
-        if (kv_valid < 32) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i >= kv_valid) sv[i] = 0xff800000u;  // -inf -> P = 0
-        }
-        uint32_t pk[16];
-#if STB_ATTN_DEBUG_SKIP == 1
-#pragma unroll
-        for (int i = 0; i < 16; ++i) pk[i] = sv[i] ^ dv[i + 16];
-#else
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = ex2f(fmaf(__uint_as_float(sv[i]), sl2, -lse2));
-          const float p1 = ex2f(fmaf(__uint_as_float(sv[i + 1]), sl2, -lse2));
-          const float d0 = p0 * (__uint_as_float(dv[i]) - delta);       // softmax scale applied in the epilogue
-          const float d1 = p1 * (__uint_as_float(dv[i + 1]) - delta);
-          pk[i / 2] = pack_bf16x2(d0, d1);
-        }
-#endif
-        tmem_st_32x32b_x16(Yb(buf) + lane_off + 32 * w, pk);
-      }
-#endif
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(ds_full(buf));
-    }
-    mbar_wait(dq_done, 0, 57);
-    tc_fence_after();
-    // both warpgroups cover all 128 lanes: split the HD columns between them
-    if (p.fuse_prep) {
-      // dQ row -> gradient of the q projection output; each warpgroup owns HD/2 columns, the two partial
-      // (sum x^2, sum g x) pairs meet in shared memory (the Q tile area is free: Q lives in TMEM)
-      constexpr int NC = HD / 2;
-      const int col = w * NC;
-      const __nv_bfloat16* xrow = p.src + (long long)b * p.src_b + (long long)qrow * p.src_s + h * HD + col;
-      const __nv_bfloat16* wq = (qrow < p.s_split) ? p.wq1 : p.wq0;
-      const float* cs = p.cosT ? p.cosT + (long long)qrow * HD + col : nullptr;
-      const float* sn = p.sinT ? p.sinT + (long long)qrow * HD + col : nullptr;
-      float ss = 0.f, sgx = 0.f;
-      qk_grad_pass1<NC>(DQ + lane_off + col, p.scale, row_ok, xrow, wq ? wq + col : nullptr, cs, sn, ss, sgx);
-      float2* part = reinterpret_cast<float2*>(smem_raw + (q_smem - smem_u32(smem_raw)));   // [2][128]
-      part[w * 128 + r] = make_float2(ss, sgx);
-      named_bar_sync(3, 256);
-      const float2 other = part[(w ^ 1) * 128 + r];
-      ss += other.x;
-      sgx += other.y;
-      const float rstd = rsqrtf(ss / HD + p.eps);
-      qk_grad_pass2<NC>(DQ + lane_off + col, row_ok, xrow, rstd, sgx * rstd / HD,
-                        p.dq + (long long)b * p.dq_b + (long long)qrow * p.dq_s + (long long)h * p.dq_h + col);
-    } else {
-      __nv_bfloat16* dqrow = p.dq + (long long)b * p.dq_b + (long long)qrow * p.dq_s + (long long)h * p.dq_h;
-#pragma unroll 1
-      for (int c = 0; c < HD / 2; c += 32) {
-        const int col = w * (HD / 2) + c;
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(DQ + lane_off + col, v);
-        tc_wait_ld();
-        if (row_ok) {
-          uint4* dp = reinterpret_cast<uint4*>(dqrow + col);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(v[q * 8 + 0]) * p.scale, __uint_as_float(v[q * 8 + 1]) * p.scale);
-            u.y = pack_bf16x2(__uint_as_float(v[q * 8 + 2]) * p.scale, __uint_as_float(v[q * 8 + 3]) * p.scale);
-            u.z = pack_bf16x2(__uint_as_float(v[q * 8 + 4]) * p.scale, __uint_as_float(v[q * 8 + 5]) * p.scale);
-            u.w = pack_bf16x2(__uint_as_float(v[q * 8 + 6]) * p.scale, __uint_as_float(v[q * 8 + 7]) * p.scale);
-            dp[q] = u;
+      for (int j = 0; j < n_kv; ++j) {
+        const int stg = j % Cfg::STAGES;
+        mbar_wait(s_empty(stg), ((j / Cfg::STAGES) & 1) ^ 1u, 50);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(s_full(stg), 2 * Cfg::SMALL);
+          for (int a = 0; a < ATOMS; ++a) {
+            tma_load_4d(k_smem + stg * Cfg::SMALL + a * SMALL_ATOM, &maps.k64, s_full(stg), a * 64, h, j * 64, b);
+            tma_load_4d(v_smem + stg * Cfg::SMALL + a * SMALL_ATOM, &maps.v64, s_full(stg), a * 64, h, j * 64, b);
           }
         }
+        __syncwarp();
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 10) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  } else {
+    reg_alloc<232>();
+    const int cw = wg - 1, wq = warp & 3;
+    const float sl2 = p.scale * 1.4426950408889634f;
+    // this thread's two query rows
+    float l2[2], dl[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q = q0 + cw * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+      const long long o = ((long long)b * p.H + h) * p.Sq + min(q, p.Sq - 1);
+      l2[hh] = __ldg(p.lse + o) * 1.4426950408889634f;
+      dl[hh] = __ldg(p.delta + o);
+    }
+    float dq_acc[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) dq_acc[i] = 0.f;
+    mbar_wait(qd_full, 0, 51);
+    for (int j = 0; j < n_kv; ++j) {
+      const int stg = j % Cfg::STAGES;
+      mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 52);
+      const uint32_t ka = k_smem + stg * Cfg::SMALL, va = v_smem + stg * Cfg::SMALL;
+      float sc[32], dp[32];
+      wg_fence();
+      mma_kmajor_n64<HD>(sc, q_smem + cw * 8192, BIG_ATOM, ka, SMALL_ATOM);    // S  = Q K^T
+      mma_kmajor_n64<HD>(dp, do_smem + cw * 8192, BIG_ATOM, va, SMALL_ATOM);   // dP = dO V^T
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(sc);
+      wg_fence_regs(dp);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const bool ok = j * 64 + 8 * i + 2 * (lane & 3) + e < p.Sk;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int x = 4 * i + 2 * hh + e;
+            const float pv = ok ? ex2f(fmaf(sc[x], sl2, -l2[hh])) : 0.f;
+            dp[x] = pv * (dp[x] - dl[hh]);   // dS (softmax scale applied in the epilogue)
+          }
+        }
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {   // 64 keys / 16
+        uint32_t a[4];
+        acc_to_afrag(dp, kk, a);
+        wgmma_rs_mn<HD>(dq_acc, a, sdesc_mn(ka, kk * 2048, SMALL_ATOM), 1u);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(dq_acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(s_empty(stg));
+    }
+    // ---- epilogue through the (now idle) Q / dO tiles
+    named_bar_sync(1, 256);
+    float* stage_rows = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw))) + cw * 64 * (HD + 4);
+    const int t = threadIdx.x & 127;
+    const int r = t >> 1, half = t & 1;
+    const int qrow = q0 + cw * 64 + r;
+    const bool row_ok = qrow < p.Sq;
+    stage_acc<HD>(stage_rows, dq_acc, p.scale);
+    named_bar_sync(2 + cw, 128);
+    const __nv_bfloat16* xrow = nullptr;
+    const __nv_bfloat16* wqn = nullptr;
+    const float *cs = nullptr, *sn = nullptr;
+    if (p.fuse_prep) {   // dQ row -> gradient of the q projection output
+      const int qc = min(qrow, p.Sq - 1);
+      xrow = p.src + (long long)b * p.src_b + (long long)qc * p.src_s + h * HD;
+      wqn = (qrow < p.s_split) ? p.wq1 : p.wq0;
+      cs = p.cosT ? p.cosT + (long long)qc * HD : nullptr;
+      sn = p.sinT ? p.sinT + (long long)qc * HD : nullptr;
+    }
+    store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dq + (long long)b * p.dq_b + (long long)qrow * p.dq_s + (long long)h * p.dq_h,
+                       row_ok, p.fuse_prep != 0, xrow, wqn, cs, sn, p.eps);
   }
 }
 

@@ -1,21 +1,14 @@
-// simpletuner_b200 — joint (non-causal) softmax attention forward on tcgen05, sm_100a.
+// simpletuner_b200 — joint (non-causal) softmax attention forward on wgmma, sm_90a.
 //
 // Replaces F.scaled_dot_product_attention at reference flux/transformer.py:200-207 (and the SD3 /
 // PixArt call sites) for the training path: O = softmax(Q K^T * scale) V, plus the per-row
 // log-sum-exp that the backward kernel consumes.
 //
-// One CTA owns 256 query rows (two 128-row tiles, "A" and "B") of one (batch, head) and streams the
-// whole key/value sequence in 128-key tiles:
-//   warps 0-3  : softmax warpgroup for Q tile A   (thread r <-> TMEM lane r <-> query row r)
-//   warps 4-7  : softmax warpgroup for Q tile B
-//   warp  8    : TMA producer (Q once, K/V double-buffered)
-//   warp  9    : MMA issuer (single thread): S = Q K^T (SS), O += P V (P from TMEM, V MN-major)
-//   warp  10   : TMEM allocator
-// TMEM (512 cols): S_A [0,128) S_B [128,256) O_A [256,256+HD) O_B [384,384+HD); P (bf16) is written
-// in place over the first 64 columns of its S buffer.  While one warpgroup runs softmax on its
-// tile the tensor pipe works on the other tile's MMAs (ping-pong).
-// The running max is only refreshed when it grows by more than 2^8 (lazy rescale), so the O
-// accumulator is touched by CUDA cores only a handful of times per row.
+// One CTA owns 128 query rows of one (batch, head) and streams the whole key/value sequence in 128-key tiles:
+//   warpgroup 0    : TMA producer (Q once, K / V double-buffered; one warp issues)
+//   warpgroups 1, 2: 64 query rows each.  S = Q K^T (wgmma, both operands in shared memory, S in registers),
+//                    online softmax in registers, O += P V (wgmma with P as the register A operand, V MN-major).
+// The two consumer warpgroups run independently, so one's softmax overlaps the other's MMAs.
 #pragma once
 #include "common.cuh"
 
@@ -43,13 +36,28 @@ struct AttnFwdCfg {
   static constexpr int ATOMS = HD / 64;
   static constexpr int TILE_BYTES = 128 * HD * 2;
   static constexpr int KV_STAGES = 2;
-  static constexpr int SMEM_BYTES = 2 * TILE_BYTES + KV_STAGES * 2 * TILE_BYTES + 1024 + 256;
+  static constexpr int SMEM_BYTES = TILE_BYTES + KV_STAGES * 2 * TILE_BYTES + 1024 + 256;
   static constexpr int THREADS = 384;
 };
 
-// BIAS = true (text encoders only): the bias tile is added to the raw scores (pre-divided by the softmax scale) in both
-// softmax passes.  Every query row needs at least one finite logit in its FIRST key tile (true for a causal mask and for
-// un-masked relative-position biases).  The BIAS = false instantiation is the training kernel, byte-identical to before.
+// A operand (64 x 16, bf16) of k-step kk from a 64 x N fp32 accumulator in wgmma layout
+template <int R>
+__device__ __forceinline__ void acc_to_afrag(const float (&d)[R], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(d[8 * kk + 0], d[8 * kk + 1]);
+  a[1] = pack_bf16x2(d[8 * kk + 2], d[8 * kk + 3]);
+  a[2] = pack_bf16x2(d[8 * kk + 4], d[8 * kk + 5]);
+  a[3] = pack_bf16x2(d[8 * kk + 6], d[8 * kk + 7]);
+}
+
+template <int N>
+__device__ __forceinline__ void wgmma_rs_mn(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t accumulate) {
+  if constexpr (N == 128) wgmma_rs_n128<1>(d, a, b, accumulate);
+  else wgmma_rs_n64<1>(d, a, b, accumulate);
+}
+
+// BIAS = true (text encoders only): the bias tile is added to the raw scores (pre-divided by the softmax scale).  Every
+// query row needs at least one finite logit in its FIRST key tile (true for a causal mask and for un-masked
+// relative-position biases).
 template <int HD, bool BIAS = false>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p) {
@@ -61,312 +69,193 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t q_smem = smem_base;                       // 2 tiles
-  const uint32_t k_smem = q_smem + 2 * TILE;               // NSTG tiles
-  const uint32_t v_smem = k_smem + NSTG * TILE;            // NSTG tiles
+  const uint32_t q_smem = smem_base;
+  const uint32_t k_smem = q_smem + TILE;
+  const uint32_t v_smem = k_smem + NSTG * TILE;
   const uint32_t bar_base = v_smem + NSTG * TILE;
-  // barrier map
   const uint32_t q_full = bar_base;
   auto k_full = [&](int s) { return bar_base + 8u * (1 + s); };
   auto k_empty = [&](int s) { return bar_base + 8u * (1 + NSTG + s); };
   auto v_full = [&](int s) { return bar_base + 8u * (1 + 2 * NSTG + s); };
   auto v_empty = [&](int s) { return bar_base + 8u * (1 + 3 * NSTG + s); };
-  auto s_full = [&](int t) { return bar_base + 8u * (1 + 4 * NSTG + t); };
-  auto p_full = [&](int t) { return bar_base + 8u * (3 + 4 * NSTG + t); };
-  auto o_done = [&](int t) { return bar_base + 8u * (5 + 4 * NSTG + t); };
-  const uint32_t tmem_slot = bar_base + 8u * (7 + 4 * NSTG);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 256;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
+  const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int n_kv = (p.Sk + 127) / 128;
 
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.q);
     tma_prefetch_desc(&maps.k);
     tma_prefetch_desc(&maps.v);
-  }
-  if (warp == 9 && lane == 0) {
     mbar_init(q_full, 1);
     for (int s = 0; s < NSTG; ++s) {
       mbar_init(k_full(s), 1);
-      mbar_init(k_empty(s), 1);
+      mbar_init(k_empty(s), 8);
       mbar_init(v_full(s), 1);
-      mbar_init(v_empty(s), 1);
-    }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(s_full(t), 1);
-      mbar_init(p_full(t), 128);
-      mbar_init(o_done(t), 1);
+      mbar_init(v_empty(s), 8);
     }
     fence_mbar_init();
   }
-  if (warp == 10) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  auto S_col = [&](int t) { return tmem_base + uint32_t(t * 128); };
-  auto O_col = [&](int t) { return tmem_base + uint32_t(256 + t * 128); };
 
-  // Producer / MMA warps run their loops warp-uniformly; only the issuing instructions are executed by
-  // one elected lane, so descriptors live in uniform registers and UTCHMMA / UTMALDG issue back to back.
-  if (warp == 8) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(q_full, 2 * TILE);
-      for (int t = 0; t < 2; ++t)
-        for (int a = 0; a < ATOMS; ++a)
-          tma_load_4d(q_smem + t * TILE + a * ATOM_BYTES, &maps.q, q_full, a * 64, h, q0 + t * 128, b);
-    }
-    __syncwarp();
-    for (int j = 0; j < n_kv; ++j) {
-      const int stg = j % NSTG;
-      const uint32_t par = ((j / NSTG) & 1) ^ 1u;
-      mbar_wait(k_empty(stg), par, 10);
+    reg_dealloc<40>();
+    if (warp == 0) {
       if (elect_one()) {
-        mbar_arrive_expect_tx(k_full(stg), TILE);
-        for (int a = 0; a < ATOMS; ++a)
-          tma_load_4d(k_smem + stg * TILE + a * ATOM_BYTES, &maps.k, k_full(stg), a * 64, h, j * 128, b);
+        mbar_arrive_expect_tx(q_full, TILE);
+        for (int a = 0; a < ATOMS; ++a) tma_load_4d(q_smem + a * ATOM_BYTES, &maps.q, q_full, a * 64, h, q0, b);
       }
       __syncwarp();
-      mbar_wait(v_empty(stg), par, 11);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(v_full(stg), TILE);
-        for (int a = 0; a < ATOMS; ++a)
-          tma_load_4d(v_smem + stg * TILE + a * ATOM_BYTES, &maps.v, v_full(stg), a * 64, h, j * 128, b);
+      for (int j = 0; j < n_kv; ++j) {
+        const int stg = j % NSTG;
+        const uint32_t par = ((j / NSTG) & 1) ^ 1u;
+        mbar_wait(k_empty(stg), par, 10);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(k_full(stg), TILE);
+          for (int a = 0; a < ATOMS; ++a)
+            tma_load_4d(k_smem + stg * TILE + a * ATOM_BYTES, &maps.k, k_full(stg), a * 64, h, j * 128, b);
+        }
+        __syncwarp();
+        mbar_wait(v_empty(stg), par, 11);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(v_full(stg), TILE);
+          for (int a = 0; a < ATOMS; ++a)
+            tma_load_4d(v_smem + stg * TILE + a * ATOM_BYTES, &maps.v, v_full(stg), a * 64, h, j * 128, b);
+        }
+        __syncwarp();
       }
-      __syncwarp();
     }
-  } else if (warp == 9) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);  // Q (K-major) x K (K-major)
-    constexpr uint32_t idesc_o = make_idesc_bf16(128, HD, 0, 1);   // P (TMEM)    x V (MN-major)
-    auto issue_S = [&](int t, int stg) {
-      const uint32_t qa = q_smem + t * TILE;
-      const uint32_t ka = k_smem + stg * TILE;
+  } else {
+    // ===================== consumers: 64 query rows each =====================
+    reg_alloc<232>();
+    const int cw = wg - 1;
+    const int wq = warp & 3;
+    const int r_lo = q0 + cw * 64 + wq * 16 + (lane >> 2);   // rows r_lo and r_lo + 8
+    const float sl2 = p.scale * 1.4426950408889634f;
+    float s_acc[64];
+    float o_acc[HD / 2];
 #pragma unroll
-      for (int kk = 0; kk < HD / 16; ++kk) {
-        const uint64_t ad = sdesc_k(qa, (kk / 4) * ATOM_BYTES + (kk % 4) * 32);
-        const uint64_t bd = sdesc_k(ka, (kk / 4) * ATOM_BYTES + (kk % 4) * 32);
-        mma_ss(S_col(t), ad, bd, idesc_s, kk > 0);
-      }
-    };
-    auto issue_PV = [&](int t, int stg, bool acc) {
-      const uint32_t va = v_smem + stg * TILE;
+    for (int i = 0; i < HD / 2; ++i) o_acc[i] = 0.f;
+    float m_row[2] = {-INFINITY, -INFINITY};   // raw-score row max
+    float l_row[2] = {0.f, 0.f};               // this thread's share of the row sum
+    const __nv_bfloat16* brow[2] = {nullptr, nullptr};
+    if constexpr (BIAS) {
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {  // 128 keys / 16
-        const uint64_t bd = sdesc_mn(va, kk * 2048, ATOM_BYTES);
-        mma_ts(O_col(t), S_col(t) + kk * 8, bd, idesc_o, (acc || kk > 0) ? 1u : 0u);
-      }
-    };
+      for (int hh = 0; hh < 2; ++hh)
+        brow[hh] = p.bias + (long long)h * p.bias_h + (long long)min(r_lo + 8 * hh, p.Sq - 1) * p.bias_q;
+    }
+    const uint32_t qa = q_smem + cw * 8192;
     mbar_wait(q_full, 0, 20);
-    mbar_wait(k_full(0), 0, 21);
-    tc_fence_after();
-    if (elect_one()) {
-      issue_S(0, 0);
-      tc_commit(s_full(0));
-      issue_S(1, 0);
-      tc_commit(s_full(1));
-      tc_commit(k_empty(0));
-    }
-    __syncwarp();
+
     for (int j = 0; j < n_kv; ++j) {
       const int stg = j % NSTG;
       const uint32_t par = (j / NSTG) & 1;
-      const int stg_n = (j + 1) % NSTG;
-      const uint32_t par_n = ((j + 1) / NSTG) & 1;
-      const bool more = (j + 1 < n_kv);
-      mbar_wait(v_full(stg), par, 22);
-      if (more) mbar_wait(k_full(stg_n), par_n, 23);
-      // ---- tile A
-      mbar_wait(p_full(0), j & 1, 24);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_PV(0, stg, j > 0);
-        tc_commit(o_done(0));
-        if (more) {
-          issue_S(0, stg_n);
-          tc_commit(s_full(0));
-        }
+      // ---- S = Q K^T
+      mbar_wait(k_full(stg), par, 21);
+      const uint32_t ka = k_smem + stg * TILE;
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < HD / 16; ++kk) {
+        const uint32_t off = (kk / 4) * ATOM_BYTES + (kk % 4) * 32;
+        wgmma_ss_n128<0, 0>(s_acc, sdesc_k(qa, off), sdesc_k(ka, off), kk > 0 ? 1u : 0u);
       }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(s_acc);
       __syncwarp();
-      // ---- tile B
-      mbar_wait(p_full(1), j & 1, 25);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_PV(1, stg, j > 0);
-        tc_commit(o_done(1));
-        tc_commit(v_empty(stg));
-        if (more) {
-          issue_S(1, stg_n);
-          tc_commit(s_full(1));
-          tc_commit(k_empty(stg_n));
-        }
-      }
-      __syncwarp();
-    }
-  } else if (warp < 8) {
-    // ===================== softmax warpgroups =====================
-    const int t = warp >> 2;                 // Q tile
-    const int r = (warp & 3) * 32 + lane;    // row within tile == TMEM lane
-    const uint32_t lane_off = uint32_t((warp & 3) * 32) << 16;
-    const uint32_t s_t = S_col(t) + lane_off;
-    const uint32_t o_t = O_col(t) + lane_off;
-    const float sl2 = p.scale * 1.4426950408889634f;
-    float m_used = -INFINITY;  // raw-score max currently baked into O and l
-    float l = 0.f;
-    // BIAS: this thread's bias row (query index clamped for the ragged last Q tile; those rows are never written)
-    const __nv_bfloat16* brow = nullptr;
-    if constexpr (BIAS)
-      brow = p.bias + (long long)h * p.bias_h + (long long)min(q0 + t * 128 + r, p.Sq - 1) * p.bias_q;
-    auto add_bias = [&](uint32_t (&v)[64], int col0, int kv_left) {   // v[i] += bias[col0 + i] / scale for i < kv_left
-      if constexpr (BIAS) {
-        const __nv_bfloat16* bp = brow + col0;
-        if (kv_left >= 64 && ((reinterpret_cast<uintptr_t>(bp) & 15) == 0)) {
-#pragma unroll
-          for (int q8 = 0; q8 < 8; ++q8) {
-            const uint4 u = __ldg(reinterpret_cast<const uint4*>(bp) + q8);
-            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              v[q8 * 8 + 2 * e] = __float_as_uint(fmaf(bf16_lo(w[e]), p.inv_scale, __uint_as_float(v[q8 * 8 + 2 * e])));
-              v[q8 * 8 + 2 * e + 1] = __float_as_uint(fmaf(bf16_hi(w[e]), p.inv_scale, __uint_as_float(v[q8 * 8 + 2 * e + 1])));
-            }
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 64; ++i)
-            if (i < kv_left) v[i] = __float_as_uint(fmaf(__bfloat162float(bp[i]), p.inv_scale, __uint_as_float(v[i])));
-        }
-      }
-    };
+      if (lane == 0) mbar_arrive(k_empty(stg));
 
-    for (int j = 0; j < n_kv; ++j) {
-      mbar_wait(s_full(t), j & 1, 30);
-      tc_fence_after();
-      const int kv_valid = p.Sk - j * 128;  // >= 1; < 128 only on the last, ragged tile
-      const bool ragged = kv_valid < 128;   // CTA-uniform: only the last, ragged key tile pays for masking
-      // ---- pass 1: row max, two 64-column TMEM reads (4 independent max chains)
-      float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
+      // ---- online softmax (s_acc[4 i + 2 hh + e] = row r_lo + 8 hh, key 8 i + 2 (lane % 4) + e)
+      const int kv_valid = p.Sk - j * 128;
 #pragma unroll
-      for (int c = 0; c < 128; c += 64) {
-        uint32_t v[64];
-        tmem_ld_32x32b_x64(s_t + c, v);
-        tc_wait_ld();
-        add_bias(v, j * 128 + c, kv_valid - c);
-        if (ragged) {
+      for (int i = 0; i < 16; ++i) {
 #pragma unroll
-          for (int i = 0; i < 64; ++i)
-            if (c + i >= kv_valid) v[i] = 0xff800000u;  // -inf
-        }
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * i + 2 * (lane & 3) + e;
 #pragma unroll
-        for (int i = 0; i < 64; i += 4) {
-          m0 = fmaxf(m0, __uint_as_float(v[i]));
-          m1 = fmaxf(m1, __uint_as_float(v[i + 1]));
-          m2 = fmaxf(m2, __uint_as_float(v[i + 2]));
-          m3 = fmaxf(m3, __uint_as_float(v[i + 3]));
-        }
-      }
-      const float m_tile = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-      // ---- lazy rescale decision (warp-uniform, tcgen05.ld/st are warp-collective)
-      const bool need = (m_tile - m_used) * sl2 > 8.0f;  // true on the first tile (m_used = -inf)
-      if (__any_sync(0xffffffffu, need)) {
-        const float m_new = fmaxf(m_used, m_tile);
-        const float alpha = ex2f((m_used - m_new) * sl2);  // 0 on the first tile
-        l *= alpha;
-        m_used = m_new;
-        if (j > 0) {
-          mbar_wait(o_done(t), (j - 1) & 1, 31);  // PV_{j-1} has landed in O
-          tc_fence_after();
-#pragma unroll 1
-          for (int c = 0; c < HD; c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(o_t + c, v);
-            tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-            tmem_st_32x32b_x32(o_t + c, v);
+          for (int hh = 0; hh < 2; ++hh) {
+            float v = s_acc[4 * i + 2 * hh + e];
+            if constexpr (BIAS) {
+              if (c < kv_valid) v = fmaf(__bfloat162float(brow[hh][j * 128 + c]), p.inv_scale, v);
+            }
+            if (c >= kv_valid) v = -INFINITY;
+            s_acc[4 * i + 2 * hh + e] = v;
           }
-          tc_wait_st();
         }
       }
-      // ---- pass 2: P = exp2(s*sl2 - m*sl2) -> bf16, in place over the first 64 columns of S (packed FFMA2 / FADD2 math).
-      // The packed store of columns [c/2, c/2 + 32) only overwrites fp32 columns that are already in registers.
-      const float2 sl2x2 = make_float2(sl2, sl2), nmb = make_float2(-m_used * sl2, -m_used * sl2);
-      float2 lacc = make_float2(0.f, 0.f);
+      float alpha[2], nmb[2];
 #pragma unroll
-      for (int c = 0; c < 128; c += 64) {
-        uint32_t v[64];
-        tmem_ld_32x32b_x64(s_t + c, v);
-        tc_wait_ld();
-        add_bias(v, j * 128 + c, kv_valid - c);
-        if (ragged) {
+      for (int hh = 0; hh < 2; ++hh) {
+        float m = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < 64; ++i)
-            if (c + i >= kv_valid) v[i] = 0xff800000u;  // exp2(-inf) = 0
-        }
+        for (int i = 0; i < 16; ++i) m = fmaxf(m, fmaxf(s_acc[4 * i + 2 * hh], s_acc[4 * i + 2 * hh + 1]));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        const float m_new = fmaxf(m_row[hh], m);
+        alpha[hh] = ex2f((m_row[hh] - m_new) * sl2);   // 0 on the first tile
+        m_row[hh] = m_new;
+        nmb[hh] = -m_new * sl2;
+        l_row[hh] *= alpha[hh];
+      }
 #pragma unroll
-        for (int h2 = 0; h2 < 64; h2 += 32) {
-          uint32_t pk[16];
+      for (int i = 0; i < HD / 8; ++i) {
+        o_acc[4 * i + 0] *= alpha[0];
+        o_acc[4 * i + 1] *= alpha[0];
+        o_acc[4 * i + 2] *= alpha[1];
+        o_acc[4 * i + 3] *= alpha[1];
+      }
 #pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float2 a = __ffma2_rn(make_float2(__uint_as_float(v[h2 + i]), __uint_as_float(v[h2 + i + 1])), sl2x2, nmb);
-            const float2 x = make_float2(ex2f(a.x), ex2f(a.y));
-            lacc = __fadd2_rn(lacc, x);
-            pk[i / 2] = pack_bf16x2(x.x, x.y);
+      for (int i = 0; i < 16; ++i) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float x = ex2f(fmaf(s_acc[4 * i + 2 * hh + e], sl2, nmb[hh]));
+            l_row[hh] += x;
+            s_acc[4 * i + 2 * hh + e] = x;
           }
-          tmem_st_32x32b_x16(s_t + (c + h2) / 2, pk);
         }
       }
-      const float l0 = lacc.x, l1 = lacc.y;
-      const float lsum = l0 + l1;
-      l += lsum;
-      tc_wait_st();
-      tc_fence_before();
-      mbar_arrive(p_full(t));
+
+      // ---- O += P V
+      mbar_wait(v_full(stg), par, 22);
+      const uint32_t va = v_smem + stg * TILE;
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {   // 128 keys / 16
+        uint32_t a[4];
+        acc_to_afrag(s_acc, kk, a);
+        wgmma_rs_mn<HD>(o_acc, a, sdesc_mn(va, kk * 2048, ATOM_BYTES), 1u);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_regs(o_acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(v_empty(stg));
     }
 
     // ---- epilogue: O / l -> bf16 -> global; LSE
-    mbar_wait(o_done(t), (n_kv - 1) & 1, 32);
-    tc_fence_after();
-    const int s = q0 + t * 128 + r;
-    const bool row_ok = s < p.Sq;
-    const float inv_l = 1.f / l;
-    __nv_bfloat16* orow = p.O + (long long)b * p.o_b + (long long)s * p.o_s + (long long)h * p.o_h;
-#pragma unroll 1
-    for (int c = 0; c < HD; c += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(o_t + c, v);
-      tc_wait_ld();
-      if (row_ok) {
-        uint4* dp = reinterpret_cast<uint4*>(orow + c);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 u;
-          u.x = pack_bf16x2(__uint_as_float(v[q * 8 + 0]) * inv_l, __uint_as_float(v[q * 8 + 1]) * inv_l);
-          u.y = pack_bf16x2(__uint_as_float(v[q * 8 + 2]) * inv_l, __uint_as_float(v[q * 8 + 3]) * inv_l);
-          u.z = pack_bf16x2(__uint_as_float(v[q * 8 + 4]) * inv_l, __uint_as_float(v[q * 8 + 5]) * inv_l);
-          u.w = pack_bf16x2(__uint_as_float(v[q * 8 + 6]) * inv_l, __uint_as_float(v[q * 8 + 7]) * inv_l);
-          dp[q] = u;
-        }
+    for (int hh = 0; hh < 2; ++hh) {
+      float l = l_row[hh];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const int s = r_lo + 8 * hh;
+      const float inv_l = 1.f / l;
+      if (s < p.Sq) {
+        __nv_bfloat16* orow = p.O + (long long)b * p.o_b + (long long)s * p.o_s + (long long)h * p.o_h;
+#pragma unroll
+        for (int i = 0; i < HD / 8; ++i)
+          *reinterpret_cast<uint32_t*>(orow + 8 * i + 2 * (lane & 3)) =
+              pack_bf16x2(o_acc[4 * i + 2 * hh] * inv_l, o_acc[4 * i + 2 * hh + 1] * inv_l);
+        if (p.lse && (lane & 3) == 0) p.lse[((long long)b * p.H + h) * p.Sq + s] = m_row[hh] * p.scale + logf(l);
       }
     }
-    if (row_ok && p.lse) p.lse[((long long)b * p.H + h) * p.Sq + s] = m_used * p.scale + logf(l);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 10) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

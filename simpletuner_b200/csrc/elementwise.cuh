@@ -3,6 +3,8 @@
 // coalesced accesses; the bf16 rounding points of the reference chain are reproduced so results
 // track the reference path bit-for-bit wherever that is cheap.
 #pragma once
+#include <cooperative_groups.h>
+
 #include "common.cuh"
 
 namespace stb {
@@ -576,18 +578,46 @@ __device__ __forceinline__ void pointwise_loss(float d, int loss_type, float c, 
 }
 
 // ------------------------------------------------------------------------------------------------
+// Loss reduction without floating-point atomics: the loss kernels run as ONE cluster of LOSS_CTAS CTAs of
+// LOSS_THREADS threads (a fixed grid, so every thread sums a fixed set of elements in a fixed order); each CTA reduces
+// its threads in a fixed tree, and CTA 0 adds the CTA sums in rank order through distributed shared memory.  The loss
+// is therefore the same bit for bit from run to run.
+// ------------------------------------------------------------------------------------------------
+constexpr int LOSS_CTAS = 8;
+constexpr int LOSS_THREADS = 1024;
+
+__device__ __forceinline__ void loss_cluster_store(float acc, float scale, float* loss_out) {
+  __shared__ float red[LOSS_THREADS / 32];
+  __shared__ float cta_sum;
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    const float v = warp_sum(red[threadIdx.x]);
+    if (threadIdx.x == 0) cta_sum = v;
+  }
+  cooperative_groups::cluster_group cl = cooperative_groups::this_cluster();
+  cl.sync();
+  if (cl.block_rank() == 0 && threadIdx.x == 0) {
+    float t = 0.f;
+    for (unsigned r = 0; r < cl.num_blocks(); ++r) t += *cl.map_shared_rank(&cta_sum, r);
+    *loss_out = t * scale;
+  }
+  cl.sync();   // the other CTAs' shared memory stays alive until CTA 0 has read it
+}
+
+// ------------------------------------------------------------------------------------------------
 // Loss: mean over batch of mean over (C,H,W) of (pred.float() - target.float())^2 with
 // target = noise - latents (flow matching, common.py:4610-4611, 6286, 6426-6429), where pred arrives
 // in the packed token layout (unpack_latents, flux/__init__.py:33-44, folded into the index math).
 // Also emits d loss / d pred in the packed layout (bf16) scaled by `grad_scale`.
-// partial sums -> atomicAdd into loss_out[0] (fp32), caller zeroes it.
+// loss_out[0] (fp32) is written, not accumulated; launch as one cluster (loss_cluster_store).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(LOSS_THREADS)
 flow_mse_loss_kernel(const __nv_bfloat16* __restrict__ pred_packed, const __nv_bfloat16* __restrict__ lat,
                      const __nv_bfloat16* __restrict__ noise, float* __restrict__ loss_out,
                      __nv_bfloat16* __restrict__ dpred_packed, float grad_scale, int B, int C, int Hh,
                      int Ww, int layout, int loss_type, const float* __restrict__ huber_c) {
-  __shared__ float red[8];
   const long long n = (long long)B * C * Hh * Ww;
   const float inv = 1.f / float((long long)C * Hh * Ww) / float(B);
   float acc = 0.f;
@@ -611,15 +641,7 @@ flow_mse_loss_kernel(const __nv_bfloat16* __restrict__ pred_packed, const __nv_b
     acc += lv;
     if (dpred_packed) dpred_packed[pi] = __float2bfloat16(lg * inv * grad_scale);
   }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    float v = red[threadIdx.x];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(loss_out, v * inv);
-  }
+  loss_cluster_store(acc, inv, loss_out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -658,12 +680,11 @@ ddpm_prep_pack_kernel(const __nv_bfloat16* __restrict__ lat, const __nv_bfloat16
 // loss = mean_b [ w_b * mean_chw (pred.float() - target.float())^2 ]   (common.py:6376-6398, 6426-6429)
 // pred: packed tokens [B, (Hh/2)(Ww/2), 4C] (layout as flow_mse_loss_kernel); target: [B, C, Hh, Ww] bf16
 // (epsilon: the noise; v-prediction: get_velocity(...)); weights: fp32 [B] min-SNR weights or nullptr.
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(LOSS_THREADS)
 target_mse_loss_kernel(const __nv_bfloat16* __restrict__ pred_packed, const __nv_bfloat16* __restrict__ target,
                        const float* __restrict__ weights, float* __restrict__ loss_out,
                        __nv_bfloat16* __restrict__ dpred_packed, float grad_scale, int B, int C, int Hh, int Ww,
                        int layout, int loss_type, const float* __restrict__ huber_c) {
-  __shared__ float red[8];
   const long long n = (long long)B * C * Hh * Ww;
   const float inv = 1.f / float((long long)C * Hh * Ww) / float(B);
   float acc = 0.f;
@@ -685,15 +706,7 @@ target_mse_loss_kernel(const __nv_bfloat16* __restrict__ pred_packed, const __nv
     acc += wgt * lv;
     if (dpred_packed) dpred_packed[pi] = __float2bfloat16(lg * wgt * inv * grad_scale);
   }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    float v = red[threadIdx.x];
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(loss_out, v * inv);
-  }
+  loss_cluster_store(acc, inv, loss_out);
 }
 
 // ------------------------------------------------------------------------------------------------

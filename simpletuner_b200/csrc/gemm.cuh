@@ -1,19 +1,17 @@
-// simpletuner_b200 — persistent warp-specialised tcgen05 GEMM for sm_100a.
+// simpletuner_b200 — persistent warp-specialised wgmma GEMM for sm_90a.
 //
 //   D[b, s, n] = epilogue( sum_seg  A_seg[b, s, :] . W_seg[n, :]  + bias[n] )
 //
 // Every operand is K-major bf16 ("TN": activations [rows, K], nn.Linear weights [N, K]), fp32
-// accumulation in TMEM.  Up to three K-segments are chained in one mainloop so that
+// accumulation in registers.  Up to three K-segments are chained in one mainloop so that
 //   * torch.cat([attn, mlp], -1) @ W^T          (reference flux/transformer.py:460-464)
 //   * x @ W^T + (x A^T) B^T   (PEFT LoRA linear, reference common.py:1094-1117)
 // become extra k-blocks of the same tile instead of extra kernels / extra HBM round trips.
 //
-// Roles (256 threads): warp0 = TMA producer, warp1 = MMA issuer (one thread), warp2 = TMEM
-// allocator, warps 4..7 = epilogue (TMEM -> registers -> fused epilogue -> global).
-// A CTA owns MT x 128 rows and BN columns of D per tile; TMEM holds 512/(MT*BN) accumulator
-// stages so the epilogue of tile i overlaps the mainloop of tile i+1 when there are >= 2.
-// PAIR = true is the default for large problems: a 2-CTA cluster (cta_group::2) owns a 256 x BN tile, each CTA
-// stages half of it, the leader issues M = 256 MMAs (see the comment at the kernel).  CONV = true turns the A
+// Roles (384 threads, three warpgroups): warpgroup 0 = TMA producer (one warp issues), warpgroups 1 and 2 =
+// consumers, each owning 64 rows of the CTA's 128 x BN tile: wgmma m64nBNk16 from shared memory, then the fused
+// epilogue straight from the accumulator registers.  The grid is persistent, so the producer already streams the
+// k-blocks of the next tile while the consumers run the epilogue of the current one.  CONV = true turns the A
 // operand into the shifted NHWC window of a 3x3 convolution (implicit GEMM, VAE encoder).
 #pragma once
 #include <type_traits>
@@ -37,7 +35,6 @@ struct GemmParams {
   int N;
   int nseg;
   int kblocks[3];  // ceil(K_seg / 64)
-  int kmmas_last[3];  // UMMA_K=16 steps needed in the last k-block of the segment (1..4)
   int w_kn[3];        // 1: the segment's weight is given as [K, N] row-major (contraction index = row): the B operand is
                       // staged MN-major (64 k-rows x 64 n-columns SWIZZLE_128B boxes) — dgrad reads W itself, no W^T copy
   int epi;
@@ -55,9 +52,6 @@ struct GemmParams {
   // maps.a[0] is then a 4-D map (c, x, y, img) with box (64, 128, 1, 1) and x element-stride = conv_stride;
   // k-block kb covers tap kb / conv_cblocks (dy = tap / 3, dx = tap % 3) and channels (kb % conv_cblocks) * 64.
   int conv_h_out, conv_stride, conv_pad, conv_cblocks;
-  // CONV + pair: 1 = the two CTAs take pixels [s0, s0+128) and [s0+128, s0+256) of one output row (W_out > 128);
-  //              2 = they take two consecutive output rows of <= 128 pixels each
-  int conv_pair_rows;
 };
 
 struct GemmMaps {
@@ -65,36 +59,14 @@ struct GemmMaps {
   CUtensorMap w[3];  // 2-D (k, n),   box (64, BN),      SWIZZLE_128B;  w_kn: 2-D (n, k), box (64, 64)
 };
 
-template <int MT, int BN>
-struct GemmCfg {
-  static constexpr int BM = 128 * MT;
-  static constexpr int BK = 64;
-  static constexpr int A_BYTES = 128 * BK * 2;          // one 128-row A tile
-  static constexpr int W_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = MT * A_BYTES + W_BYTES;
-  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int ACC_COLS = MT * BN;
-  static constexpr int ACC_STAGES = (512 / ACC_COLS) >= 2 ? 2 : 1;
-  static constexpr int TMEM_COLS = (ACC_COLS * ACC_STAGES) <= 32    ? 32
-                                   : (ACC_COLS * ACC_STAGES) <= 64  ? 64
-                                   : (ACC_COLS * ACC_STAGES) <= 128 ? 128
-                                   : (ACC_COLS * ACC_STAGES) <= 256 ? 256
-                                                                    : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-};
-
-// CTA-pair tile: 256 x BN per 2-CTA cluster; per CTA 128 rows of A + BN/2 rows of W per stage, 128 x BN accumulator
 template <int BN>
-struct GemmPairCfg {
-  static constexpr int BM = 256;
+struct GemmCfg {
+  static constexpr int BM = 128;
   static constexpr int BK = 64;
-  static constexpr int A_BYTES = 128 * BK * 2;
-  static constexpr int W_BYTES = (BN / 2) * BK * 2;
+  static constexpr int A_BYTES = BM * BK * 2;
+  static constexpr int W_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
   static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int ACC_COLS = BN;
-  static constexpr int ACC_STAGES = (512 / ACC_COLS) >= 2 ? 2 : 1;
-  static constexpr int TMEM_COLS = 512;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 
@@ -112,121 +84,133 @@ __device__ __forceinline__ void gemm_tile_coords(int tile, int tiles_m, int tile
   tn = within / gsize;
 }
 
-// PAIR = true: cta_group::2 kernel (launch with cluster dims (2,1,1), MT must be 1).  The cluster owns a 256 x BN
-// tile: CTA rank r stages A rows [128 r, 128 r + 128) and W rows [BN/2 r, BN/2 r + BN/2) of every k-block in its own
-// shared memory (6 KB -> 4 KB of operand fetch per SM per MMA k-step at BN = 256), the leader issues one M = 256
-// tcgen05.mma per k-step for both SMs, and each CTA drains its own 128 accumulator lanes.
-template <int MT, int BN, bool CONV = false, bool PAIR = false>
-__global__ void __launch_bounds__(256, 1)
+__device__ __forceinline__ void ld_bf16x2(const __nv_bfloat16* p, bool two, float& a, float& b) {
+  if (two) {
+    const uint32_t u = *reinterpret_cast<const uint32_t*>(p);
+    a = bf16_lo(u);
+    b = bf16_hi(u);
+  } else {
+    a = __bfloat162float(p[0]);
+    b = 0.f;
+  }
+}
+__device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, bool two, float a, float b) {
+  if (two) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
+  else p[0] = __float2bfloat16(a);
+}
+
+// Fused epilogue of two adjacent columns (n, n+1) of one output row; f = accumulator + bias.
+__device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s, int n, bool two, float f0, float f1) {
+  const long long drow = (long long)b * p.d_batch_stride + (long long)s * p.d_row_stride;
+  __nv_bfloat16* xp = p.aux ? p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride + n : nullptr;
+  if (p.epi == EPI_GELU) {
+    if (xp) st_bf16x2(xp, two, f0, f1);
+    // the activation sees the bf16-rounded pre-activation, as the reference's
+    // nn.Linear -> nn.GELU chain does (bf16 tensor between the two modules)
+    f0 = gelu_tanh(gemm_bf16r(f0));
+    f1 = gelu_tanh(gemm_bf16r(f1));
+  } else if (p.epi == EPI_GATE_RES) {
+    float g0, g1, r0, r1;
+    ld_bf16x2(p.gate + (long long)b * p.gate_batch_stride + n, two, g0, g1);
+    ld_bf16x2(p.res + (long long)b * p.res_batch_stride + (long long)s * p.res_row_stride + n, two, r0, r1);
+    // full fine-tune: keep the (bf16) linear output — the gate gradient is sum_s dOut * y
+    if (xp) st_bf16x2(xp, two, f0, f1);
+    // reference order: bias -> (bf16 linear output) -> gate * y -> residual + (...)
+    // (flux/transformer.py:464-465, 584-586, 652-653); each step is a bf16 tensor there.
+    float o[2] = {r0 + gemm_bf16r(g0 * gemm_bf16r(f0)), r1 + gemm_bf16r(g1 * gemm_bf16r(f1))};
+    if (p.nan_to_num) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        float v = gemm_bf16r(o[j]);
+        if (v != v) v = 0.f;
+        else if (v == INFINITY) v = 65504.f;
+        else if (v == -INFINITY) v = -65504.f;
+        o[j] = v;
+      }
+    }
+    f0 = o[0];
+    f1 = o[1];
+  } else if (p.epi == EPI_MUL_DGELU) {
+    float x0, x1;
+    ld_bf16x2(xp, two, x0, x1);
+    f0 *= gelu_tanh_grad(x0);
+    f1 *= gelu_tanh_grad(x1);
+  } else if (p.epi == EPI_MUL) {
+    float x0, x1;
+    ld_bf16x2(xp, two, x0, x1);
+    f0 = gemm_bf16r(f0) * x0;
+    f1 = gemm_bf16r(f1) * x1;
+  } else if (p.epi == EPI_QUICK_GELU) {
+    const float y0 = gemm_bf16r(f0), y1 = gemm_bf16r(f1);
+    f0 = y0 / (1.f + __expf(-1.702f * y0));
+    f1 = y1 / (1.f + __expf(-1.702f * y1));
+  } else if (p.epi == EPI_ADD_RES) {
+    float r0, r1;
+    ld_bf16x2(p.res + (long long)b * p.res_batch_stride + (long long)s * p.res_row_stride + n, two, r0, r1);
+    f0 += r0;
+    f1 += r1;
+  }
+  st_bf16x2(p.D + drow + n, two, f0, f1);
+}
+
+template <int BN, int TB>
+__device__ __forceinline__ void gemm_wgmma(float (&acc)[BN / 2], uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (BN == 256) wgmma_ss_n256<0, TB>(acc, a, b, accumulate);
+  else if constexpr (BN == 128) wgmma_ss_n128<0, TB>(acc, a, b, accumulate);
+  else wgmma_ss_n64<0, TB>(acc, a, b, accumulate);
+}
+
+template <int BN, bool CONV = false>
+__global__ void __launch_bounds__(384, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
-  using Cfg = typename std::conditional<PAIR, GemmPairCfg<BN>, GemmCfg<MT, BN>>::type;
-  static_assert(!PAIR || MT == 1, "pair kernel: MT = 1");
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int tile0 = PAIR ? int(blockIdx.x >> 1) : int(blockIdx.x);
-  const int tile_step = PAIR ? int(gridDim.x >> 1) : int(gridDim.x);
+  using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int ACC_STAGES = Cfg::ACC_STAGES;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto accf_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto acce_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + ACC_STAGES + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 2 * ACC_STAGES);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
 
-  const bool row_pairs = PAIR && CONV && p.conv_pair_rows == 2;
-  const int tiles_per_batch = row_pairs ? 1 : (p.rows_per_batch + Cfg::BM - 1) / Cfg::BM;
-  const int tiles_m = row_pairs ? (p.num_batches + 1) / 2 : tiles_per_batch * p.num_batches;
-  // (batch, first row) of this CTA's 128-row half of m-tile `tm`
-  auto tile_origin = [&](int tm, int& b, int& s0) {
-    if (row_pairs) {
-      b = 2 * tm + int(rank);
-      s0 = 0;
-    } else {
-      b = tm / tiles_per_batch;
-      s0 = (tm - b * tiles_per_batch) * Cfg::BM + (PAIR ? int(rank) * 128 : 0);
-    }
-  };
+  const int tiles_per_batch = (p.rows_per_batch + Cfg::BM - 1) / Cfg::BM;
+  const int tiles_m = tiles_per_batch * p.num_batches;
   const int tiles_n = (p.N + BN - 1) / BN;
   const int num_tiles = tiles_m * tiles_n;
-  int kb_total = 0;
-  for (int s = 0; s < p.nseg; ++s) kb_total += p.kblocks[s];
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < p.nseg; ++s) {
       tma_prefetch_desc(&maps.a[s]);
       tma_prefetch_desc(&maps.w[s]);
     }
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < ACC_STAGES; ++s) {
-      mbar_init(accf_bar(s), 1);
-      mbar_init(acce_bar(s), PAIR ? 8 : 4);   // pair: the leader's barrier collects both CTAs' epilogue warps
+      mbar_init(empty_bar(s), 8);   // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if constexpr (PAIR) {
-      tmem_alloc2(tmem_slot, Cfg::TMEM_COLS);
-      tmem_relinquish2();
-    } else {
-      tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  __syncthreads();
 
-  if (warp == 0) {
-    // ===================== TMA producer (warp-uniform loop, one elected lane issues) =====================
-    {
+  if (wg == 0) {
+    // ===================== TMA producer (warp 0, one elected lane issues) =====================
+    reg_dealloc<40>();
+    if (warp == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int tm, tn;
         gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
-        int b, s0;
-        tile_origin(tm, b, s0);
+        const int b = tm / tiles_per_batch;
+        const int s0 = (tm - b * tiles_per_batch) * Cfg::BM;
         const int n0 = tn * BN;
         for (int seg = 0; seg < p.nseg; ++seg) {
           for (int kb = 0; kb < p.kblocks[seg]; ++kb) {
             mbar_wait(empty_bar(stage), phase ^ 1u, 1);
             const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
             if (elect_one()) {
-              if constexpr (PAIR) {
-                // both CTAs' bytes are accounted on the leader's barrier (the MMA issuer waits there)
-                if (rank == 0) mbar_arrive_expect_tx(full_bar(stage), 2 * Cfg::STAGE_BYTES);
-                if constexpr (CONV) {
-                  const int tap = kb / p.conv_cblocks;
-                  const int c0 = (kb - tap * p.conv_cblocks) * 64;
-                  const int img = b / p.conv_h_out, yo = b - img * p.conv_h_out;   // b past the last row -> img out of range -> zeros
-                  const int dy = tap / 3, dx = tap - dy * 3;
-                  tma_load_4d_pair(sa, &maps.a[0], full_bar(stage), c0, s0 * p.conv_stride + dx - p.conv_pad,
-                                   yo * p.conv_stride + dy - p.conv_pad, img);
-                } else {
-                  tma_load_3d_pair(sa, &maps.a[seg], full_bar(stage), kb * 64, s0, b);
-                }
-                if (p.w_kn[seg]) {
-#pragma unroll
-                  for (int g = 0; g < BN / 128; ++g)
-                    tma_load_2d_pair(sa + Cfg::A_BYTES + g * 8192, &maps.w[seg], full_bar(stage), n0 + int(rank) * (BN / 2) + g * 64, kb * 64);
-                } else {
-                  tma_load_2d_pair(sa + Cfg::A_BYTES, &maps.w[seg], full_bar(stage), kb * 64, n0 + int(rank) * (BN / 2));
-                }
-              } else {
               mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
               if constexpr (CONV) {
                 // implicit-GEMM 3x3 conv: shifted input window; TMA zero-fills the halo (x / y out of range)
@@ -237,17 +221,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
                 tma_load_4d(sa, &maps.a[0], full_bar(stage), c0, s0 * p.conv_stride + dx - p.conv_pad,
                             yo * p.conv_stride + dy - p.conv_pad, img);
               } else {
-#pragma unroll
-                for (int mt = 0; mt < MT; ++mt)
-                  tma_load_3d(sa + mt * Cfg::A_BYTES, &maps.a[seg], full_bar(stage), kb * 64, s0 + mt * 128, b);
+                tma_load_3d(sa, &maps.a[seg], full_bar(stage), kb * 64, s0, b);
               }
               if (p.w_kn[seg]) {
 #pragma unroll
                 for (int g = 0; g < BN / 64; ++g)
-                  tma_load_2d(sa + MT * Cfg::A_BYTES + g * 8192, &maps.w[seg], full_bar(stage), n0 + g * 64, kb * 64);
+                  tma_load_2d(sa + Cfg::A_BYTES + g * 8192, &maps.w[seg], full_bar(stage), n0 + g * 64, kb * 64);
               } else {
-                tma_load_2d(sa + MT * Cfg::A_BYTES, &maps.w[seg], full_bar(stage), kb * 64, n0);
-              }
+                tma_load_2d(sa + Cfg::A_BYTES, &maps.w[seg], full_bar(stage), kb * 64, n0);
               }
             }
             __syncwarp();
@@ -259,289 +240,73 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         }
       }
     }
-  } else if (warp == 1 && rank == 0) {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    {
-      constexpr uint32_t idesc_k = make_idesc_bf16(PAIR ? 256 : 128, BN, 0, 0);
-      constexpr uint32_t idesc_mn = make_idesc_bf16(PAIR ? 256 : 128, BN, 0, 1);   // B operand MN-major (w_kn segments)
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        mbar_wait(acce_bar(acc), acc_phase ^ 1u, 2);
-        tc_fence_after();
-        const uint32_t d_base = tmem_base + acc * Cfg::ACC_COLS;
-        uint32_t accumulate = 0;
-        for (int seg = 0; seg < p.nseg; ++seg) {
-          for (int kb = 0; kb < p.kblocks[seg]; ++kb) {
-            mbar_wait(full_bar(stage), phase, 3);
-            tc_fence_after();
-            const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-            const uint32_t sw = sa + MT * Cfg::A_BYTES;
-            const int nk = (kb == p.kblocks[seg] - 1) ? p.kmmas_last[seg] : 4;
-            const bool wkn = p.w_kn[seg] != 0;
-            const uint32_t idesc = wkn ? idesc_mn : idesc_k;
-            if (elect_one()) {
-              for (int kk = 0; kk < nk; ++kk) {
-                const uint64_t bdesc = wkn ? sdesc_mn(sw, kk * 2048, 8192) : sdesc_k(sw, kk * 32);
-                if constexpr (PAIR) {
-                  mma_ss2(d_base, sdesc_k(sa, kk * 32), bdesc, idesc, accumulate);
-                } else {
-#pragma unroll
-                  for (int mt = 0; mt < MT; ++mt) {
-                    const uint64_t adesc = sdesc_k(sa, mt * Cfg::A_BYTES + kk * 32);
-                    mma_ss(d_base + mt * BN, adesc, bdesc, idesc, accumulate);
-                  }
-                }
-                accumulate = 1;
-              }
-              // frees the smem slot (in both CTAs of a pair) once these MMAs retire
-              if constexpr (PAIR) tc_commit2(empty_bar(stage)); else tc_commit(empty_bar(stage));
-            }
-            __syncwarp();
-            accumulate = 1;
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-        }
-        if (elect_one()) {  // accumulator complete -> epilogue (of both CTAs of a pair)
-          if constexpr (PAIR) tc_commit2(accf_bar(acc)); else tc_commit(accf_bar(acc));
-        }
-        __syncwarp();
-        if (++acc == ACC_STAGES) {
-          acc = 0;
-          acc_phase ^= 1u;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int ew = warp - 4;  // == warp % 4 -> TMEM lanes [32*ew, 32*ew+32)
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+  } else {
+    // ===================== consumers: 64 rows each =====================
+    reg_alloc<232>();
+    const int cw = wg - 1;               // rows [64 cw, 64 cw + 64) of the tile
+    const int wq = warp & 3;             // warp within the warpgroup: rows 16 wq .. 16 wq + 15
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int tm, tn;
       gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
-      int b, s0;
-      tile_origin(tm, b, s0);
+      const int b = tm / tiles_per_batch;
+      const int s0 = (tm - b * tiles_per_batch) * Cfg::BM + cw * 64;
       const int n0 = tn * BN;
-      mbar_wait(accf_bar(acc), acc_phase, 4);
-      tc_fence_after();
-#pragma unroll 1
-      for (int mt = 0; mt < MT; ++mt) {
-        const int s = s0 + mt * 128 + ew * 32 + lane;
-        const bool row_ok = s < p.rows_per_batch && b < p.num_batches;
-        __nv_bfloat16* drow = p.D + (long long)b * p.d_batch_stride + (long long)s * p.d_row_stride;
-        const __nv_bfloat16* rrow =
-            p.res ? p.res + (long long)b * p.res_batch_stride + (long long)s * p.res_row_stride : nullptr;
-        __nv_bfloat16* xrow =
-            p.aux ? p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride : nullptr;
-        const __nv_bfloat16* grow = p.gate ? p.gate + (long long)b * p.gate_batch_stride : nullptr;
-        const uint32_t t_row = tmem_base + (uint32_t(ew * 32) << 16) + acc * Cfg::ACC_COLS + mt * BN;
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-          if (n0 + c >= p.N) break;  // warp-uniform
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(t_row + c, v);
-          tc_wait_ld();
-          const int n = n0 + c;
-          const bool full = (n + 32 <= p.N);
-          float f[32];
+      uint32_t accumulate = 0;
+      int prev_stage = -1;
+      for (int seg = 0; seg < p.nseg; ++seg) {
+        const bool wkn = __shfl_sync(0xffffffffu, p.w_kn[seg], 0) != 0;
+        for (int kb = 0; kb < p.kblocks[seg]; ++kb) {
+          mbar_wait(full_bar(stage), phase, 3);
+          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + cw * 8192;
+          const uint32_t sw = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+          // K past the end of the segment is zero-filled by TMA, so the last k-block runs all four K steps too
+          wg_fence();
+          if (wkn) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (p.bias) {
-            if (full) {
-              const uint4* bp = reinterpret_cast<const uint4*>(p.bias + n);
+            for (int kk = 0; kk < 4; ++kk) gemm_wgmma<BN, 1>(acc, sdesc_k(sa, kk * 32), sdesc_mn(sw, kk * 2048, 8192), kk > 0 ? 1u : accumulate);
+          } else {
 #pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint4 u = __ldg(bp + q);
-                f[q * 8 + 0] += bf16_lo(u.x); f[q * 8 + 1] += bf16_hi(u.x);
-                f[q * 8 + 2] += bf16_lo(u.y); f[q * 8 + 3] += bf16_hi(u.y);
-                f[q * 8 + 4] += bf16_lo(u.z); f[q * 8 + 5] += bf16_hi(u.z);
-                f[q * 8 + 6] += bf16_lo(u.w); f[q * 8 + 7] += bf16_hi(u.w);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (n + j < p.N) f[j] += __bfloat162float(p.bias[n + j]);
-            }
+            for (int kk = 0; kk < 4; ++kk) gemm_wgmma<BN, 0>(acc, sdesc_k(sa, kk * 32), sdesc_k(sw, kk * 32), kk > 0 ? 1u : accumulate);
           }
-          if (row_ok) {
-            if (p.epi == EPI_GELU) {
-              if (xrow) {
-                if (full) {
-                  uint4* xp = reinterpret_cast<uint4*>(xrow + n);
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) {
-                    uint4 u;
-                    u.x = pack_bf16x2(f[q * 8 + 0], f[q * 8 + 1]);
-                    u.y = pack_bf16x2(f[q * 8 + 2], f[q * 8 + 3]);
-                    u.z = pack_bf16x2(f[q * 8 + 4], f[q * 8 + 5]);
-                    u.w = pack_bf16x2(f[q * 8 + 6], f[q * 8 + 7]);
-                    xp[q] = u;
-                  }
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j)
-                    if (n + j < p.N) xrow[n + j] = __float2bfloat16(f[j]);
-                }
-              }
-              // the activation sees the bf16-rounded pre-activation, as the reference's
-              // nn.Linear -> nn.GELU chain does (bf16 tensor between the two modules)
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = gelu_tanh(__bfloat162float(__float2bfloat16(f[j])));
-            } else if (p.epi == EPI_GATE_RES) {
-              float g[32], r[32];
-              if (full) {
-                const uint4* gp = reinterpret_cast<const uint4*>(grow + n);
-                const uint4* rp = reinterpret_cast<const uint4*>(rrow + n);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  uint4 u = __ldg(gp + q);
-                  g[q * 8 + 0] = bf16_lo(u.x); g[q * 8 + 1] = bf16_hi(u.x);
-                  g[q * 8 + 2] = bf16_lo(u.y); g[q * 8 + 3] = bf16_hi(u.y);
-                  g[q * 8 + 4] = bf16_lo(u.z); g[q * 8 + 5] = bf16_hi(u.z);
-                  g[q * 8 + 6] = bf16_lo(u.w); g[q * 8 + 7] = bf16_hi(u.w);
-                  uint4 w = rp[q];
-                  r[q * 8 + 0] = bf16_lo(w.x); r[q * 8 + 1] = bf16_hi(w.x);
-                  r[q * 8 + 2] = bf16_lo(w.y); r[q * 8 + 3] = bf16_hi(w.y);
-                  r[q * 8 + 4] = bf16_lo(w.z); r[q * 8 + 5] = bf16_hi(w.z);
-                  r[q * 8 + 6] = bf16_lo(w.w); r[q * 8 + 7] = bf16_hi(w.w);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  g[j] = (n + j < p.N) ? __bfloat162float(grow[n + j]) : 0.f;
-                  r[j] = (n + j < p.N) ? __bfloat162float(rrow[n + j]) : 0.f;
-                }
-              }
-              // reference order: bias -> (bf16 linear output) -> gate * y -> residual + (...)
-              // (flux/transformer.py:464-465, 584-586, 652-653); each step is a bf16 tensor there.
-              if (xrow) {   // full fine-tune: keep the (bf16) linear output — the gate gradient is sum_s dOut * y
-                if (full) {
-                  uint4* xp = reinterpret_cast<uint4*>(xrow + n);
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) {
-                    uint4 u;
-                    u.x = pack_bf16x2(f[q * 8 + 0], f[q * 8 + 1]);
-                    u.y = pack_bf16x2(f[q * 8 + 2], f[q * 8 + 3]);
-                    u.z = pack_bf16x2(f[q * 8 + 4], f[q * 8 + 5]);
-                    u.w = pack_bf16x2(f[q * 8 + 6], f[q * 8 + 7]);
-                    xp[q] = u;
-                  }
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j)
-                    if (n + j < p.N) xrow[n + j] = __float2bfloat16(f[j]);
-                }
-              }
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                float y = __bfloat162float(__float2bfloat16(f[j]));
-                float gy = __bfloat162float(__float2bfloat16(g[j] * y));
-                float o = r[j] + gy;
-                if (p.nan_to_num) {
-                  o = __bfloat162float(__float2bfloat16(o));
-                  if (o != o) o = 0.f;
-                  else if (o == INFINITY) o = 65504.f;
-                  else if (o == -INFINITY) o = -65504.f;
-                }
-                f[j] = o;
-              }
-            } else if (p.epi == EPI_MUL_DGELU) {
-              if (full) {
-                const uint4* xp = reinterpret_cast<const uint4*>(xrow + n);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  uint4 u = xp[q];
-                  f[q * 8 + 0] *= gelu_tanh_grad(bf16_lo(u.x)); f[q * 8 + 1] *= gelu_tanh_grad(bf16_hi(u.x));
-                  f[q * 8 + 2] *= gelu_tanh_grad(bf16_lo(u.y)); f[q * 8 + 3] *= gelu_tanh_grad(bf16_hi(u.y));
-                  f[q * 8 + 4] *= gelu_tanh_grad(bf16_lo(u.z)); f[q * 8 + 5] *= gelu_tanh_grad(bf16_hi(u.z));
-                  f[q * 8 + 6] *= gelu_tanh_grad(bf16_lo(u.w)); f[q * 8 + 7] *= gelu_tanh_grad(bf16_hi(u.w));
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (n + j < p.N) f[j] *= gelu_tanh_grad(__bfloat162float(xrow[n + j]));
-              }
-            } else if (p.epi == EPI_MUL) {
-              if (full) {
-                const uint4* xp = reinterpret_cast<const uint4*>(xrow + n);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  uint4 u = xp[q];
-                  f[q * 8 + 0] = gemm_bf16r(f[q * 8 + 0]) * bf16_lo(u.x); f[q * 8 + 1] = gemm_bf16r(f[q * 8 + 1]) * bf16_hi(u.x);
-                  f[q * 8 + 2] = gemm_bf16r(f[q * 8 + 2]) * bf16_lo(u.y); f[q * 8 + 3] = gemm_bf16r(f[q * 8 + 3]) * bf16_hi(u.y);
-                  f[q * 8 + 4] = gemm_bf16r(f[q * 8 + 4]) * bf16_lo(u.z); f[q * 8 + 5] = gemm_bf16r(f[q * 8 + 5]) * bf16_hi(u.z);
-                  f[q * 8 + 6] = gemm_bf16r(f[q * 8 + 6]) * bf16_lo(u.w); f[q * 8 + 7] = gemm_bf16r(f[q * 8 + 7]) * bf16_hi(u.w);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (n + j < p.N) f[j] = gemm_bf16r(f[j]) * __bfloat162float(xrow[n + j]);
-              }
-            } else if (p.epi == EPI_QUICK_GELU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const float y = gemm_bf16r(f[j]);
-                f[j] = y / (1.f + __expf(-1.702f * y));
-              }
-            } else if (p.epi == EPI_ADD_RES) {
-              if (full) {
-                const uint4* rp = reinterpret_cast<const uint4*>(rrow + n);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  uint4 w = rp[q];
-                  f[q * 8 + 0] += bf16_lo(w.x); f[q * 8 + 1] += bf16_hi(w.x);
-                  f[q * 8 + 2] += bf16_lo(w.y); f[q * 8 + 3] += bf16_hi(w.y);
-                  f[q * 8 + 4] += bf16_lo(w.z); f[q * 8 + 5] += bf16_hi(w.z);
-                  f[q * 8 + 6] += bf16_lo(w.w); f[q * 8 + 7] += bf16_hi(w.w);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (n + j < p.N) f[j] += __bfloat162float(rrow[n + j]);
-              }
-            }
-            if (full) {
-              uint4* dp = reinterpret_cast<uint4*>(drow + n);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint4 u;
-                u.x = pack_bf16x2(f[q * 8 + 0], f[q * 8 + 1]);
-                u.y = pack_bf16x2(f[q * 8 + 2], f[q * 8 + 3]);
-                u.z = pack_bf16x2(f[q * 8 + 4], f[q * 8 + 5]);
-                u.w = pack_bf16x2(f[q * 8 + 6], f[q * 8 + 7]);
-                dp[q] = u;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (n + j < p.N) drow[n + j] = __float2bfloat16(f[j]);
-            }
+          accumulate = 1;
+          wg_commit();
+          // keep one k-block in flight; the one before it has retired -> free its slot
+          wg_wait<1>();
+          wg_fence_regs(acc);
+          if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+          prev_stage = stage;
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1u;
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_remote(acce_bar(acc), 0u); else mbar_arrive(acce_bar(acc));
-      }
-      if (++acc == ACC_STAGES) {
-        acc = 0;
-        acc_phase ^= 1u;
+      wg_wait<0>();
+      wg_fence_regs(acc);
+      if (lane == 0) mbar_arrive(empty_bar(prev_stage));
+
+      // ===================== epilogue from registers =====================
+      // accumulator layout (m64nBN): acc[4 i + 2 h + j] = row 16 wq + lane / 4 + 8 h, column 8 i + 2 (lane % 4) + j
+      const int r_lo = s0 + wq * 16 + (lane >> 2);
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int n = n0 + 8 * i + 2 * (lane & 3);
+        if (n < p.N) {
+          const bool two = n + 1 < p.N;
+          float b0 = 0.f, b1 = 0.f;
+          if (p.bias) ld_bf16x2(p.bias + n, two, b0, b1);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int s = r_lo + 8 * h;
+            if (s < p.rows_per_batch && b < p.num_batches)
+              gemm_epi_pair(p, b, s, n, two, acc[4 * i + 2 * h] + b0, acc[4 * i + 2 * h + 1] + b1);
+          }
+        }
       }
     }
-  }
-
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();   // pair: the peer may still touch our smem / barriers / TMEM
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc2(tmem_base, Cfg::TMEM_COLS); else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 

@@ -1,5 +1,5 @@
-// simpletuner_b200 — non-GEMM kernels of the VAE latent-encode path (AutoencoderKL encoder), sm_100a.
-// Activations are NHWC bf16 so that every 3x3 / 1x1 conv is a tcgen05 GEMM over pixels
+// simpletuner_b200 — non-GEMM kernels of the VAE latent-encode path (AutoencoderKL encoder), sm_90a.
+// Activations are NHWC bf16 so that every 3x3 / 1x1 conv is a wgmma GEMM over pixels
 // (gemm.cuh, CONV mode: 9 shifted K-segments whose halo TMA zero-fills).  Here: the HBM-bound pieces.
 //   conv_in_3ch_kernel     : 3 -> C conv3x3 on the NCHW pixel tensor (K = 27: CUDA cores), writes NHWC
 //   groupnorm_stats_kernel : per (image, group) sum / sum-of-squares over H*W*(C/G)   (fp32 atomics)
@@ -59,46 +59,29 @@ conv_in_3ch_kernel(const __nv_bfloat16* __restrict__ px, const __nv_bfloat16* __
 }
 
 // Tensor-core version of the RGB stem conv: per 128-pixel tile an im2col A tile [128 px x 32] (k = (c, dy, dx): 27
-// taps + 5 zeros) is built in shared memory in the SWIZZLE_128B K-major layout the UMMA descriptors expect, the padded
-// weights [C x 32] sit next to it, and two K = 16 tcgen05 MMAs produce the [128 x C] outputs in TMEM.
-// Persistent CTAs; A tiles and accumulators are double-buffered so building tile i+1 overlaps the MMA / drain of tile i.
-// warps 0-3: build A row (thread = pixel = TMEM lane) + epilogue; warp 4: MMA issuer; warp 5: TMEM allocator.
+// taps + 5 zeros) is built in shared memory in the SWIZZLE_128B K-major layout the wgmma descriptors expect, the padded
+// weights [C x 32] sit next to it, and two K = 16 wgmma produce the [128 x C] outputs in registers.
+// Persistent CTAs of two warpgroups; warpgroup w builds and multiplies pixels [64 w, 64 w + 64) of each tile.
 __device__ __forceinline__ uint32_t sw128_row_chunk(uint32_t tile, int row, int chunk) {
   return tile + uint32_t(row >> 3) * 1024u + uint32_t(row & 7) * 128u + uint32_t((chunk ^ (row & 7)) << 4);
 }
 
-__global__ void __launch_bounds__(192, 1)
+template <int C>
+__global__ void __launch_bounds__(256, 1)
 conv_in_3ch_mma_kernel(const __nv_bfloat16* __restrict__ px, const __nv_bfloat16* __restrict__ w,
-                       const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ out, int B, int H, int W, int C) {
+                       const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ out, int B, int H, int W) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w_smem = base;                       // [256 rows x 128 B]
-  auto a_smem = [&](int u) { return base + 32768u + uint32_t(u) * 16384u; };
-  const uint32_t bar_base = base + 65536u;
-  auto a_full = [&](int u) { return bar_base + 8u * u; };
-  auto acc_full = [&](int u) { return bar_base + 8u * (2 + u); };
-  auto acc_empty = [&](int u) { return bar_base + 8u * (4 + u); };
-  const uint32_t tmem_slot = bar_base + 48u;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t w_smem = base;                       // [C rows x 128 B]
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const uint32_t a_smem = base + 32768u + uint32_t(wg) * 8192u;   // [64 rows x 128 B] per warpgroup
+  const int warp = t >> 5, lane = t & 31;
   const int tiles_x = (W + 127) / 128;
   const long long num_tiles = (long long)B * H * tiles_x;
 
-  if (threadIdx.x == 0) {
-    for (int u = 0; u < 2; ++u) {
-      mbar_init(a_full(u), 128);
-      mbar_init(acc_full(u), 1);
-      mbar_init(acc_empty(u), 4);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 5) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  // weights: row t = output channel, 27 taps then zeros up to k = 32, swizzled like a TMA box would be
-  for (int t = threadIdx.x; t < C; t += blockDim.x) {
-    const unsigned short* wr = reinterpret_cast<const unsigned short*>(w) + t * 27;
+  // weights: row = output channel, 27 taps then zeros up to k = 32, swizzled like a TMA box would be
+  for (int o = threadIdx.x; o < C; o += blockDim.x) {
+    const unsigned short* wr = reinterpret_cast<const unsigned short*>(w) + o * 27;
     uint32_t v[16];
 #pragma unroll
     for (int k = 0; k < 32; k += 2) {
@@ -107,58 +90,20 @@ conv_in_3ch_mma_kernel(const __nv_bfloat16* __restrict__ px, const __nv_bfloat16
     }
 #pragma unroll
     for (int c4 = 0; c4 < 4; ++c4)
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sw128_row_chunk(w_smem, t, c4)), "r"(v[c4 * 4 + 0]),
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sw128_row_chunk(w_smem, o, c4)), "r"(v[c4 * 4 + 0]),
                    "r"(v[c4 * 4 + 1]), "r"(v[c4 * 4 + 2]), "r"(v[c4 * 4 + 3]) : "memory");
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp < 4) {
-    const int r = threadIdx.x;   // pixel within the tile == TMEM lane
-    const uint32_t lane_off = uint32_t(warp * 32) << 16;
-    auto drain = [&](long long tile, int it) {
-      const int u = it & 1;
-      mbar_wait(acc_full(u), (it >> 1) & 1, 61);
-      tc_fence_after();
-      const int tx = int(tile % tiles_x);
-      const long long row = tile / tiles_x;          // b * H + y
-      const int x = tx * 128 + r;
-      __nv_bfloat16* orow = out + (row * W + x) * C;
-#pragma unroll 1
-      for (int c = 0; c < C; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + u * 256 + c, v);
-        tc_wait_ld();
-        if (x < W) {
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            if (c + q4 * 8 < C) {
-              float bv[8], o[8];
-              unpack8(__ldg(reinterpret_cast<const uint4*>(bias + c) + q4), bv);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) o[i] = __uint_as_float(v[q4 * 8 + i]) + bv[i];
-              reinterpret_cast<uint4*>(orow + c)[q4] = pack8(o);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty(u));
-    };
-    int it = 0;
-    long long prev = -1;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int u = it & 1;
-      // A[u] was last read by the MMAs of tile it-2, whose accumulator this thread drained already (program order)
-      const int tx = int(tile % tiles_x);
-      const long long row = tile / tiles_x;
-      const int y = int(row % H);
-      const int b = int(row / H);
-      const int x = tx * 128 + r;
+  float acc[C / 2];
+  for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int tx = int(tile % tiles_x);
+    const long long row = tile / tiles_x;   // b * H + y
+    const int y = int(row % H);
+    const int b = int(row / H);
+    if (t < 64) {
+      const int x = tx * 128 + wg * 64 + t;
       uint32_t pk[16];
 #pragma unroll
       for (int k = 0; k < 32; k += 2) {
@@ -178,36 +123,36 @@ conv_in_3ch_mma_kernel(const __nv_bfloat16* __restrict__ px, const __nv_bfloat16
       }
 #pragma unroll
       for (int c4 = 0; c4 < 4; ++c4)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sw128_row_chunk(a_smem(u), r, c4)), "r"(pk[c4 * 4 + 0]),
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sw128_row_chunk(a_smem, t, c4)), "r"(pk[c4 * 4 + 0]),
                      "r"(pk[c4 * 4 + 1]), "r"(pk[c4 * 4 + 2]), "r"(pk[c4 * 4 + 3]) : "memory");
       fence_proxy_async_smem();
-      mbar_arrive(a_full(u));
-      if (prev >= 0) drain(prev, it - 1);
-      prev = tile;
     }
-    if (prev >= 0) drain(prev, it - 1);
-  } else if (warp == 4) {
-    const uint32_t idesc = make_idesc_bf16(128, C, 0, 0);
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int u = it & 1;
-      mbar_wait(acc_empty(u), ((it >> 1) & 1) ^ 1u, 62);
-      mbar_wait(a_full(u), (it >> 1) & 1, 63);
-      tc_fence_after();
-      if (elect_one()) {
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk)
-          mma_ss(tmem_base + u * 256, sdesc_k(a_smem(u), kk * 32), sdesc_k(w_smem, kk * 32), idesc, kk > 0);
-        tc_commit(acc_full(u));
-      }
-      __syncwarp();
+    for (int kk = 0; kk < 2; ++kk) {
+      if constexpr (C == 256) wgmma_ss_n256<0, 0>(acc, sdesc_k(a_smem, kk * 32), sdesc_k(w_smem, kk * 32), kk > 0 ? 1u : 0u);
+      else if constexpr (C == 128) wgmma_ss_n128<0, 0>(acc, sdesc_k(a_smem, kk * 32), sdesc_k(w_smem, kk * 32), kk > 0 ? 1u : 0u);
+      else wgmma_ss_n64<0, 0>(acc, sdesc_k(a_smem, kk * 32), sdesc_k(w_smem, kk * 32), kk > 0 ? 1u : 0u);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    // every warp of the warpgroup is past its MMAs before the A rows are rebuilt for the next tile
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    // acc[4 i + 2 hh + e] = pixel 16 warp + lane / 4 + 8 hh of this warpgroup, channel 8 i + 2 (lane % 4) + e
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int x = tx * 128 + wg * 64 + warp * 16 + (lane >> 2) + 8 * hh;
+      if (x >= W) continue;
+      __nv_bfloat16* orow = out + (row * W + x) * C;
+#pragma unroll
+      for (int i = 0; i < C / 8; ++i) {
+        const int c = 8 * i + 2 * (lane & 3);
+        const uint32_t bv = __ldg(reinterpret_cast<const uint32_t*>(bias + c));
+        *reinterpret_cast<uint32_t*>(orow + c) = pack_bf16x2(acc[4 * i + 2 * hh] + bf16_lo(bv), acc[4 * i + 2 * hh + 1] + bf16_hi(bv));
+      }
+    }
   }
 }
 

@@ -1,16 +1,18 @@
-// simpletuner_b200 — "TN over rows" tcgen05 GEMM for weight gradients, sm_100a.
+// simpletuner_b200 — "TN over rows" wgmma GEMM for weight gradients, sm_90a.
 //
 //   out[r, n] += alpha * sum_{b,s}  L[b, s, r] * Rm[b, s, n]          (fp32 out, atomics across row splits)
 //
 // Both operands are contracted over their SLOW dimension (the token rows), i.e. both are MN-major
-// for the tensor core: A = Rm^T tile [128 n x 64 rows], B = L^T tile [R x 64 rows], D^T[n, r] in TMEM.
+// for the tensor core: A = Rm^T tile [128 n x 64 rows], B = L^T tile [RN x 64 rows], D^T[n, r] in registers
+// (RN = the rank block rounded up to 64; TMA zero-fills the columns past R).
 // Used for the LoRA weight gradients (autograd of peft lora.Linear, reference common.py:1094-1117):
 //   dA = (dY B)^T X      -> L = dY B [M, r],   Rm = X  [M, K]
 //   dB^T = (X A^T)^T dY  -> L = X A^T [M, r],  Rm = dY [M, N]
 // HBM-bound (reads Rm once); grid = n-tiles x row-splits so that ~all SMs stream concurrently.
-// Roles (256 threads): warp0 TMA producer, warp1 MMA issuer, warp2 TMEM alloc, warps 4-7 epilogue.
+// Roles (384 threads): warpgroup 0 TMA producer, warpgroups 1-2 wgmma + epilogue (64 n each).
 #pragma once
 #include "common.cuh"
+#include "wgrad_full.cuh"
 
 namespace stb {
 
@@ -29,21 +31,19 @@ struct WgradMaps {
   CUtensorMap l;   // 3-D (r, s, b) box (64, 64, 1) SWIZZLE_128B
 };
 
-template <int RP>
+template <int RN>
 struct WgradCfg {
-  static constexpr int R_ATOMS = (RP + 63) / 64;          // [64 rows x 64 r] boxes of the L operand
   static constexpr int A_BYTES = 2 * 8192;                // two [64 rows x 64 n] atoms
-  static constexpr int B_BYTES = 8192 * R_ATOMS;
+  static constexpr int B_BYTES = 8192 * (RN / 64);
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = 6;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-  static constexpr int TMEM_COLS = RP <= 32 ? 32 : (RP <= 64 ? 64 : 128);
 };
 
-template <int RP>  // padded rank block: multiple of 16, <= 128
-__global__ void __launch_bounds__(256, 1)
+template <int RN>  // rank block rounded up to 64 (64 or 128)
+__global__ void __launch_bounds__(384, 1)
 wgrad_tn_kernel(const __grid_constant__ WgradMaps maps, const WgradParams p) {
-  using Cfg = WgradCfg<RP>;
+  using Cfg = WgradCfg<RN>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int A_BYTES = Cfg::A_BYTES;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
@@ -53,13 +53,10 @@ wgrad_tn_kernel(const __grid_constant__ WgradMaps maps, const WgradParams p) {
   const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t acc_bar = bar_base + 8u * (2 * STAGES);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 1);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
   const int n0 = blockIdx.x * 128;
   const int b = blockIdx.y / p.splits_per_batch;
   const int s_begin = (blockIdx.y % p.splits_per_batch) * p.rows_per_split;
@@ -67,29 +64,20 @@ wgrad_tn_kernel(const __grid_constant__ WgradMaps maps, const WgradParams p) {
   const int kblocks = (s_end - s_begin + 63) / 64;
   if (kblocks <= 0) return;  // uniform per CTA
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.rm);
     tma_prefetch_desc(&maps.l);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);
     }
-    mbar_init(acc_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
-    {
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (warp == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = 0; kb < kblocks; ++kb) {
@@ -101,8 +89,7 @@ wgrad_tn_kernel(const __grid_constant__ WgradMaps maps, const WgradParams p) {
           tma_load_3d(sa, &maps.rm, full_bar(stage), n0, s, b);
           tma_load_3d(sa + 8192, &maps.rm, full_bar(stage), n0 + 64, s, b);
 #pragma unroll
-          for (int ra = 0; ra < Cfg::R_ATOMS; ++ra)
-            tma_load_3d(sa + A_BYTES + ra * 8192, &maps.l, full_bar(stage), ra * 64, s, b);
+          for (int ra = 0; ra < RN / 64; ++ra) tma_load_3d(sa + A_BYTES + ra * 8192, &maps.l, full_bar(stage), ra * 64, s, b);
         }
         __syncwarp();
         if (++stage == STAGES) {
@@ -111,66 +98,54 @@ wgrad_tn_kernel(const __grid_constant__ WgradMaps maps, const WgradParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(128, RP, 1, 1);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t accumulate = 0;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(full_bar(stage), phase, 61);
-        tc_fence_after();
-        const uint32_t sa = smem_base + stage * STAGE_BYTES;
-        // rows beyond s_end inside the last block belong to the next split: skip whole 16-row MMAs that
-        // start past the end; partial 16-row groups cannot occur because rows_per_split % 64 == 0 and rows
-        // >= S are zero-filled by TMA.
-        const int rows_here = min(64, s_end - (s_begin + kb * 64));
-        const int nk = (rows_here + 15) / 16;
-        if (elect_one()) {
-          for (int kk = 0; kk < nk; ++kk) {
-            const uint64_t ad = sdesc_mn(sa, kk * 2048, 8192);
-            const uint64_t bd = sdesc_mn(sa, A_BYTES + kk * 2048, 8192);
-            mma_ss(tmem_base, ad, bd, idesc, accumulate);
-            accumulate = 1;
-          }
-          tc_commit(empty_bar(stage));
-        }
-        __syncwarp();
+  } else {
+    reg_alloc<232>();
+    const int cw = wg - 1, wq = warp & 3;
+    float acc[RN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t accumulate = 0;
+    int prev_stage = -1;
+    for (int kb = 0; kb < kblocks; ++kb) {
+      mbar_wait(full_bar(stage), phase, 61);
+      const uint32_t sa = smem_base + stage * STAGE_BYTES;
+      // a block never reaches into the next split (rows_per_split % 64 == 0); rows >= S are zero-filled by TMA
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        wgmma_mn_mn<RN>(acc, sdesc_mn(sa + cw * 8192, kk * 2048, 8192), sdesc_mn(sa + A_BYTES, kk * 2048, 8192), accumulate);
         accumulate = 1;
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
       }
-      if (elect_one()) tc_commit(acc_bar);
-      __syncwarp();
+      wg_commit();
+      wg_wait<1>();
+      wg_fence_regs(acc);
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+      prev_stage = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
     }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    mbar_wait(acc_bar, 0, 62);
-    tc_fence_after();
-    const int n = n0 + ew * 32 + lane;
-    const uint32_t t_row = tmem_base + (uint32_t(ew * 32) << 16);
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    // acc[4 i + 2 hh + e] = D^T row n_lo + 8 hh (an n), column 8 i + 2 (lane % 4) + e (an r)
+    const int n_lo = n0 + cw * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-    for (int c = 0; c < RP; c += 16) {
-      uint32_t v[16];
-      tmem_ld_32x32b_x16(t_row + c, v);
-      tc_wait_ld();
-      if (n < p.N) {
+    for (int hh = 0; hh < 2; ++hh) {
+      const int n = n_lo + 8 * hh;
+      if (n >= p.N) continue;
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (c + j < p.R) {
-            if (p.partial) p.partial[((long long)blockIdx.y * p.R + (c + j)) * p.N + n] = __uint_as_float(v[j]);
-            else atomicAdd(p.out + (long long)(c + j) * p.N + n, p.alpha * __uint_as_float(v[j]));
+      for (int i = 0; i < RN / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = 8 * i + 2 * (lane & 3) + e;
+          if (r < p.R) {
+            const float v = acc[4 * i + 2 * hh + e];
+            if (p.partial) p.partial[((long long)blockIdx.y * p.R + r) * p.N + n] = v;
+            else atomicAdd(p.out + (long long)r * p.N + n, p.alpha * v);
           }
-      }
+        }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 

@@ -1,21 +1,21 @@
-// simpletuner_b200 — full-rank weight gradient GEMM on tcgen05, sm_100a (round 2: full fine-tune, BASELINE config 3).
+// simpletuner_b200 — full-rank weight gradient GEMM on wgmma, sm_90a (full fine-tune, BASELINE config 3).
 //
-//   dW[n, k] = alpha * sum_{b,s} dY[b, s, n] * X[b, s, k]   (+ dW_old[n, k])        bf16 out, fp32 accumulation in TMEM
+//   dW[n, k] = alpha * sum_{b,s} dY[b, s, n] * X[b, s, k]   (+ dW_old[n, k])        bf16 out, fp32 accumulation
 //
 // This is the autograd of every nn.Linear weight the reference trains when `model_type=full`
 // (reference trainer.py:7126 `accelerator.backward`; SD3 blocks sd3/transformer.py:145-241).  Both operands are contracted
 // over their SLOW dimension (the token rows), so both are MN-major for the tensor core — the layout of wgrad.cuh (the
 // rank-r LoRA version), generalised to a persistent, tiled kernel:
-//   A = dY^T tile [128 n x 64 tokens]  (two   [64 tokens x 64 n] SWIZZLE_128B boxes)
-//   B = X^T  tile [BN  k x 64 tokens]  (BN/64 [64 tokens x 64 k] boxes),  D tile [128 x BN] fp32 in TMEM,
+//   A = dY^T tile [128 n x 64 tokens]  (two   [64 tokens x 64 n] SWIZZLE_128B boxes, one per consumer warpgroup)
+//   B = X^T  tile [BN  k x 64 tokens]  (BN/64 [64 tokens x 64 k] boxes),  D tile [128 x BN] fp32 in registers,
 // k-blocks run over (batch, 64-token chunk); rows past the end of a batch slab are zero-filled by TMA, so ragged
 // sequences and strided [B, S, N] views (a row range of the joint hidden buffer) need no copies.
-// Roles (256 threads): warp0 TMA producer, warp1 MMA issuer, warp2 TMEM alloc, warps 4-7 epilogue; TMEM holds two
-// accumulator stages so the bf16 store of tile i overlaps the mainloop of tile i+1.
+// Roles (384 threads): warpgroup 0 TMA producer, warpgroups 1-2 wgmma + epilogue (64 n-rows each).
 // Algorithmic work: 2 * M * N * K flops (M = B*S tokens) — the same as the forward GEMM of that layer.
 #pragma once
 #include "common.cuh"
 #include "elementwise.cuh"
+#include "gemm.cuh"
 
 namespace stb {
 
@@ -38,15 +38,22 @@ struct WgradFullCfg {
   static constexpr int B_BYTES = (BN / 64) * 8192;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int ACC_STAGES = 512 / BN >= 2 ? 2 : 1;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
+// D (64 x N) += A^T B over 16 token rows, both operands MN-major
+template <int N>
+__device__ __forceinline__ void wgmma_mn_mn(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (N == 256) wgmma_ss_n256<1, 1>(d, a, b, accumulate);
+  else if constexpr (N == 128) wgmma_ss_n128<1, 1>(d, a, b, accumulate);
+  else wgmma_ss_n64<1, 1>(d, a, b, accumulate);
+}
+
 template <int BN>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 wgrad_full_kernel(const __grid_constant__ WgradFullMaps maps, const WgradFullParams p) {
   using Cfg = WgradFullCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES, ACC_STAGES = Cfg::ACC_STAGES;
+  constexpr int STAGES = Cfg::STAGES;
   constexpr int A_BYTES = Cfg::A_BYTES, STAGE_BYTES = Cfg::STAGE_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
@@ -54,168 +61,112 @@ wgrad_full_kernel(const __grid_constant__ WgradFullMaps maps, const WgradFullPar
   const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto accf_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto acce_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + ACC_STAGES + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 2 * ACC_STAGES);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
   const int tiles_n = (p.N + 127) / 128;
   const int tiles_k = (p.K + BN - 1) / BN;
   const int num_tiles = tiles_n * tiles_k;
   const int chunks = (p.S + 63) / 64;       // 64-token chunks per batch slab
   const int kblocks = chunks * p.B;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.dy);
     tma_prefetch_desc(&maps.x);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < ACC_STAGES; ++s) {
-      mbar_init(accf_bar(s), 1);
-      mbar_init(acce_bar(s), 4);
+      mbar_init(empty_bar(s), 8);
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (warp == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        // k-tile fastest: CTAs running side by side share the dY columns (A) of one n-tile through L2
+        const int tn = tile / tiles_k, tk = tile - tn * tiles_k;
+        const int n0 = tn * 128, k0 = tk * BN;
+        for (int kb = 0; kb < kblocks; ++kb) {
+          const int b = kb / chunks, s = (kb - b * chunks) * 64;
+          mbar_wait(empty_bar(stage), phase ^ 1u, 80);
+          const uint32_t sa = smem_base + stage * STAGE_BYTES;
+          if (elect_one()) {
+            mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
+            tma_load_3d(sa, &maps.dy, full_bar(stage), n0, s, b);
+            tma_load_3d(sa + 8192, &maps.dy, full_bar(stage), n0 + 64, s, b);
+#pragma unroll
+            for (int a = 0; a < BN / 64; ++a) tma_load_3d(sa + A_BYTES + a * 8192, &maps.x, full_bar(stage), k0 + a * 64, s, b);
+          }
+          __syncwarp();
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+    }
+  } else {
+    reg_alloc<232>();
+    const int cw = wg - 1, wq = warp & 3;
+    float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      // k-tile fastest: CTAs running side by side share the dY columns (A) of one n-tile through L2
       const int tn = tile / tiles_k, tk = tile - tn * tiles_k;
-      const int n0 = tn * 128, k0 = tk * BN;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        const int b = kb / chunks, s = (kb - b * chunks) * 64;
-        mbar_wait(empty_bar(stage), phase ^ 1u, 80);
-        const uint32_t sa = smem_base + stage * STAGE_BYTES;
-        if (elect_one()) {
-          mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
-          tma_load_3d(sa, &maps.dy, full_bar(stage), n0, s, b);
-          tma_load_3d(sa + 8192, &maps.dy, full_bar(stage), n0 + 64, s, b);
-#pragma unroll
-          for (int a = 0; a < BN / 64; ++a) tma_load_3d(sa + A_BYTES + a * 8192, &maps.x, full_bar(stage), k0 + a * 64, s, b);
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, BN, 1, 1);
-    int stage = 0, acc = 0;
-    uint32_t phase = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(acce_bar(acc), acc_phase ^ 1u, 81);
-      tc_fence_after();
-      const uint32_t d_base = tmem_base + acc * BN;
+      const int k0 = tk * BN;
       uint32_t accumulate = 0;
+      int prev_stage = -1;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(full_bar(stage), phase, 82);
-        tc_fence_after();
         const uint32_t sa = smem_base + stage * STAGE_BYTES;
-        // tokens past the end of the slab are zeros (TMA fill): whole 16-token MMAs beyond it can be skipped
-        const int s = (kb % chunks) * 64;
-        const int nk = (min(64, p.S - s) + 15) / 16;
-        if (elect_one()) {
-          for (int kk = 0; kk < nk; ++kk) {
-            mma_ss(d_base, sdesc_mn(sa, kk * 2048, 8192), sdesc_mn(sa, A_BYTES + kk * 2048, 8192), idesc, accumulate);
-            accumulate = 1;
-          }
-          tc_commit(empty_bar(stage));
+        // tokens past the end of the slab are zeros (TMA fill), so a ragged last chunk runs all four K steps too
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          wgmma_mn_mn<BN>(acc, sdesc_mn(sa + cw * 8192, kk * 2048, 8192), sdesc_mn(sa + A_BYTES, kk * 2048, 8192), accumulate);
+          accumulate = 1;
         }
-        __syncwarp();
-        accumulate = 1;
+        wg_commit();
+        wg_wait<1>();
+        wg_fence_regs(acc);
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+        prev_stage = stage;
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1u;
         }
       }
-      if (elect_one()) tc_commit(accf_bar(acc));
-      __syncwarp();
-      if (++acc == ACC_STAGES) {
-        acc = 0;
-        acc_phase ^= 1u;
-      }
-    }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int tn = tile / tiles_k, tk = tile - tn * tiles_k;
-      const int n = tn * 128 + ew * 32 + lane;
-      const int k0 = tk * BN;
-      mbar_wait(accf_bar(acc), acc_phase, 83);
-      tc_fence_after();
-      __nv_bfloat16* orow = p.out + (long long)n * p.out_row_stride;
-      const uint32_t t_row = tmem_base + (uint32_t(ew * 32) << 16) + acc * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        if (k0 + c >= p.K) break;   // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(t_row + c, v);
-        tc_wait_ld();
-        if (n < p.N) {
-          const int k = k0 + c;
-          if (k + 32 <= p.K) {
-            uint4* dp = reinterpret_cast<uint4*>(orow + k);
+      wg_wait<0>();
+      wg_fence_regs(acc);
+      if (lane == 0) mbar_arrive(empty_bar(prev_stage));
+      // acc[4 i + 2 hh + e] = dW row n_lo + 8 hh, column k0 + 8 i + 2 (lane % 4) + e
+      const int n_lo = tn * 128 + cw * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              float f[8];
+      for (int hh = 0; hh < 2; ++hh) {
+        const int n = n_lo + 8 * hh;
+        if (n >= p.N) continue;
+        __nv_bfloat16* orow = p.out + (long long)n * p.out_row_stride;
 #pragma unroll
-              for (int j = 0; j < 8; ++j) f[j] = p.alpha * __uint_as_float(v[q * 8 + j]);
-              if (p.accumulate) {
-                const uint4 o = dp[q];
-                f[0] += bf16_lo(o.x); f[1] += bf16_hi(o.x); f[2] += bf16_lo(o.y); f[3] += bf16_hi(o.y);
-                f[4] += bf16_lo(o.z); f[5] += bf16_hi(o.z); f[6] += bf16_lo(o.w); f[7] += bf16_hi(o.w);
-              }
-              uint4 u;
-              u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
-              u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
-              dp[q] = u;
+        for (int i = 0; i < BN / 8; ++i) {
+          const int k = k0 + 8 * i + 2 * (lane & 3);
+          if (k < p.K) {   // K % 8 == 0: the pair is whole
+            float f0 = p.alpha * acc[4 * i + 2 * hh], f1 = p.alpha * acc[4 * i + 2 * hh + 1];
+            uint32_t* dp = reinterpret_cast<uint32_t*>(orow + k);
+            if (p.accumulate) {
+              const uint32_t o = *dp;
+              f0 += bf16_lo(o);
+              f1 += bf16_hi(o);
             }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (k + j < p.K) {
-                float f = p.alpha * __uint_as_float(v[j]);
-                if (p.accumulate) f += __bfloat162float(orow[k + j]);
-                orow[k + j] = __float2bfloat16(f);
-              }
+            *dp = pack_bf16x2(f0, f1);
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acce_bar(acc));
-      if (++acc == ACC_STAGES) {
-        acc = 0;
-        acc_phase ^= 1u;
-      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -30,8 +30,8 @@ from .. import ops
 
 EPS = 1e-6
 # Keep the post-norm / post-RoPE q, k of every block for the backward instead of re-running the RMSNorm + RoPE pass there:
-# +2 B S D bytes per block (Flux.1-dev, B = 4: +13 GB over 57 blocks, 100 -> 113 GB of 180 GB) for one HBM-bound kernel less
-# per block in backward.  STB_SAVE_QK=0 restores the recompute (larger batches / buckets).
+# +2 B S D bytes per block (Flux.1-dev: +3.2 GB per sample over 57 blocks) for one HBM-bound kernel less per block in
+# backward.  STB_SAVE_QK=0 restores the recompute (larger batches / buckets).
 import os as _os
 SAVE_QK = _os.environ.get("STB_SAVE_QK", "1") != "0"
 # The LayerNorm-modulated block input (the A operand of the q|k|v projections and of their adapters' weight gradients) is kept
@@ -163,7 +163,7 @@ def make_pack(params, n_out: int, k_in: int, scaling: float, device, lokr_scales
 
 
 def _lokr_grads(pack: LokrPack, x: torch.Tensor, dy: torch.Tensor):
-    """Factor gradients through delta W = kron(w1, w2) * scale: the full weight gradient of the group (one MN-major tcgen05
+    """Factor gradients through delta W = kron(w1, w2) * scale: the full weight gradient of the group (one MN-major wgmma
     GEMM, dy^T x), contracted per member against the other Kronecker factor."""
     from ..lycoris import lokr_factor_grads
     dW = ops.wgrad_full(dy, x)                       # [members * n_out, K] bf16
@@ -340,8 +340,8 @@ def _qk_fwd(qkv, D, H, hd, img_plan: AttnPlan, txt_plan: Optional[AttnPlan], S_t
 
 
 def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, sin, qk=None):
-    """Returns d_qkv [B, S, 3D] given d_o.  `qk` = the (q, k) pair saved by the forward (180 GB of HBM: spending 2 B S D
-    bytes per block is cheaper than re-running the RMSNorm + RoPE pass in backward); recomputed when absent."""
+    """Returns d_qkv [B, S, 3D] given d_o.  `qk` = the (q, k) pair saved by the forward (spending 2 B S D bytes per block
+    is cheaper than re-running the RMSNorm + RoPE pass in backward); recomputed when absent."""
     B, S, _ = qkv.shape
     q, k = qk if qk is not None else _qk_fwd(qkv, D, H, hd, img_plan, txt_plan, S_txt, cos, sin)
     v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
@@ -352,9 +352,8 @@ def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, s
                      dq=d_qkv[:, :, 0:D].unflatten(-1, (H, hd)), dk=d_qkv[:, :, D:2 * D].unflatten(-1, (H, hd)), dv=dv)
         return d_qkv
     # The backward of RMSNorm + RoPE stays a separate HBM-bound pass.  libstb200 can also run it inside the
-    # attention-backward epilogues (ops.attn_bwd(qk_prep=...), tests: attn_bwd_fused_prep*), but with one CTA per
-    # SM the longer, latency-bound epilogue is not overlapped by anything: measured +38 ms of attention backward
-    # against 14 ms saved per Flux step (profiles/r01/bench_n1_v4.json vs v3), so it is not used here.
+    # attention-backward epilogues (ops.attn_bwd(qk_prep=...), tests: attn_bwd_fused_prep*); the step keeps the separate
+    # pass because the longer epilogue of the fused form is not overlapped by anything (not measured on H100).
     dq = torch.empty_like(q)
     dk = torch.empty_like(k)
     ops.attn_bwd(q, k, v, o.view(B, S, H, hd), d_o.view(B, S, H, hd), lse, dq=dq, dk=dk, dv=dv)

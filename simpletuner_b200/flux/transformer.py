@@ -496,7 +496,8 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         """common.py:3550-3636 / flux/transformer.py:1240-1287: blocks selected by `gradient_checkpointing_interval`
         (every block when None) are re-run in backward instead of keeping their saved set (block input only is kept),
         through torch.utils.checkpoint like the reference.  Off by default: the block schedules already keep a minimal
-        activation set (100 GB at B = 4, 1024^2), so on a 180 GB B200 recompute only costs time."""
+        activation set; on an 80 GB H100 that holds one 1024^2 sample next to the Flux.1-dev weights, and larger batches need
+        recompute."""
         self.gradient_checkpointing = True
 
     def disable_gradient_checkpointing(self):

@@ -11,10 +11,10 @@ reference drives at simpletuner/helpers/training/trainer.py:3390-3505:
     for lora in net.loras: lora.lokr_w1, lora.lokr_w2, lora.org_weight  (helpers/training/peft_init.py:34-38)
 
 Algorithm (restated in oracle/lokr_oracle.py): delta W = kron(lokr_w1 [a, c], lokr_w2 [b, d]) * scale, forward
-y = linear(x, W + delta W * multiplier).  B200 mapping: the adapted weight IS rebuilt — once per optimizer step, straight into
+y = linear(x, W + delta W * multiplier).  Kernel mapping: the adapted weight IS rebuilt — once per optimizer step, straight into
 the fused / transposed projection layouts the block schedules read (flux/transformer.py `plans()`), so forward and dgrad are
-the plain tcgen05 GEMMs of the un-adapted model with no adapter work at all.  Backward forms the full weight gradient with the
-MN-major tcgen05 weight-gradient kernel (`stb_wgrad_full`, exactly what autograd computes through `torch.kron` in the
+the plain wgmma GEMMs of the un-adapted model with no adapter work at all.  Backward forms the full weight gradient with the
+MN-major wgmma weight-gradient kernel (`stb_wgrad_full`, exactly what autograd computes through `torch.kron` in the
 reference) and contracts it against the other Kronecker factor:
     d w1[i, k] = scale * sum_{j, l} dW[(i, j), (k, l)] w2[j, l];   d w2[j, l] = scale * sum_{i, k} dW[(i, j), (k, l)] w1[i, k].
 Unsupported LyCORIS options raise NotImplementedError (other algos, dropout / rank_dropout / module_dropout, bypass_mode,

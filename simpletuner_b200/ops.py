@@ -472,12 +472,16 @@ def colsum2(dy, z=None, want_sum: bool = True):
     return sm, dt
 
 
-DETERMINISTIC = os.environ.get("STB_DETERMINISTIC", "0") == "1"
+DETERMINISTIC = os.environ.get("STB_DETERMINISTIC", "1") != "0"
+# per (device, stream) reduction workspace.  A buffer that is outgrown is kept alive, never freed: a CUDA graph captured
+# while it was current still reads and writes it on replay, so its memory must not go back to an allocator pool.
 _ws_cache: dict = {}
+_ws_retired: list = []
 
 
 def set_deterministic(on: bool) -> None:
-    """LoRA weight gradients without floating-point atomics (slab partials + ordered reduction): bit-identical run to run."""
+    """LoRA weight gradients without floating-point atomics (slab partials + ordered reduction): bit-identical run to run.
+    On by default; off (or STB_DETERMINISTIC=0) accumulates the row splits with fp32 atomics instead."""
     global DETERMINISTIC
     DETERMINISTIC = bool(on)
 
@@ -496,6 +500,8 @@ def skinny_tn(L, Rm, alpha: float = 1.0, out: Optional[torch.Tensor] = None):
         key = (L.device.index, _stream())
         ws = _ws_cache.get(key)
         if ws is None or ws.numel() < need:
+            if ws is not None:
+                _ws_retired.append(ws)
             ws = _ws_cache[key] = torch.empty((need,), device=L.device, dtype=torch.float32)
         check(_lib.lib().stb_skinny_tn_ws(L3.data_ptr(), L3.stride(0), L3.stride(1), R3.data_ptr(), R3.stride(0), R3.stride(1),
                                           out.data_ptr(), B, S, R, N, alpha, ws.data_ptr(), ws.numel(), _stream()))

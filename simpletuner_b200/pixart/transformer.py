@@ -10,8 +10,8 @@ Same constructor arguments / `.config`, forward signature (`hidden_states [B,4,H
 Block schedule (reference :57-145 -> diffusers BasicTransformerBlock, norm_type="ada_norm_single"), one
 torch.autograd.Function per block, every arithmetic step a libstb200 kernel:
     mod = scale_shift_table + t           [B, 6D]
-    LN-modulate -> fused QKV GEMM (+LoRA K-segment) -> tcgen05 attention -> to_out GEMM, gate + residual epilogue
-    to_q GEMM | to_k,to_v GEMM on the projected caption -> tcgen05 cross attention -> to_out GEMM + residual epilogue
+    LN-modulate -> fused QKV GEMM (+LoRA K-segment) -> wgmma attention -> to_out GEMM, gate + residual epilogue
+    to_q GEMM | to_k,to_v GEMM on the projected caption -> wgmma cross attention -> to_out GEMM + residual epilogue
     LN-modulate -> FF GEMM (GELU epilogue) -> FF GEMM, gate + residual epilogue
 head_dim 72 is not an MMA-K multiple: the projection weights are zero-padded per head to 128 once (derived,
 frozen layouts), so q/k/v come out of the GEMM already in the [B,S,H,128] layout the attention kernel wants, the

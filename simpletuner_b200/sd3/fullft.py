@@ -5,7 +5,7 @@ Here EVERY parameter of the joint block receives its gradient — what `accelera
 diffusers' JointTransformerBlock in the reference (trainer.py:7126; sd3/transformer.py:145-241):
 
   * weights of the fused q|k|v projections, the output projections and both FeedForward linears: `ops.wgrad_full`
-    (tcgen05, both operands MN-major; csrc/wgrad_full.cuh) — dW = dY^T X over the token rows, 2 M N K flops each, i.e.
+    (wgmma, both operands MN-major; csrc/wgrad_full.cuh) — dW = dY^T X over the token rows, 2 M N K flops each, i.e.
     the full-FT step is 3x the forward's linear work (BASELINE.md 3: 6.8 TF per SD3.5-medium sample);
   * biases and the adaLN chunks (shift / scale / gate of norm1, norm1_context, the dual-attention norm): per-(batch, column)
     token reductions `ops.colsum2` (sum_s dy, sum_s dy * z with z = LayerNorm(x) or the gated linear output that the

@@ -1,4 +1,4 @@
-"""Seams B3 / B4: use only the tcgen05 attention under the unmodified diffusers model.
+"""Seams B3 / B4: use only the wgmma attention under the unmodified diffusers model.
 
 B4 — packed backend module.  The reference loads a module by name and calls whichever of these it exports
 (helpers/training/attention_backend.py:236-254, 405-411): `flash_attn_qkvpacked_func(qkv[B,S,3,H,D], dropout_p,

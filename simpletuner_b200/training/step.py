@@ -177,9 +177,6 @@ class GraphedTrainStep:
             raise NotImplementedError("GraphedTrainStep: lora_dropout > 0 draws a per-step host seed; run the eager TrainStep")
         if getattr(den, "_lycoris_network", None) is not None:
             raise NotImplementedError("GraphedTrainStep: LoKr rebuilds the projection layouts between steps; run the eager TrainStep")
-        from .. import ops
-        if ops.DETERMINISTIC:
-            raise NotImplementedError("GraphedTrainStep: deterministic mode keeps a reduction workspace outside the graph pool")
         self.step = step
         self.warmup = warmup
         self._graphs: Dict[Any, Any] = {}

@@ -7,7 +7,7 @@ what caching/vae.py:1331-1343 consumes; `encode_scaled(samples)` additionally fu
 `scale_vae_latents_for_cache` (foundation_mixins.py:68-81).  Parameter names follow the diffusers state_dict
 (`encoder.down_blocks.0.resnets.0.conv1.weight`, `encoder.mid_block.attentions.0.to_q.weight`, `quant_conv.weight` …).
 
-Layout: activations NHWC bf16.  Every 3x3 conv is the tcgen05 implicit-GEMM kernel (ops.conv3x3_nhwc; weights are
+Layout: activations NHWC bf16.  Every 3x3 conv is the wgmma implicit-GEMM kernel (ops.conv3x3_nhwc; weights are
 re-laid once to [C_out, (dy, dx, c_in)]); 1x1 shortcuts / attention projections are ops.gemm over pixels; the
 mid-block single-head attention (head_dim 512) runs as score GEMM -> row softmax -> PV GEMM per image; GroupNorm+SiLU
 is a two-kernel NHWC pass.  Inference only (the reference runs it under torch.no_grad).

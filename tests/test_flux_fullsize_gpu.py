@@ -20,6 +20,9 @@ def full():
     torch.manual_seed(0)
     dev = torch.device("cuda", 0)
     w = bench.build_model(dev, None, rank=16, seed=0)
+    # an 80 GB card does not hold the B = 4 backward at this size with every activation saved: keep them only at block
+    # boundaries (the reference's default gradient_checkpointing=true); the forward values are unchanged
+    w._denoiser().enable_gradient_checkpointing()
     batch = bench.synth_batch(4, dev, seed=7)
     return w, batch
 

@@ -11,21 +11,3 @@ def test_kernel(name):
     r = CHECKS[name]()
     assert r["ok"], r
 
-
-def test_pair_attention_forward_kernel_opt_in():
-    """The CTA-pair attention forward (STB_ATTN_FWD_PAIR=1, read once per process) against fp32 torch math."""
-    import json
-    import os
-    import subprocess
-    import sys
-    from pathlib import Path
-
-    root = Path(__file__).resolve().parent.parent
-    code = ("import json; from tests.kernel_checks import CHECKS; "
-            "names = ['attn_fwd_128', 'attn_fwd_256', 'attn_fwd_ragged', 'attn_fwd_strided', 'attn_fwd_long', 'attn_fwd_bigscore', "
-            "'attn_fwd_cross_300', 'attn_bwd_ragged']; print(json.dumps([CHECKS[n]() for n in names]))")
-    env = dict(os.environ, STB_ATTN_FWD_PAIR="1")
-    out = subprocess.run([sys.executable, "-c", code], cwd=str(root), env=env, capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    res = json.loads(out.stdout.strip().splitlines()[-1])
-    assert all(r["ok"] for r in res), res

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """libstb200 attention forward / backward next to torch's F.scaled_dot_product_attention (the kernel the reference's
 default `attention_mechanism="diffusers"` path calls, reference flux/transformer.py:200-207) on the same box, same
-shapes, CUDA events, SM clocks recorded.  Writes gpurun_out/attn_vs_sdpa.json (copy it to profiles/rNN/).
+shapes, CUDA events, SM clocks recorded.  Writes bench_out/attn_vs_sdpa.json.
 
   python tools/attn_vs_sdpa.py [tag]
 """
@@ -83,7 +83,7 @@ def main():
         except Exception as e:  # noqa
             res["shapes"].append({"shape": shp, "error": str(e)[:300]})
         print(json.dumps(res["shapes"][-1]), flush=True)
-    out = ROOT / "gpurun_out"
+    out = ROOT / "bench_out"
     out.mkdir(exist_ok=True)
     (out / f"attn_vs_sdpa_{tag}.json").write_text(json.dumps(res, indent=1))
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Kernel micro-benchmarks (CUDA events, rotating buffers larger than L2) -> gpurun_out/microbench.json."""
+"""Kernel micro-benchmarks (CUDA events, rotating buffers larger than L2) -> bench_out/microbench.json."""
 import json
 import sys
 import time
@@ -93,7 +93,7 @@ def main():
                 r = {"kind": "attn", "B": B, "H": H, "S": S, "error": str(e)[:200]}
             print(json.dumps(r), flush=True)
             res.append(r)
-    out = ROOT / "gpurun_out"
+    out = ROOT / "bench_out"
     out.mkdir(exist_ok=True)
     (out / f"microbench_{int(time.time())}.json").write_text(json.dumps(res, indent=1))
 

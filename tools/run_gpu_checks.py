@@ -3,7 +3,7 @@
 
 A worker process runs checks one after another and prints one JSON line per check; if a kernel
 traps (CUDA context dies) or a check hangs, the parent records it and restarts a worker on the
-remaining checks.  Results -> gpurun_out/kernel_checks.json.
+remaining checks.  Results -> bench_out/kernel_checks.json.
 """
 import json
 import os
@@ -95,7 +95,7 @@ def main():
             results.append(rec)
             print("CRASH " + json.dumps(rec), flush=True)
             remaining.pop(0)
-    out = ROOT / "gpurun_out"
+    out = ROOT / "bench_out"
     out.mkdir(exist_ok=True)
     (out / "kernel_checks.json").write_text(json.dumps(results, indent=1))
     npass = sum(1 for r in results if r.get("ok"))
