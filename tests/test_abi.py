@@ -30,6 +30,42 @@ def test_library_exports_every_declared_symbol():
     assert handle.stb_version() == 100
 
 
+# entry points that launch nothing: version, error text, launch counters, workspace size, optimizer chunk size
+_BOOKKEEPING = {"stb_version", "stb_last_error", "stb_launch_count", "stb_reset_launch_count", "stb_skinny_tn_workspace",
+                "stb_adamw_bf16_chunk"}
+# GPU tests outside the kernel_checks registry that compare a wrapper with a reference
+_GPU_TEST_FILES = ("test_adamw_bf16.py", "test_lora_dropout_gpu.py", "test_text_encoders.py")
+
+
+def _wrappers():
+    """{stb_* symbol: names of the top-level functions / classes of the Python layer whose body calls it}"""
+    import ast
+
+    found = {}
+    for rel in ("simpletuner_b200/ops.py", "simpletuner_b200/training/optim.py"):
+        for node in ast.parse((ROOT / rel).read_text()).body:
+            if isinstance(node, (ast.FunctionDef, ast.ClassDef)):
+                for sub in ast.walk(node):
+                    if isinstance(sub, ast.Attribute) and sub.attr.startswith("stb_"):
+                        found.setdefault(sub.attr, set()).add(node.name)
+    return found
+
+
+def test_every_kernel_entry_point_has_a_gpu_check():
+    """Each kernel entry point of include/stb200.h is reached by a wrapper that tests/kernel_checks.py or a named GPU test
+    calls, so a new kernel cannot land without an element-wise check."""
+    wrappers = _wrappers()
+    tests = ROOT / "tests"
+    texts = [(tests / "kernel_checks.py").read_text()] + [(tests / f).read_text() for f in _GPU_TEST_FILES]
+    unchecked = {}
+    for sym in sorted(set(_declared()) - _BOOKKEEPING):
+        names = wrappers.get(sym)
+        assert names, f"{sym} is declared in include/stb200.h but no Python wrapper calls it"
+        if not any(re.search(rf"\b{n}\s*\(", t) for n in names for t in texts):
+            unchecked[sym] = sorted(names)
+    assert not unchecked, f"entry points whose wrappers no GPU check calls: {unchecked}"
+
+
 def test_product_path_fails_loudly_without_cuda():
     from simpletuner_b200 import _lib, ops
 
