@@ -265,18 +265,18 @@ static int launch_attn_bwd(const stb_attn_bwd_args* a, const stb::AttnBwdMaps& m
         static_cast<const __nv_bfloat16*>(a->d_o), a->do_b, a->do_s, a->do_h, a->delta, a->B, a->H, a->Sq);
     STB_LAUNCH_CHECK("attn_bwd_delta");
   }
-  constexpr int SMEM = stb::AttnBwdCfg<HD>::SMEM_BYTES;
+  constexpr int SMEM1 = stb::AttnBwdCfg<HD>::DKDV_SMEM_BYTES, SMEM2 = stb::AttnBwdCfg<HD>::DQ_SMEM_BYTES;
   auto k1 = stb::attn_bwd_dkdv_kernel<HD>;
   auto k2 = stb::attn_bwd_dq_kernel<HD>;
   static bool configured = false;
   if (!configured) {
-    if (int r = set_smem(k1, SMEM)) return r;
-    if (int r = set_smem(k2, SMEM)) return r;
+    if (int r = set_smem(k1, SMEM1)) return r;
+    if (int r = set_smem(k2, SMEM2)) return r;
     configured = true;
   }
-  k1<<<dim3((a->Sk + 127) / 128, a->H, a->B), 384, SMEM, st>>>(maps, p);
+  k1<<<dim3((a->Sk + 63) / 64, a->H, a->B), 384, SMEM1, st>>>(maps, p);
   STB_LAUNCH_CHECK("attn_bwd_dkdv");
-  k2<<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM, st>>>(maps, p);
+  k2<<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM2, st>>>(maps, p);
   STB_LAUNCH_CHECK("attn_bwd_dq");
   return 0;
 }
@@ -413,8 +413,6 @@ int stb_attn_bwd(const stb_attn_bwd_args* a, void* stream) {
     return make_map(m, ptr, 4, d, s, bx);
   };
   if (int r = mk(&maps.q128, a->q, a->q_b, a->q_s, a->q_h, a->Sq, 128)) return r;
-  if (int r = mk(&maps.k128, a->k, a->k_b, a->k_s, a->k_h, a->Sk, 128)) return r;
-  if (int r = mk(&maps.v128, a->v, a->v_b, a->v_s, a->v_h, a->Sk, 128)) return r;
   if (int r = mk(&maps.do128, a->d_o, a->do_b, a->do_s, a->do_h, a->Sq, 128)) return r;
   if (int r = mk(&maps.q64, a->q, a->q_b, a->q_s, a->q_h, a->Sq, 64)) return r;
   if (int r = mk(&maps.k64, a->k, a->k_b, a->k_s, a->k_h, a->Sk, 64)) return r;

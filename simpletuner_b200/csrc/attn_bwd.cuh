@@ -4,13 +4,14 @@
 //   P = exp(S*scale - LSE),  dV = P^T dO,  dP = dO V^T,  dS = P o (dP - Delta) * scale,
 //   dQ = dS K,  dK = dS^T Q,   Delta_i = sum_d dO_id O_id
 //
-// Two deterministic kernels, no atomics; 384 threads each: warpgroup 0 is the TMA producer, warpgroups 1 and 2
-// own 64 rows each of the CTA's 128 resident rows.
-//   attn_bwd_dkdv_kernel : one CTA per (b, h, 128-key tile); streams 64-row query tiles.  Transposed domain
-//       (accumulator row = key): S^T = K Q^T, dP^T = V dO^T in registers; P^T and dS^T become the register A operand of
-//       dV += P^T dO,  dK += dS^T Q  (dO / Q tiles re-read from the same shared-memory bytes as MN-major operands).
-//   attn_bwd_dq_kernel   : one CTA per (b, h, 128-row query tile); streams 64-key tiles: S = Q K^T, dP = dO V^T,
-//       dS in registers, dQ += dS K.
+// Two deterministic kernels, no atomics; 384 threads each: warpgroup 0 is the TMA producer (three-stage ring),
+// warpgroups 1 and 2 consume.
+//   attn_bwd_dkdv_kernel : one CTA per (b, h, 64-key tile); streams 64-row query tiles.  Transposed domain
+//       (accumulator row = key): warpgroup 1 forms S^T = K Q^T and P^T and runs dV += P^T dO, warpgroup 2 forms
+//       dP^T = V dO^T and dS^T (with P^T handed over through shared memory) and runs dK += dS^T Q  (dO / Q tiles re-read
+//       from the same shared-memory bytes as MN-major operands).
+//   attn_bwd_dq_kernel   : one CTA per (b, h, 128-row query tile), warpgroups 1 and 2 own 64 rows each; streams 64-key
+//       tiles: S = Q K^T, dP = dO V^T, dS in registers, dQ += dS K.
 // The accumulators are staged through shared memory (fp32) for the store, so that one thread handles contiguous
 // columns of a row — the fused q / k pre-processing backward (qk_prep) needs whole-row sums.
 #pragma once
@@ -44,8 +45,8 @@ struct AttnBwdParams {
 };
 
 struct AttnBwdMaps {
-  // 4-D (d, h, s, b) SWIZZLE_128B; box (64, 1, 128, 1) for the resident operands, (64, 1, 64, 1) for the streamed ones
-  CUtensorMap q128, k128, v128, do128, q64, k64, v64, do64;
+  // 4-D (d, h, s, b) SWIZZLE_128B; box (64, 1, 128, 1) for the dQ kernel's resident Q / dO, (64, 1, 64, 1) otherwise
+  CUtensorMap q128, do128, q64, k64, v64, do64;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -78,12 +79,18 @@ template <int HD>
 struct AttnBwdCfg {
   static constexpr int BIG = 128 * HD * 2;   // resident 128-row tile
   static constexpr int SMALL = 64 * HD * 2;  // streamed 64-row tile
-  static constexpr int STAGES = 2;
-  static constexpr int SMEM_BYTES = 2 * BIG + STAGES * 2 * SMALL + 1024 + 256;
+  static constexpr int STAGES = 3;
+  static constexpr int STAT = 64 * 8;        // per stage (dK / dV kernel): 64 query rows x {LSE * log2(e), Delta}
+  static constexpr int PT = 64 * 64 * 4;     // one fp32 P^T tile handed between the dK / dV warpgroups
+  static constexpr int DKDV_SMEM_BYTES = 2 * SMALL + STAGES * (2 * SMALL + STAT) + 2 * PT + 1024 + 256;
+  static constexpr int DQ_SMEM_BYTES = 2 * BIG + STAGES * 2 * SMALL + 1024 + 256;
 };
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // fp32 accumulator (64 x HD, wgmma layout) of this warpgroup -> shared-memory rows [64][HD + 4] (multiplied by `mul`)
@@ -164,43 +171,72 @@ __device__ __forceinline__ void store_row_half(const float* row, int half, __nv_
   }
 }
 
+// m64n64k16, both operands K-major in shared memory, D = A B^T (scale-d = 0).  The accumulator is write-only ("=f"):
+// with "+f" the compiler copies the previous tile's values into the accumulator registers at the loop back edge, and
+// ptxas serializes every wgmma of a kernel in which a non-wgmma instruction defines an accumulator while MMAs are in
+// flight.
+__device__ __forceinline__ void wgmma_ss_n64_zero(float (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
+      "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]),
+        "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]),
+        "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]),
+        "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31])
+      : "l"(a), "l"(b), "r"(0u));
+}
+
 template <int HD>
 __device__ __forceinline__ void mma_kmajor_n64(float (&d)[32], uint32_t a_tile, uint32_t a_atom, uint32_t b_tile, uint32_t b_atom) {
   // d (64 x 64) = A (64 rows, K = HD, K-major boxes a_atom bytes apart) . B (64 rows, K-major boxes b_atom apart)^T
+  wgmma_ss_n64_zero(d, sdesc_k(a_tile, 0), sdesc_k(b_tile, 0));
 #pragma unroll
-  for (int kk = 0; kk < HD / 16; ++kk)
-    wgmma_ss_n64<0, 0>(d, sdesc_k(a_tile, (kk / 4) * a_atom + (kk % 4) * 32), sdesc_k(b_tile, (kk / 4) * b_atom + (kk % 4) * 32),
-                       kk > 0 ? 1u : 0u);
+  for (int kk = 1; kk < HD / 16; ++kk)
+    wgmma_ss_n64<0, 0>(d, sdesc_k(a_tile, (kk / 4) * a_atom + (kk % 4) * 32), sdesc_k(b_tile, (kk / 4) * b_atom + (kk % 4) * 32), 1u);
 }
 
 // ------------------------------------------------------------------------------------------------
 // dK / dV
 // ------------------------------------------------------------------------------------------------
+// One CTA per (b, h, 64-key tile).  The two consumer warpgroups split the work by product, so that each holds one
+// 64 x HD accumulator and one 64 x 64 product (dV and dK of 64 keys plus S^T and dP^T in one warpgroup do not fit the
+// 168 registers a 384-thread CTA has per thread, and ptxas then spills and serializes the wgmma):
+//   warpgroup 1: S^T = K Q^T -> P^T -> dV += P^T dO;  P^T (fp32) goes to warpgroup 2 through shared memory
+//   warpgroup 2: dP^T = V dO^T;  dS^T = P^T o (dP^T - Delta) -> dK += dS^T Q
+// The P^T hand-over is double-buffered (named barriers PT_FULL / PT_EMPTY + buffer), so warpgroup 1 runs up to one
+// query tile ahead and the two warpgroups' MMAs interleave on the tensor pipe.
 template <int HD>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams p) {
   using Cfg = AttnBwdCfg<HD>;
   constexpr int ATOMS = HD / 64;
-  constexpr int BIG_ATOM = 128 * 128, SMALL_ATOM = 64 * 128;
+  constexpr int ATOM = 64 * 128;   // [64 rows x 64 elems] SW128 box
+  constexpr int PT_FULL = 4, PT_EMPTY = 6;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t k_smem = smem_base, v_smem = smem_base + Cfg::BIG;
-  const uint32_t q_smem = smem_base + 2 * Cfg::BIG;                      // STAGES streamed Q tiles
+  const uint32_t k_smem = smem_base, v_smem = smem_base + Cfg::SMALL;    // resident 64-key K / V tiles
+  const uint32_t q_smem = smem_base + 2 * Cfg::SMALL;                    // STAGES streamed Q tiles
   const uint32_t do_smem = q_smem + Cfg::STAGES * Cfg::SMALL;            // STAGES streamed dO tiles
-  const uint32_t bar_base = do_smem + Cfg::STAGES * Cfg::SMALL;
+  const uint32_t stat_smem = do_smem + Cfg::STAGES * Cfg::SMALL;         // STAGES x 64 float2 {LSE * log2(e), Delta}
+  const uint32_t pt_smem = stat_smem + Cfg::STAGES * Cfg::STAT;          // 2 x P^T tile, [32 values][128 threads] fp32
+  const uint32_t bar_base = pt_smem + 2 * Cfg::PT;
   const uint32_t kv_full = bar_base;
   auto s_full = [&](int s) { return bar_base + 8u * (1 + s); };
   auto s_empty = [&](int s) { return bar_base + 8u * (1 + Cfg::STAGES + s); };
+  float* smem_f = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
+  const float2* stat_rows = reinterpret_cast<const float2*>(smem_f + (stat_smem - smem_base) / 4);
+  float* pt_rows = smem_f + (pt_smem - smem_base) / 4;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
-  const int kv0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
+  const int kv0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
   const int n_q = (p.Sq + 63) / 64;
 
   if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
     for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(s_full(s), 1);
+      mbar_init(s_full(s), 2);   // TMA bytes + the row statistics
       mbar_init(s_empty(s), 8);
     }
     fence_mbar_init();
@@ -210,11 +246,13 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
   if (wg == 0) {
     reg_dealloc<40>();
     if (warp == 0) {
+      const float* lse_bh = p.lse + ((long long)b * p.H + h) * p.Sq;
+      const float* del_bh = p.delta + ((long long)b * p.H + h) * p.Sq;
       if (elect_one()) {
-        mbar_arrive_expect_tx(kv_full, 2 * Cfg::BIG);
+        mbar_arrive_expect_tx(kv_full, 2 * Cfg::SMALL);
         for (int a = 0; a < ATOMS; ++a) {
-          tma_load_4d(k_smem + a * BIG_ATOM, &maps.k128, kv_full, a * 64, h, kv0, b);
-          tma_load_4d(v_smem + a * BIG_ATOM, &maps.v128, kv_full, a * 64, h, kv0, b);
+          tma_load_4d(k_smem + a * ATOM, &maps.k64, kv_full, a * 64, h, kv0, b);
+          tma_load_4d(v_smem + a * ATOM, &maps.v64, kv_full, a * 64, h, kv0, b);
         }
       }
       __syncwarp();
@@ -224,93 +262,135 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
         if (elect_one()) {
           mbar_arrive_expect_tx(s_full(stg), 2 * Cfg::SMALL);
           for (int a = 0; a < ATOMS; ++a) {
-            tma_load_4d(q_smem + stg * Cfg::SMALL + a * SMALL_ATOM, &maps.q64, s_full(stg), a * 64, h, j * 64, b);
-            tma_load_4d(do_smem + stg * Cfg::SMALL + a * SMALL_ATOM, &maps.do64, s_full(stg), a * 64, h, j * 64, b);
+            tma_load_4d(q_smem + stg * Cfg::SMALL + a * ATOM, &maps.q64, s_full(stg), a * 64, h, j * 64, b);
+            tma_load_4d(do_smem + stg * Cfg::SMALL + a * ATOM, &maps.do64, s_full(stg), a * 64, h, j * 64, b);
           }
         }
+        // Queries past Sq get LSE = +inf, so that their P (and with it dS) is exactly 0.
+        float2* st = const_cast<float2*>(stat_rows) + stg * 64;
+#pragma unroll
+        for (int r = lane; r < 64; r += 32) {
+          const int q = j * 64 + r;
+          st[r] = q < p.Sq ? make_float2(__ldg(lse_bh + q) * 1.4426950408889634f, __ldg(del_bh + q)) : make_float2(INFINITY, 0.f);
+        }
         __syncwarp();
+        if (lane == 0) mbar_arrive(s_full(stg));
       }
     }
   } else {
     reg_alloc<232>();
     const int cw = wg - 1;
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const float* lse_bh = p.lse + ((long long)b * p.H + h) * p.Sq;
-    const float* del_bh = p.delta + ((long long)b * p.H + h) * p.Sq;
-    float dv_acc[HD / 2], dk_acc[HD / 2];
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) dv_acc[i] = dk_acc[i] = 0.f;
+    const int t = threadIdx.x & 127;
+    float acc[HD / 2];   // dV (warpgroup 1) or dK (warpgroup 2) of the CTA's 64 keys; the first MMA initialises it
     mbar_wait(kv_full, 0, 41);
-    for (int j = 0; j < n_q; ++j) {
-      const int stg = j % Cfg::STAGES;
-      mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 42);
-      const uint32_t qa = q_smem + stg * Cfg::SMALL, da = do_smem + stg * Cfg::SMALL;
-      float st[32], dpt[32];
-      wg_fence();
-      mma_kmajor_n64<HD>(st, k_smem + cw * 8192, BIG_ATOM, qa, SMALL_ATOM);    // S^T  = K Q^T
-      mma_kmajor_n64<HD>(dpt, v_smem + cw * 8192, BIG_ATOM, da, SMALL_ATOM);   // dP^T = V dO^T
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(st);
-      wg_fence_regs(dpt);
-      // st[4 i + 2 hh + e]: key row (16 wq + lane / 4 + 8 hh), query column 8 i + 2 (lane % 4) + e
+    // s[4 i + 2 hh + e]: key row (16 wq + lane / 4 + 8 hh), query column 8 i + 2 (lane % 4) + e;
+    // stat4[4 i + lane % 4] = {LSE * log2(e), Delta} of query columns 8 i + 2 (lane % 4) + {0, 1}
+    if (cw == 0) {
+      const float sl2 = p.scale * 1.4426950408889634f;
+      for (int j = 0; j < n_q; ++j) {
+        const int stg = j % Cfg::STAGES, buf = j & 1;
+        mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 42);
+        const uint32_t qa = q_smem + stg * Cfg::SMALL, da = do_smem + stg * Cfg::SMALL;
+        const float4* stat4 = reinterpret_cast<const float4*>(stat_rows + stg * 64);
+        float s[32];
+        wg_fence();
+        mma_kmajor_n64<HD>(s, k_smem, ATOM, qa, ATOM);   // S^T = K Q^T
+        wg_commit();
+        wg_wait<0>();   // S^T, and the previous tile's dV
+        wg_fence_regs(s);
+        if (j > 0) {   // both MMAs of this warpgroup that read the previous stage have retired
+          __syncwarp();
+          if (lane == 0) mbar_arrive(s_empty((j - 1) % Cfg::STAGES));
+        }
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int q = j * 64 + 8 * i + 2 * (lane & 3) + e;
-          const bool ok = q < p.Sq;
-          const float l2 = ok ? __ldg(lse_bh + q) * 1.4426950408889634f : 0.f;
-          const float dl = ok ? __ldg(del_bh + q) : 0.f;
+        for (int i = 0; i < 8; ++i) {
+          const float4 sv = stat4[4 * i + (lane & 3)];
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
-            const int x = 4 * i + 2 * hh + e;
-            const float pv = ok ? ex2f(fmaf(st[x], sl2, -l2)) : 0.f;
-            st[x] = pv;                        // P^T
-            dpt[x] = pv * (dpt[x] - dl);       // dS^T (softmax scale applied in the epilogue)
+            s[4 * i + 2 * hh] = ex2f(fmaf(s[4 * i + 2 * hh], sl2, -sv.x));   // P^T
+            s[4 * i + 2 * hh + 1] = ex2f(fmaf(s[4 * i + 2 * hh + 1], sl2, -sv.z));
           }
         }
-      wg_fence();
+        if (j >= 2) named_bar_sync(PT_EMPTY + buf, 256);   // warpgroup 2 has read P^T of tile j - 2
+        float* pt = pt_rows + buf * (Cfg::PT / 4);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {   // 64 queries / 16
-        uint32_t a[4];
-        acc_to_afrag(st, kk, a);
-        wgmma_rs_mn<HD>(dv_acc, a, sdesc_mn(da, kk * 2048, SMALL_ATOM), 1u);
-        acc_to_afrag(dpt, kk, a);
-        wgmma_rs_mn<HD>(dk_acc, a, sdesc_mn(qa, kk * 2048, SMALL_ATOM), 1u);
+        for (int x = 0; x < 32; ++x) pt[x * 128 + t] = s[x];
+        named_bar_arrive(PT_FULL + buf, 256);
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {   // 64 queries / 16
+          uint32_t a[4];
+          acc_to_afrag(s, kk, a);
+          wgmma_rs_mn<HD>(acc, a, sdesc_mn(da, kk * 2048, ATOM), (j > 0 || kk > 0) ? 1u : 0u);   // dV += P^T dO
+        }
+        wg_commit();
       }
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(dv_acc);
-      wg_fence_regs(dk_acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty(stg));
+    } else {
+      for (int j = 0; j < n_q; ++j) {
+        const int stg = j % Cfg::STAGES, buf = j & 1;
+        mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 43);
+        const uint32_t qa = q_smem + stg * Cfg::SMALL, da = do_smem + stg * Cfg::SMALL;
+        const float4* stat4 = reinterpret_cast<const float4*>(stat_rows + stg * 64);
+        float s[32];
+        wg_fence();
+        mma_kmajor_n64<HD>(s, v_smem, ATOM, da, ATOM);   // dP^T = V dO^T
+        wg_commit();
+        wg_wait<0>();   // dP^T, and the previous tile's dK
+        wg_fence_regs(s);
+        if (j > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(s_empty((j - 1) % Cfg::STAGES));
+        }
+        named_bar_sync(PT_FULL + buf, 256);
+        const float* pt = pt_rows + buf * (Cfg::PT / 4);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 sv = stat4[4 * i + (lane & 3)];
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {   // dS^T (softmax scale applied in the epilogue)
+            const int x = 4 * i + 2 * hh;
+            s[x] = pt[x * 128 + t] * (s[x] - sv.y);
+            s[x + 1] = pt[(x + 1) * 128 + t] * (s[x + 1] - sv.w);
+          }
+        }
+        if (j + 2 < n_q) named_bar_arrive(PT_EMPTY + buf, 256);
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          uint32_t a[4];
+          acc_to_afrag(s, kk, a);
+          wgmma_rs_mn<HD>(acc, a, sdesc_mn(qa, kk * 2048, ATOM), (j > 0 || kk > 0) ? 1u : 0u);   // dK += dS^T Q
+        }
+        wg_commit();
+      }
     }
-    // ---- epilogue: stage dV and dK rows through the (now idle) K / V tiles, then store row-contiguously
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    // ---- epilogue: stage the dV (warpgroup 1) / dK (warpgroup 2) rows through the (now idle) K / V / Q tiles, then
+    // store row-contiguously
     named_bar_sync(1, 256);
-    float* stage_rows = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw))) + cw * 64 * (HD + 4);
-    const int t = threadIdx.x & 127;
+    float* stage_rows = smem_f + cw * 64 * (HD + 4);
     const int r = t >> 1, half = t & 1;
-    const int kv = kv0 + cw * 64 + r;
+    const int kv = kv0 + r;
     const bool row_ok = kv < p.Sk;
-    stage_acc<HD>(stage_rows, dv_acc, 1.f);
+    stage_acc<HD>(stage_rows, acc, cw == 0 ? 1.f : p.scale);
     named_bar_sync(2 + cw, 128);
-    store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dv + (long long)b * p.dv_b + (long long)kv * p.dv_s + (long long)h * p.dv_h,
-                       row_ok, false, nullptr, nullptr, nullptr, nullptr, 0.f);
-    named_bar_sync(2 + cw, 128);
-    stage_acc<HD>(stage_rows, dk_acc, p.scale);
-    named_bar_sync(2 + cw, 128);
-    const __nv_bfloat16* xrow = nullptr;
-    const __nv_bfloat16* wk = nullptr;
-    const float *cs = nullptr, *sn = nullptr;
-    if (p.fuse_prep) {   // dK row -> gradient of the k projection output (token index == key index)
-      xrow = p.src + (long long)b * p.src_b + (long long)min(kv, p.Sk - 1) * p.src_s + p.k_off + h * HD;
-      wk = (kv < p.s_split) ? p.wk1 : p.wk0;
-      cs = p.cosT ? p.cosT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
-      sn = p.sinT ? p.sinT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
+    if (cw == 0) {
+      store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dv + (long long)b * p.dv_b + (long long)kv * p.dv_s + (long long)h * p.dv_h,
+                         row_ok, false, nullptr, nullptr, nullptr, nullptr, 0.f);
+    } else {
+      const __nv_bfloat16* xrow = nullptr;
+      const __nv_bfloat16* wk = nullptr;
+      const float *cs = nullptr, *sn = nullptr;
+      if (p.fuse_prep) {   // dK row -> gradient of the k projection output (token index == key index)
+        xrow = p.src + (long long)b * p.src_b + (long long)min(kv, p.Sk - 1) * p.src_s + p.k_off + h * HD;
+        wk = (kv < p.s_split) ? p.wk1 : p.wk0;
+        cs = p.cosT ? p.cosT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
+        sn = p.sinT ? p.sinT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
+      }
+      store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h,
+                         row_ok, p.fuse_prep != 0, xrow, wk, cs, sn, p.eps);
     }
-    store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h,
-                       row_ok, p.fuse_prep != 0, xrow, wk, cs, sn, p.eps);
   }
 }
 
@@ -385,10 +465,12 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
       l2[hh] = __ldg(p.lse + o) * 1.4426950408889634f;
       dl[hh] = __ldg(p.delta + o);
     }
-    float dq_acc[HD / 2];
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) dq_acc[i] = 0.f;
+    float dq_acc[HD / 2];   // the first MMA initialises it
     mbar_wait(qd_full, 0, 51);
+    // Per key tile, three wgmma groups: S, dP, dQ.  The previous tile's dQ MMA retires behind this tile's S (its dS
+    // fragments stay live until then, so dP is issued only after it: all of them together exceed the 168 registers of
+    // a 384-thread CTA); exp(S) runs while dP is on the tensor pipe.  A stage goes back to the producer once the dQ MMA
+    // reading its K has retired.
     for (int j = 0; j < n_kv; ++j) {
       const int stg = j % Cfg::STAGES;
       mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 52);
@@ -396,11 +478,16 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
       float sc[32], dp[32];
       wg_fence();
       mma_kmajor_n64<HD>(sc, q_smem + cw * 8192, BIG_ATOM, ka, SMALL_ATOM);    // S  = Q K^T
+      wg_commit();
+      wg_wait<1>();   // the previous tile's dQ
+      if (j > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(s_empty((j - 1) % Cfg::STAGES));
+      }
       mma_kmajor_n64<HD>(dp, do_smem + cw * 8192, BIG_ATOM, va, SMALL_ATOM);   // dP = dO V^T
       wg_commit();
-      wg_wait<0>();
+      wg_wait<1>();   // S
       wg_fence_regs(sc);
-      wg_fence_regs(dp);
 #pragma unroll
       for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -409,23 +496,24 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const int x = 4 * i + 2 * hh + e;
-            const float pv = ok ? ex2f(fmaf(sc[x], sl2, -l2[hh])) : 0.f;
-            dp[x] = pv * (dp[x] - dl[hh]);   // dS (softmax scale applied in the epilogue)
+            sc[x] = ok ? ex2f(fmaf(sc[x], sl2, -l2[hh])) : 0.f;   // P
           }
         }
+      wg_wait<0>();   // dP
+      wg_fence_regs(dp);
+#pragma unroll
+      for (int x = 0; x < 32; ++x) dp[x] = sc[x] * (dp[x] - dl[(x >> 1) & 1]);   // dS (softmax scale applied in the epilogue)
       wg_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {   // 64 keys / 16
         uint32_t a[4];
         acc_to_afrag(dp, kk, a);
-        wgmma_rs_mn<HD>(dq_acc, a, sdesc_mn(ka, kk * 2048, SMALL_ATOM), 1u);
+        wgmma_rs_mn<HD>(dq_acc, a, sdesc_mn(ka, kk * 2048, SMALL_ATOM), (j > 0 || kk > 0) ? 1u : 0u);
       }
       wg_commit();
-      wg_wait<0>();
-      wg_fence_regs(dq_acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty(stg));
     }
+    wg_wait<0>();
+    wg_fence_regs(dq_acc);
     // ---- epilogue through the (now idle) Q / dO tiles
     named_bar_sync(1, 256);
     float* stage_rows = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw))) + cw * 64 * (HD + 4);
