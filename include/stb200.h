@@ -125,7 +125,7 @@ typedef struct {
   long long q_b, q_s, q_h, k_b, k_s, k_h, v_b, v_s, v_h, o_b, o_s, o_h, do_b, do_s, do_h;
   const float* lse;  /* [B, H, Sq] from the forward */
   float* delta;      /* [B, H, Sq] fp32 scratch: rowsum(dO * O) */
-  float* dq_accum;   /* [B, Sq, H, HD] fp32 scratch (zeroed by the call) */
+  float* dq_accum;   /* unused: neither read nor written (kept for ABI compatibility) */
   void *dq, *dk, *dv;
   long long dq_b, dq_s, dq_h, dk_b, dk_s, dk_h, dv_b, dv_s, dv_h;
   const stb_qk_prep* qk_prep; /* NULL: dq / dk are the gradients of the q / k inputs */

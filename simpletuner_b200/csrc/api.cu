@@ -22,7 +22,6 @@
 #include "optim.cuh"
 #include "elementwise.cuh"
 #include "gemm.cuh"
-#include "wgrad_full.cuh"
 #include "lokr.cuh"
 #include "vae.cuh"
 #include "wgrad.cuh"
@@ -108,7 +107,28 @@ struct MapKeyHash {
 std::mutex g_map_mu;
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 
-// bf16 tensor map, SWIZZLE_128B, dims/strides innermost-first (strides in BYTES for dims 1..rank-1)
+// bf16 SWIZZLE_128B map, dims / box / per-dimension traversal strides innermost-first, strides in BYTES for dims
+// 1..rank-1; not cached (the strided conv windows use it directly)
+int make_map_strided(CUtensorMap* out, const void* ptr, int rank, const unsigned long long* dims,
+                     const unsigned long long* strides_bytes, const unsigned* box, const unsigned* estrides) {
+  auto fn = encode_fn();
+  if (!fn) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  if (reinterpret_cast<uintptr_t>(ptr) & 15) return fail(STB_ERR_ARG, "tensor base pointer must be 16-byte aligned");
+  for (int i = 0; i + 1 < rank; ++i)
+    if (strides_bytes[i] & 15) return fail(STB_ERR_ARG, "tensor stride %d (%llu bytes) must be a multiple of 16 bytes", i, strides_bytes[i]);
+  cuuint64_t gdim[4];
+  cuuint64_t gstr[3];
+  cuuint32_t bx[4], es[4];
+  for (int i = 0; i < rank; ++i) gdim[i] = dims[i], bx[i] = box[i], es[i] = estrides[i];
+  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", int(r));
+  return 0;
+}
+
+// make_map_strided with unit traversal strides, cached by (pointer, shape, strides, box)
 int make_map(CUtensorMap* out, const void* ptr, int rank, const unsigned long long* dims,
              const unsigned long long* strides_bytes, const unsigned* box) {
   MapKey key;
@@ -125,20 +145,8 @@ int make_map(CUtensorMap* out, const void* ptr, int rank, const unsigned long lo
       return 0;
     }
   }
-  auto fn = encode_fn();
-  if (!fn) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  if (reinterpret_cast<uintptr_t>(ptr) & 15) return fail(STB_ERR_ARG, "tensor base pointer must be 16-byte aligned");
-  for (int i = 0; i + 1 < rank; ++i)
-    if (strides_bytes[i] & 15) return fail(STB_ERR_ARG, "tensor stride %d (%llu bytes) must be a multiple of 16 bytes", i, strides_bytes[i]);
-  cuuint64_t gdim[4];
-  cuuint64_t gstr[3];
-  cuuint32_t bx[4], es[4];
-  for (int i = 0; i < rank; ++i) gdim[i] = dims[i], bx[i] = box[i], es[i] = 1;
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", int(r));
+  static const unsigned unit[4] = {1, 1, 1, 1};
+  if (int r = make_map_strided(out, ptr, rank, dims, strides_bytes, box, unit)) return r;
   {
     std::lock_guard<std::mutex> lk(g_map_mu);
     if (g_maps.size() > 65536) g_maps.clear();
@@ -147,51 +155,54 @@ int make_map(CUtensorMap* out, const void* ptr, int rank, const unsigned long lo
   return 0;
 }
 
-// fp32 map without swizzle (dq accumulator reduce-add)
-int make_map_f32(CUtensorMap* out, const void* ptr, int rank, const unsigned long long* dims,
-                 const unsigned long long* strides_bytes, const unsigned* box) {
-  auto fn = encode_fn();
-  if (!fn) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t gdim[4];
-  cuuint64_t gstr[3];
-  cuuint32_t bx[4], es[4];
-  for (int i = 0; i < rank; ++i) gdim[i] = dims[i], bx[i] = box[i], es[i] = 1;
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled(f32) failed with CUresult %d", int(r));
-  return 0;
+// Token-major operand [B, S, C] (row stride s_stride, batch stride b_stride, in elements) as the 3-D map (C, S, B) with
+// box (64, rows, 1).  With one batch the batch stride addresses nothing, so S rows stand in for it: views of a larger
+// buffer then encode whatever batch stride they carry.
+int make_token_map(CUtensorMap* out, const void* ptr, int C, int S, int B, long long s_stride, long long b_stride,
+                   unsigned rows) {
+  const unsigned long long d[3] = {(unsigned long long)C, (unsigned long long)S, (unsigned long long)B};
+  const unsigned long long sb[2] = {(unsigned long long)s_stride * 2ull,
+                                    (unsigned long long)(B == 1 ? s_stride * (long long)S : b_stride) * 2ull};
+  const unsigned bx[3] = {64, rows, 1};
+  return make_map(out, ptr, 3, d, sb, bx);
 }
 
-// bf16 SWIZZLE_128B map with per-dimension traversal strides (strided conv windows); not cached
-int make_map_strided(CUtensorMap* out, const void* ptr, int rank, const unsigned long long* dims,
-                     const unsigned long long* strides_bytes, const unsigned* box, const unsigned* estrides) {
-  auto fn = encode_fn();
-  if (!fn) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  if (reinterpret_cast<uintptr_t>(ptr) & 15) return fail(STB_ERR_ARG, "tensor base pointer must be 16-byte aligned");
-  cuuint64_t gdim[4];
-  cuuint64_t gstr[3];
-  cuuint32_t bx[4], es[4];
-  for (int i = 0; i < rank; ++i) gdim[i] = dims[i], bx[i] = box[i], es[i] = estrides[i];
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(STB_ERR_CUDA, "cuTensorMapEncodeTiled(strided) failed with CUresult %d", int(r));
-  return 0;
+// Attention operand [B, S, H, HD] with element strides (sb, ss, sh) as the 4-D map (HD, H, S, B), box (64, 1, rows, 1):
+// one head's rows of one batch per load
+int make_head_map(CUtensorMap* out, const void* ptr, int HD, int H, int S, int B, long long sb, long long ss,
+                  long long sh, unsigned rows) {
+  const unsigned long long d[4] = {(unsigned long long)HD, (unsigned long long)H, (unsigned long long)S, (unsigned long long)B};
+  const unsigned long long s[3] = {(unsigned long long)sh * 2ull, (unsigned long long)ss * 2ull, (unsigned long long)sb * 2ull};
+  const unsigned bx[4] = {64, 1, rows, 1};
+  return make_map(out, ptr, 4, d, s, bx);
 }
 
-template <typename K>
-int set_smem(K kernel, int bytes) {
-  STB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+// Raises Kernel's dynamic shared-memory limit before its first launch.  Thread-safe: concurrent first calls both set
+// the same value; a failed call is reported and retried on the next launch.
+template <auto Kernel>
+int set_smem(int bytes) {
+  static std::atomic<bool> done{false};
+  if (done.load(std::memory_order_acquire)) return 0;
+  STB_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  done.store(true, std::memory_order_release);
   return 0;
 }
 
 // ---------------------------------------------------------------- GEMM
+// One launch of the persistent GEMM for GEMM and conv3x3 alike: one CTA per SM, or one per tile when there are fewer
+template <int BN, bool CONV>
+int launch_gemm_kernel(const stb::GemmMaps& maps, const stb::GemmParams& p, cudaStream_t st, const char* name) {
+  using Cfg = stb::GemmCfg<BN>;
+  if (int r = set_smem<stb::gemm_bf16_tn_kernel<BN, CONV>>(Cfg::SMEM_BYTES)) return r;
+  const long long tiles = (long long)((p.rows_per_batch + Cfg::BM - 1) / Cfg::BM) * p.num_batches * ((p.N + BN - 1) / BN);
+  const int grid = (int)std::min<long long>(tiles, num_sms());
+  stb::gemm_bf16_tn_kernel<BN, CONV><<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
+  STB_LAUNCH_CHECK(name);
+  return 0;
+}
+
 template <int BN>
 int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
-  using Cfg = stb::GemmCfg<BN>;
   stb::GemmMaps maps;
   std::memset(&maps, 0, sizeof maps);
   stb::GemmParams p;
@@ -199,12 +210,8 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   for (int s = 0; s < a->nseg; ++s) {
     const stb_gemm_seg& g = a->seg[s];
     if (g.K <= 0 || (g.K & 7)) return fail(STB_ERR_ARG, "segment %d: K=%d must be a positive multiple of 8", s, g.K);
-    unsigned long long ad[3] = {(unsigned long long)g.K, (unsigned long long)a->rows_per_batch,
-                                (unsigned long long)a->num_batches};
-    unsigned long long as[2] = {(unsigned long long)g.a_row_stride * 2ull, (unsigned long long)g.a_batch_stride * 2ull};
-    if (a->num_batches == 1) as[1] = as[0] * (unsigned long long)a->rows_per_batch;
-    unsigned ab[3] = {64, 128, 1};
-    if (int r = make_map(&maps.a[s], g.a, 3, ad, as, ab)) return r;
+    if (int r = make_token_map(&maps.a[s], g.a, g.K, a->rows_per_batch, a->num_batches, g.a_row_stride, g.a_batch_stride, 128))
+      return r;
     if (g.w_kn) {   // [K, N] row-major: contraction index = row; staged as 64 x 64 MN-major boxes
       unsigned long long wd[2] = {(unsigned long long)a->N, (unsigned long long)g.K};
       unsigned long long ws[1] = {(unsigned long long)g.w_row_stride * 2ull};
@@ -237,23 +244,21 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   p.aux = static_cast<__nv_bfloat16*>(a->aux);
   p.aux_batch_stride = a->aux_batch_stride;
   p.aux_row_stride = a->aux_row_stride;
-
-  auto kernel = stb::gemm_bf16_tn_kernel<BN, false>;
-  static bool configured = false;
-  if (!configured) {
-    if (int r = set_smem(kernel, Cfg::SMEM_BYTES)) return r;
-    configured = true;
-  }
-  const long long tiles = (long long)((a->rows_per_batch + Cfg::BM - 1) / Cfg::BM) * a->num_batches * ((a->N + BN - 1) / BN);
-  const int grid = (int)std::min<long long>(tiles, num_sms());
-  kernel<<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
-  STB_LAUNCH_CHECK("gemm_bf16_tn");
-  return 0;
+  return launch_gemm_kernel<BN, false>(maps, p, st, "gemm_bf16_tn");
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
+
+template <int HD, bool BIAS>
+static int launch_attn_fwd(const stb::AttnFwdMaps& maps, const stb::AttnFwdParams& p, dim3 grid, cudaStream_t st) {
+  constexpr int SMEM = stb::AttnFwdCfg<HD>::SMEM_BYTES;
+  if (int r = set_smem<stb::attn_fwd_kernel<HD, BIAS>>(SMEM)) return r;
+  stb::attn_fwd_kernel<HD, BIAS><<<grid, 384, SMEM, st>>>(maps, p);
+  STB_LAUNCH_CHECK(BIAS ? "attn_fwd_bias" : "attn_fwd");
+  return 0;
+}
 
 template <int HD>
 static int launch_attn_bwd(const stb_attn_bwd_args* a, const stb::AttnBwdMaps& maps, const stb::AttnBwdParams& p,
@@ -266,18 +271,25 @@ static int launch_attn_bwd(const stb_attn_bwd_args* a, const stb::AttnBwdMaps& m
     STB_LAUNCH_CHECK("attn_bwd_delta");
   }
   constexpr int SMEM1 = stb::AttnBwdCfg<HD>::DKDV_SMEM_BYTES, SMEM2 = stb::AttnBwdCfg<HD>::DQ_SMEM_BYTES;
-  auto k1 = stb::attn_bwd_dkdv_kernel<HD>;
-  auto k2 = stb::attn_bwd_dq_kernel<HD>;
-  static bool configured = false;
-  if (!configured) {
-    if (int r = set_smem(k1, SMEM1)) return r;
-    if (int r = set_smem(k2, SMEM2)) return r;
-    configured = true;
-  }
-  k1<<<dim3((a->Sk + 63) / 64, a->H, a->B), 384, SMEM1, st>>>(maps, p);
+  if (int r = set_smem<stb::attn_bwd_dkdv_kernel<HD>>(SMEM1)) return r;
+  if (int r = set_smem<stb::attn_bwd_dq_kernel<HD>>(SMEM2)) return r;
+  stb::attn_bwd_dkdv_kernel<HD><<<dim3((a->Sk + 63) / 64, a->H, a->B), 384, SMEM1, st>>>(maps, p);
   STB_LAUNCH_CHECK("attn_bwd_dkdv");
-  k2<<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM2, st>>>(maps, p);
+  stb::attn_bwd_dq_kernel<HD><<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM2, st>>>(maps, p);
   STB_LAUNCH_CHECK("attn_bwd_dq");
+  return 0;
+}
+
+// Weight-gradient GEMM over p's work units: one CTA per unit, at most one per SM for the persistent full-rank grid.
+template <int BN, int OUT>
+static int launch_wgrad(const stb::WgradMaps& maps, stb::WgradParams p, cudaStream_t st) {
+  constexpr int SMEM = stb::WgradCfg<BN, OUT>::SMEM_BYTES;
+  if (int r = set_smem<stb::wgrad_kernel<BN, OUT>>(SMEM)) return r;
+  p.col_tiles = (p.K + BN - 1) / BN;   // 1 for a LoRA rank (R <= BN)
+  const int units = p.splits * ((p.N + 127) / 128) * p.col_tiles;
+  const int grid = OUT == stb::WGRAD_OUT_BF16_NK ? std::min(units, num_sms()) : units;
+  stb::wgrad_kernel<BN, OUT><<<grid, 384, SMEM, st>>>(maps, p);
+  STB_LAUNCH_CHECK(OUT == stb::WGRAD_OUT_BF16_NK ? "wgrad_full" : "wgrad_tn");
   return 0;
 }
 
@@ -330,11 +342,7 @@ int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   stb::AttnFwdMaps maps;
   auto mk = [&](CUtensorMap* m, const void* ptr, long long sb, long long ss, long long sh, int S) {
-    unsigned long long d[4] = {(unsigned long long)a->HD, (unsigned long long)a->H, (unsigned long long)S,
-                               (unsigned long long)a->B};
-    unsigned long long s[3] = {(unsigned long long)sh * 2ull, (unsigned long long)ss * 2ull, (unsigned long long)sb * 2ull};
-    unsigned bx[4] = {64, 1, 128, 1};
-    return make_map(m, ptr, 4, d, s, bx);
+    return make_head_map(m, ptr, a->HD, a->H, S, a->B, sb, ss, sh, 128);
   };
   if (int r = mk(&maps.q, a->q, a->q_b, a->q_s, a->q_h, a->Sq)) return r;
   if (int r = mk(&maps.k, a->k, a->k_b, a->k_s, a->k_h, a->Sk)) return r;
@@ -348,48 +356,12 @@ int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
   p.bias = static_cast<const __nv_bfloat16*>(a->bias);
   p.bias_h = a->bias_h; p.bias_q = a->bias_q;
   p.inv_scale = a->scale != 0.f ? 1.f / a->scale : 0.f;
-  dim3 grid((a->Sq + 127) / 128, a->H, a->B);
+  const dim3 grid((a->Sq + 127) / 128, a->H, a->B);
   if (a->bias) {   // text-encoder instantiation (additive bias / mask); never taken by the training step
     if (a->scale == 0.f || a->bias_q < a->Sk) return fail(STB_ERR_ARG, "attn_fwd bias: scale must be non-zero and bias_q >= Sk");
-    if (a->HD == 128) {
-      auto kernel = stb::attn_fwd_kernel<128, true>;
-      static bool configured = false;
-      if (!configured) {
-        if (int r = set_smem(kernel, stb::AttnFwdCfg<128>::SMEM_BYTES)) return r;
-        configured = true;
-      }
-      kernel<<<grid, 384, stb::AttnFwdCfg<128>::SMEM_BYTES, st>>>(maps, p);
-    } else {
-      auto kernel = stb::attn_fwd_kernel<64, true>;
-      static bool configured = false;
-      if (!configured) {
-        if (int r = set_smem(kernel, stb::AttnFwdCfg<64>::SMEM_BYTES)) return r;
-        configured = true;
-      }
-      kernel<<<grid, 384, stb::AttnFwdCfg<64>::SMEM_BYTES, st>>>(maps, p);
-    }
-    STB_LAUNCH_CHECK("attn_fwd_bias");
-    return 0;
+    return a->HD == 128 ? launch_attn_fwd<128, true>(maps, p, grid, st) : launch_attn_fwd<64, true>(maps, p, grid, st);
   }
-  if (a->HD == 128) {
-    auto kernel = stb::attn_fwd_kernel<128, false>;
-    static bool configured = false;
-    if (!configured) {
-      if (int r = set_smem(kernel, stb::AttnFwdCfg<128>::SMEM_BYTES)) return r;
-      configured = true;
-    }
-    kernel<<<grid, 384, stb::AttnFwdCfg<128>::SMEM_BYTES, st>>>(maps, p);
-  } else {
-    auto kernel = stb::attn_fwd_kernel<64, false>;
-    static bool configured = false;
-    if (!configured) {
-      if (int r = set_smem(kernel, stb::AttnFwdCfg<64>::SMEM_BYTES)) return r;
-      configured = true;
-    }
-    kernel<<<grid, 384, stb::AttnFwdCfg<64>::SMEM_BYTES, st>>>(maps, p);
-  }
-  STB_LAUNCH_CHECK("attn_fwd");
-  return 0;
+  return a->HD == 128 ? launch_attn_fwd<128, false>(maps, p, grid, st) : launch_attn_fwd<64, false>(maps, p, grid, st);
 }
 
 int stb_attn_bwd(const stb_attn_bwd_args* a, void* stream) {
@@ -406,11 +378,7 @@ int stb_attn_bwd(const stb_attn_bwd_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   stb::AttnBwdMaps maps;
   auto mk = [&](CUtensorMap* m, const void* ptr, long long sb, long long ss, long long sh, int S, unsigned rows) {
-    unsigned long long d[4] = {(unsigned long long)a->HD, (unsigned long long)a->H, (unsigned long long)S,
-                               (unsigned long long)a->B};
-    unsigned long long s[3] = {(unsigned long long)sh * 2ull, (unsigned long long)ss * 2ull, (unsigned long long)sb * 2ull};
-    unsigned bx[4] = {64, 1, rows, 1};
-    return make_map(m, ptr, 4, d, s, bx);
+    return make_head_map(m, ptr, a->HD, a->H, S, a->B, sb, ss, sh, rows);
   };
   if (int r = mk(&maps.q128, a->q, a->q_b, a->q_s, a->q_h, a->Sq, 128)) return r;
   if (int r = mk(&maps.do128, a->d_o, a->do_b, a->do_s, a->do_h, a->Sq, 128)) return r;
@@ -520,12 +488,14 @@ int stb_qk_rmsnorm_rope_fwd(const void* src, long long src_b, long long src_s, i
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long warps = (long long)B * S;  // one warp per token
   const unsigned grid = (unsigned)((warps + 7) / 8);
-  auto SRC = static_cast<const __nv_bfloat16*>(src);
   auto cast = [](const void* p) { return static_cast<const __nv_bfloat16*>(p); };
-  if (HD == 128)
-    stb::qk_rmsnorm_rope_fwd_kernel<128><<<grid, 256, 0, st>>>(SRC, src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t, static_cast<__nv_bfloat16*>(q_out), static_cast<__nv_bfloat16*>(k_out), dst_b, dst_s, B, S, H, eps);
-  else
-    stb::qk_rmsnorm_rope_fwd_kernel<64><<<grid, 256, 0, st>>>(SRC, src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t, static_cast<__nv_bfloat16*>(q_out), static_cast<__nv_bfloat16*>(k_out), dst_b, dst_s, B, S, H, eps);
+  auto launch = [&](auto hd) {
+    stb::qk_rmsnorm_rope_fwd_kernel<decltype(hd)::value><<<grid, 256, 0, st>>>(
+        cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t,
+        static_cast<__nv_bfloat16*>(q_out), static_cast<__nv_bfloat16*>(k_out), dst_b, dst_s, B, S, H, eps);
+  };
+  if (HD == 128) launch(std::integral_constant<int, 128>{});
+  else launch(std::integral_constant<int, 64>{});
   STB_LAUNCH_CHECK("qk_rmsnorm_rope_fwd");
   return 0;
 }
@@ -541,25 +511,33 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
   const long long warps = (long long)B * S;  // one warp per token
   const unsigned grid = (unsigned)((warps + 7) / 8);
   auto cast = [](const void* p) { return static_cast<const __nv_bfloat16*>(p); };
-  if (HD == 128) {
-    if (dw) stb::qk_rmsnorm_rope_bwd_kernel<128, true><<<grid, 256, 0, st>>>(cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), ds_b, ds_s, B, S, H, eps, dw);
-    else {
-      static const bool loop_kernel = [] { const char* e = std::getenv("STB_ROPE_BWD_LOOP"); return e && e[0] == '1'; }();
-      const bool flat_ok = aligned16(dq) && aligned16(dk) && aligned16(src) && aligned16(dsrc) && !(d_b & 7) && !(d_s & 7) && !(src_s & 7) &&
-                           !(src_b & 7) && !(k_off & 7) && !(ds_s & 7) && !(ds_b & 7) && (!cos_t || (aligned16(cos_t) && aligned16(sin_t))) &&
-                           (!wq || aligned16(wq)) && (!wk || aligned16(wk)) && (!wq_added || aligned16(wq_added)) && (!wk_added || aligned16(wk_added));
-      if (flat_ok && !loop_kernel) {   // one 16-byte chunk per thread: 4.0 TB/s vs 2.7 for the warp-per-token loop
-        const long long threads = (long long)B * S * 2 * H * 16;
-        stb::qk_rmsnorm_rope_flat128_kernel<true><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
-            cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split,
-            cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), nullptr, ds_b, ds_s, B, S, H, eps);
-      } else {
-        stb::qk_rmsnorm_rope_bwd_kernel<128, false><<<grid, 256, 0, st>>>(cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), ds_b, ds_s, B, S, H, eps, dw);
-      }
+  // the warp-per-token kernel, with the RMSNorm weight gradient when dw is given
+  auto launch = [&](auto hd, auto with_dw) {
+    stb::qk_rmsnorm_rope_bwd_kernel<decltype(hd)::value, decltype(with_dw)::value><<<grid, 256, 0, st>>>(
+        cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split,
+        cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), ds_b, ds_s, B, S, H, eps, dw);
+  };
+  using HD128 = std::integral_constant<int, 128>;
+  using HD64 = std::integral_constant<int, 64>;
+  if (HD == 128 && !dw) {
+    static const bool loop_kernel = [] { const char* e = std::getenv("STB_ROPE_BWD_LOOP"); return e && e[0] == '1'; }();
+    const bool flat_ok = aligned16(dq) && aligned16(dk) && aligned16(src) && aligned16(dsrc) && !(d_b & 7) && !(d_s & 7) && !(src_s & 7) &&
+                         !(src_b & 7) && !(k_off & 7) && !(ds_s & 7) && !(ds_b & 7) && (!cos_t || (aligned16(cos_t) && aligned16(sin_t))) &&
+                         (!wq || aligned16(wq)) && (!wk || aligned16(wk)) && (!wq_added || aligned16(wq_added)) && (!wk_added || aligned16(wk_added));
+    if (flat_ok && !loop_kernel) {   // one 16-byte chunk per thread: 4.0 TB/s vs 2.7 for the warp-per-token loop
+      const long long threads = (long long)B * S * 2 * H * 16;
+      stb::qk_rmsnorm_rope_flat128_kernel<true><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
+          cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split,
+          cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), nullptr, ds_b, ds_s, B, S, H, eps);
+    } else {
+      launch(HD128{}, std::false_type{});
     }
+  } else if (HD == 128) {
+    launch(HD128{}, std::true_type{});
+  } else if (dw) {
+    launch(HD64{}, std::true_type{});
   } else {
-    if (dw) stb::qk_rmsnorm_rope_bwd_kernel<64, true><<<grid, 256, 0, st>>>(cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), ds_b, ds_s, B, S, H, eps, dw);
-    else stb::qk_rmsnorm_rope_bwd_kernel<64, false><<<grid, 256, 0, st>>>(cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split, cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), ds_b, ds_s, B, S, H, eps, dw);
+    launch(HD64{}, std::false_type{});
   }
   STB_LAUNCH_CHECK("qk_rmsnorm_rope_bwd");
   return 0;
@@ -785,45 +763,23 @@ int stb_wgrad_full(const void* dy, long long dy_b, long long dy_s, const void* x
   if (!dy || !x || !dw || B < 1 || S < 1 || N < 8 || K < 8 || (N & 7) || (K & 7)) return fail(STB_ERR_ARG, "wgrad_full: N, K must be positive multiples of 8");
   if (!aligned16(dw) || (dw_row_stride & 7)) return fail(STB_ERR_ARG, "wgrad_full: dW must be 16-byte aligned with a row stride multiple of 8");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  stb::WgradFullMaps maps;
-  unsigned bx[3] = {64, 64, 1};
-  {
-    unsigned long long d[3] = {(unsigned long long)N, (unsigned long long)S, (unsigned long long)B};
-    unsigned long long sb[2] = {(unsigned long long)dy_s * 2ull, (unsigned long long)(B == 1 ? dy_s * (long long)S : dy_b) * 2ull};
-    if (int r = make_map(&maps.dy, dy, 3, d, sb, bx)) return r;
-  }
-  {
-    unsigned long long d[3] = {(unsigned long long)K, (unsigned long long)S, (unsigned long long)B};
-    unsigned long long sb[2] = {(unsigned long long)x_s * 2ull, (unsigned long long)(B == 1 ? x_s * (long long)S : x_b) * 2ull};
-    if (int r = make_map(&maps.x, x, 3, d, sb, bx)) return r;
-  }
-  stb::WgradFullParams p;
-  p.S = S; p.B = B; p.N = N; p.K = K;
+  stb::WgradMaps maps;
+  if (int r = make_token_map(&maps.a, dy, N, S, B, dy_s, dy_b, 64)) return r;
+  if (int r = make_token_map(&maps.b, x, K, S, B, x_s, x_b, 64)) return r;
+  stb::WgradParams p{};
+  p.N = N;
+  p.K = K;
+  p.chunks = (S + 63) / 64;
+  p.splits = p.splits_per_group = 1;   // one split: every tile sums all B x chunks k-blocks
+  p.kb_per_group = p.kb_per_split = B * p.chunks;
   p.alpha = alpha;
-  p.accumulate = accumulate;
   p.out = static_cast<__nv_bfloat16*>(dw);
   p.out_row_stride = dw_row_stride;
-  const int tiles_n = (N + 127) / 128;
-  const int sms = num_sms();
+  p.accumulate = accumulate;
   // 256-wide tiles unless they leave more than half of the SMs idle
-  const bool wide = tiles_n * ((K + 255) / 256) >= sms / 2 || K <= 128;
-  if (wide) {
-    auto kern = stb::wgrad_full_kernel<256>;
-    constexpr int SMEM = stb::WgradFullCfg<256>::SMEM_BYTES;
-    static bool configured = false;
-    if (!configured) { if (int r = set_smem(kern, SMEM)) return r; configured = true; }
-    const int tiles = tiles_n * ((K + 255) / 256);
-    kern<<<std::min(tiles, sms), 384, SMEM, st>>>(maps, p);
-  } else {
-    auto kern = stb::wgrad_full_kernel<128>;
-    constexpr int SMEM = stb::WgradFullCfg<128>::SMEM_BYTES;
-    static bool configured = false;
-    if (!configured) { if (int r = set_smem(kern, SMEM)) return r; configured = true; }
-    const int tiles = tiles_n * ((K + 127) / 128);
-    kern<<<std::min(tiles, sms), 384, SMEM, st>>>(maps, p);
-  }
-  STB_LAUNCH_CHECK("wgrad_full");
-  return 0;
+  if (((N + 127) / 128) * ((K + 255) / 256) >= num_sms() / 2 || K <= 128)
+    return launch_wgrad<256, stb::WGRAD_OUT_BF16_NK>(maps, p, st);
+  return launch_wgrad<128, stb::WGRAD_OUT_BF16_NK>(maps, p, st);
 }
 
 int stb_colsum2(const void* dy, long long dy_b, long long dy_s, const void* z, long long z_b, long long z_s, float* sum,
@@ -872,50 +828,26 @@ int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm
   if (R % 8 == 0 && R <= 128 && N % 8 == 0 && aligned16(L) && aligned16(Rm) && !(l_s & 7) && !(r_s & 7) &&
       (B == 1 || (!(l_b & 7) && !(r_b & 7)))) {
     stb::WgradMaps maps;
-    unsigned bx[3] = {64, 64, 1};
-    {
-      unsigned long long d[3] = {(unsigned long long)N, (unsigned long long)S, (unsigned long long)B};
-      unsigned long long sb[2] = {(unsigned long long)r_s * 2ull, (unsigned long long)(B == 1 ? r_s * (long long)S : r_b) * 2ull};
-      if (int r = make_map(&maps.rm, Rm, 3, d, sb, bx)) return r;
-    }
-    {
-      unsigned long long d[3] = {(unsigned long long)R, (unsigned long long)S, (unsigned long long)B};
-      unsigned long long sb[2] = {(unsigned long long)l_s * 2ull, (unsigned long long)(B == 1 ? l_s * (long long)S : l_b) * 2ull};
-      if (int r = make_map(&maps.l, L, 3, d, sb, bx)) return r;
-    }
-    stb::WgradParams p;
-    p.S = S; p.B = B; p.N = N; p.R = R;
-    p.alpha = alpha;
-    p.out = out;
-    const int n_tiles = (N + 127) / 128;
+    if (int r = make_token_map(&maps.a, Rm, N, S, B, r_s, r_b, 64)) return r;
+    if (int r = make_token_map(&maps.b, L, R, S, B, l_s, l_b, 64)) return r;
     int spb, rows;
     skinny_split(B, S, N, rows, spb);
-    p.partial = nullptr;
-    if (workspace) {
-      if (workspace_elems < (long long)spb * B * R * N) return fail(STB_ERR_ARG, "skinny_tn workspace too small (stb_skinny_tn_workspace)");
-      p.partial = workspace;
-    }
-    p.rows_per_split = rows;
-    p.splits_per_batch = spb;
-    dim3 grid(n_tiles, spb * B);
-    if (R <= 64) {
-      auto kern = stb::wgrad_tn_kernel<64>;
-      static bool configured = false;
-      if (!configured) {
-        if (int r = set_smem(kern, stb::WgradCfg<64>::SMEM_BYTES)) return r;
-        configured = true;
-      }
-      kern<<<grid, 384, stb::WgradCfg<64>::SMEM_BYTES, st>>>(maps, p);
-    } else {
-      auto kern = stb::wgrad_tn_kernel<128>;
-      static bool configured = false;
-      if (!configured) {
-        if (int r = set_smem(kern, stb::WgradCfg<128>::SMEM_BYTES)) return r;
-        configured = true;
-      }
-      kern<<<grid, 384, stb::WgradCfg<128>::SMEM_BYTES, st>>>(maps, p);
-    }
-    STB_LAUNCH_CHECK("wgrad_tn");
+    if (workspace && workspace_elems < (long long)spb * B * R * N)
+      return fail(STB_ERR_ARG, "skinny_tn workspace too small (stb_skinny_tn_workspace)");
+    stb::WgradParams p{};
+    p.N = N;
+    p.K = R;
+    p.chunks = (S + 63) / 64;
+    // spb splits of `rows` tokens per batch; split y is batch y / spb, slab y of the workspace
+    p.splits = spb * B;
+    p.splits_per_group = spb;
+    p.kb_per_group = p.chunks;
+    p.kb_per_split = rows / 64;
+    p.alpha = alpha;
+    p.partial = workspace;
+    p.out_f32 = out;
+    if (int r = R <= 64 ? launch_wgrad<64, stb::WGRAD_OUT_F32_RN>(maps, p, st) : launch_wgrad<128, stb::WGRAD_OUT_F32_RN>(maps, p, st))
+      return r;
     if (workspace) {
       const long long n = (long long)R * N;
       stb::wgrad_reduce_slabs_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, (long long)num_sms() * 8), 256, 0, st>>>(
@@ -951,7 +883,6 @@ int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm
 template <int BN>
 static int launch_conv3x3(const void* x, const void* w, const void* bias, const void* res, void* out, int B, int H,
                           int W, int C_in, int C_out, int stride, cudaStream_t st) {
-  using Cfg = stb::GemmCfg<BN>;
   const int H_out = stride == 1 ? H : H / 2, W_out = stride == 1 ? W : W / 2;
   stb::GemmMaps maps;
   std::memset(&maps, 0, sizeof maps);
@@ -988,17 +919,7 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   p.conv_stride = stride;
   p.conv_pad = stride == 1 ? 1 : 0;
   p.conv_cblocks = C_in / 64;
-  auto kernel = stb::gemm_bf16_tn_kernel<BN, true>;
-  static bool configured = false;
-  if (!configured) {
-    if (int r = set_smem(kernel, Cfg::SMEM_BYTES)) return r;
-    configured = true;
-  }
-  const long long tiles = (long long)((W_out + 127) / 128) * p.num_batches * ((C_out + BN - 1) / BN);
-  const int grid = (int)std::min<long long>(tiles, num_sms());
-  kernel<<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
-  STB_LAUNCH_CHECK("conv3x3_nhwc");
-  return 0;
+  return launch_gemm_kernel<BN, true>(maps, p, st, "conv3x3_nhwc");
 }
 
 extern "C" {
@@ -1031,13 +952,9 @@ int stb_conv_in_3ch(const void* pixels, const void* w, const void* bias, void* o
     auto wt = static_cast<const __nv_bfloat16*>(w);
     auto bs = static_cast<const __nv_bfloat16*>(bias);
     auto o = static_cast<__nv_bfloat16*>(out);
-    static bool configured = false;
-    if (!configured) {
-      if (int r = set_smem(stb::conv_in_3ch_mma_kernel<256>, SMEM)) return r;
-      if (int r = set_smem(stb::conv_in_3ch_mma_kernel<128>, SMEM)) return r;
-      if (int r = set_smem(stb::conv_in_3ch_mma_kernel<64>, SMEM)) return r;
-      configured = true;
-    }
+    if (int r = set_smem<stb::conv_in_3ch_mma_kernel<256>>(SMEM)) return r;
+    if (int r = set_smem<stb::conv_in_3ch_mma_kernel<128>>(SMEM)) return r;
+    if (int r = set_smem<stb::conv_in_3ch_mma_kernel<64>>(SMEM)) return r;
     if (C == 256) stb::conv_in_3ch_mma_kernel<256><<<grid, 256, SMEM, st>>>(px, wt, bs, o, B, H, W);
     else if (C == 128) stb::conv_in_3ch_mma_kernel<128><<<grid, 256, SMEM, st>>>(px, wt, bs, o, B, H, W);
     else stb::conv_in_3ch_mma_kernel<64><<<grid, 256, SMEM, st>>>(px, wt, bs, o, B, H, W);
@@ -1047,13 +964,8 @@ int stb_conv_in_3ch(const void* pixels, const void* w, const void* bias, void* o
   const long long total = (long long)B * H * W * (C / 8);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 8);
   const int smem = (C * 27 + C) * (int)sizeof(float);
-  auto kernel = stb::conv_in_3ch_kernel;
-  static bool configured = false;
-  if (!configured) {
-    if (int r = set_smem(kernel, 512 * 28 * (int)sizeof(float))) return r;
-    configured = true;
-  }
-  kernel<<<grid, 256, smem, st>>>(static_cast<const __nv_bfloat16*>(pixels), static_cast<const __nv_bfloat16*>(w),
+  if (int r = set_smem<stb::conv_in_3ch_kernel>(512 * 28 * (int)sizeof(float))) return r;
+  stb::conv_in_3ch_kernel<<<grid, 256, smem, st>>>(static_cast<const __nv_bfloat16*>(pixels), static_cast<const __nv_bfloat16*>(w),
                                   static_cast<const __nv_bfloat16*>(bias), static_cast<__nv_bfloat16*>(out), B, H, W, C);
   STB_LAUNCH_CHECK("conv_in_3ch");
   return 0;

@@ -100,6 +100,44 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag
 #endif
 }
 
+// Ring of STAGES shared-memory stages between one TMA producer warp and the consumer warps, each stage guarded by a
+// full barrier (one arrival, plus the TMA transaction bytes) and an empty barrier (one arrival per consumer warp).
+// `bars` is the shared address of 2 * STAGES mbarriers: full[0, STAGES), then empty[0, STAGES).  Producer and consumers
+// each keep their own copy, whose {stage, phase} cursor walks the ring in the same order.
+// Inline only, and it never touches accumulator registers: a call inside a consumer loop makes ptxas serialize every
+// wgmma.
+template <int STAGES>
+struct StageRing {
+  uint32_t bars;
+  int stage = 0;
+  uint32_t phase = 0;
+
+  __device__ __forceinline__ uint32_t full_bar(int s) const { return bars + 8u * s; }
+  __device__ __forceinline__ uint32_t empty_bar(int s) const { return bars + 8u * (STAGES + s); }
+  // one thread, before the __syncthreads that publishes the barriers
+  __device__ __forceinline__ void init(uint32_t consumer_warps) const {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), consumer_warps);
+    }
+    fence_mbar_init();
+  }
+  __device__ __forceinline__ void advance() {
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+  // producer: until the consumers have released the current stage (the first lap passes at once)
+  __device__ __forceinline__ void wait_empty(int tag) const { mbar_wait(empty_bar(stage), phase ^ 1u, tag); }
+  // consumers: until the current stage's TMA bytes have landed
+  __device__ __forceinline__ void wait_full(int tag) const { mbar_wait(full_bar(stage), phase, tag); }
+  // consumers: lane 0 of each warp hands stage s back to the producer
+  __device__ __forceinline__ void release(int s) const {
+    if (lane_id() == 0) mbar_arrive(empty_bar(s));
+  }
+};
+
 // ----------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) — tile mode, mbarrier completion
 // ----------------------------------------------------------------------------------------------

@@ -947,4 +947,42 @@ cast_f32_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ o
     out[i] = __float2bfloat16(in[i]);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Per-(batch, column) reductions over the token axis, fp32 atomics into zeroed outputs:
+//   sum[b, d] = sum_s dy[b, s, d]            (gradient of an adaLN shift, bias gradients when summed over b on the host)
+//   dot[b, d] = sum_s dy[b, s, d] * z[b, s, d]   (gradient of an adaLN scale with z = LayerNorm(x), of a gate with z = the
+//                                                 gated linear output)
+// Either output may be null.  HBM-bound: reads dy (and z) once.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+colsum2_kernel(const __nv_bfloat16* __restrict__ dy, long long dy_b, long long dy_s, const __nv_bfloat16* __restrict__ z,
+               long long z_b, long long z_s, float* __restrict__ sum, float* __restrict__ dot, int B, int S, int D,
+               int rows_per_cta) {
+  const int vecs = D >> 3;
+  const int b = blockIdx.z;
+  const int s0 = blockIdx.y * rows_per_cta;
+  const int s1 = min(S, s0 + rows_per_cta);
+  for (int vi = blockIdx.x * blockDim.x + threadIdx.x; vi < vecs; vi += gridDim.x * blockDim.x) {
+    const int c = vi * 8;
+    float a[8] = {0, 0, 0, 0, 0, 0, 0, 0}, d[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int s = s0; s < s1; ++s) {
+      float g[8];
+      unpack8(*reinterpret_cast<const uint4*>(dy + b * dy_b + s * dy_s + c), g);
+      if (dot) {
+        float zz[8];
+        unpack8(*reinterpret_cast<const uint4*>(z + b * z_b + s * z_s + c), zz);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) d[j] += g[j] * zz[j];
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a[j] += g[j];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (sum) atomicAdd(sum + (long long)b * D + c + j, a[j]);
+      if (dot) atomicAdd(dot + (long long)b * D + c + j, d[j]);
+    }
+  }
+}
+
 }  // namespace stb

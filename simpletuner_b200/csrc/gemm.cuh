@@ -168,9 +168,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  StageRing<STAGES> ring{smem_base + STAGES * Cfg::STAGE_BYTES};
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -186,11 +184,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       tma_prefetch_desc(&maps.a[s]);
       tma_prefetch_desc(&maps.w[s]);
     }
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 8);   // one arrival per consumer warp
-    }
-    fence_mbar_init();
+    ring.init(8);
   }
   __syncthreads();
 
@@ -198,8 +192,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     // ===================== TMA producer (warp 0, one elected lane issues) =====================
     reg_dealloc<40>();
     if (warp == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int tm, tn;
         gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
@@ -208,34 +200,32 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         const int n0 = tn * BN;
         for (int seg = 0; seg < p.nseg; ++seg) {
           for (int kb = 0; kb < p.kblocks[seg]; ++kb) {
-            mbar_wait(empty_bar(stage), phase ^ 1u, 1);
-            const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+            ring.wait_empty(1);
+            const uint32_t sa = smem_base + ring.stage * Cfg::STAGE_BYTES;
+            const uint32_t full = ring.full_bar(ring.stage);
             if (elect_one()) {
-              mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+              mbar_arrive_expect_tx(full, Cfg::STAGE_BYTES);
               if constexpr (CONV) {
                 // implicit-GEMM 3x3 conv: shifted input window; TMA zero-fills the halo (x / y out of range)
                 const int tap = kb / p.conv_cblocks;
                 const int c0 = (kb - tap * p.conv_cblocks) * 64;
                 const int img = b / p.conv_h_out, yo = b - img * p.conv_h_out;
                 const int dy = tap / 3, dx = tap - dy * 3;
-                tma_load_4d(sa, &maps.a[0], full_bar(stage), c0, s0 * p.conv_stride + dx - p.conv_pad,
+                tma_load_4d(sa, &maps.a[0], full, c0, s0 * p.conv_stride + dx - p.conv_pad,
                             yo * p.conv_stride + dy - p.conv_pad, img);
               } else {
-                tma_load_3d(sa, &maps.a[seg], full_bar(stage), kb * 64, s0, b);
+                tma_load_3d(sa, &maps.a[seg], full, kb * 64, s0, b);
               }
               if (p.w_kn[seg]) {
 #pragma unroll
                 for (int g = 0; g < BN / 64; ++g)
-                  tma_load_2d(sa + Cfg::A_BYTES + g * 8192, &maps.w[seg], full_bar(stage), n0 + g * 64, kb * 64);
+                  tma_load_2d(sa + Cfg::A_BYTES + g * 8192, &maps.w[seg], full, n0 + g * 64, kb * 64);
               } else {
-                tma_load_2d(sa + Cfg::A_BYTES, &maps.w[seg], full_bar(stage), kb * 64, n0);
+                tma_load_2d(sa + Cfg::A_BYTES, &maps.w[seg], full, kb * 64, n0);
               }
             }
             __syncwarp();
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1u;
-            }
+            ring.advance();
           }
         }
       }
@@ -246,8 +236,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     const int cw = wg - 1;               // rows [64 cw, 64 cw + 64) of the tile
     const int wq = warp & 3;             // warp within the warpgroup: rows 16 wq .. 16 wq + 15
     float acc[BN / 2];
-    int stage = 0;
-    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int tm, tn;
       gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
@@ -259,9 +247,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       for (int seg = 0; seg < p.nseg; ++seg) {
         const bool wkn = __shfl_sync(0xffffffffu, p.w_kn[seg], 0) != 0;
         for (int kb = 0; kb < p.kblocks[seg]; ++kb) {
-          mbar_wait(full_bar(stage), phase, 3);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + cw * 8192;
-          const uint32_t sw = smem_base + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+          ring.wait_full(3);
+          const uint32_t sa = smem_base + ring.stage * Cfg::STAGE_BYTES + cw * 8192;
+          const uint32_t sw = smem_base + ring.stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
           // K past the end of the segment is zero-filled by TMA, so the last k-block runs all four K steps too
           wg_fence();
           if (wkn) {
@@ -276,17 +264,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
           // keep one k-block in flight; the one before it has retired -> free its slot
           wg_wait<1>();
           wg_fence_regs(acc);
-          if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
-          prev_stage = stage;
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
+          if (prev_stage >= 0) ring.release(prev_stage);
+          prev_stage = ring.stage;
+          ring.advance();
         }
       }
       wg_wait<0>();
       wg_fence_regs(acc);
-      if (lane == 0) mbar_arrive(empty_bar(prev_stage));
+      ring.release(prev_stage);
 
       // ===================== epilogue from registers =====================
       // accumulator layout (m64nBN): acc[4 i + 2 h + j] = row 16 wq + lane / 4 + 8 h, column 8 i + 2 (lane % 4) + j
