@@ -190,13 +190,13 @@ int set_smem(int bytes) {
 
 // ---------------------------------------------------------------- GEMM
 // One launch of the persistent GEMM for GEMM and conv3x3 alike: one CTA per SM, or one per tile when there are fewer
-template <int BN, bool CONV>
+template <int BN, int EPI, bool CONV>
 int launch_gemm_kernel(const stb::GemmMaps& maps, const stb::GemmParams& p, cudaStream_t st, const char* name) {
   using Cfg = stb::GemmCfg<BN>;
-  if (int r = set_smem<stb::gemm_bf16_tn_kernel<BN, CONV>>(Cfg::SMEM_BYTES)) return r;
+  if (int r = set_smem<stb::gemm_bf16_tn_kernel<BN, EPI, CONV>>(Cfg::SMEM_BYTES)) return r;
   const long long tiles = (long long)((p.rows_per_batch + Cfg::BM - 1) / Cfg::BM) * p.num_batches * ((p.N + BN - 1) / BN);
   const int grid = (int)std::min<long long>(tiles, num_sms());
-  stb::gemm_bf16_tn_kernel<BN, CONV><<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
+  stb::gemm_bf16_tn_kernel<BN, EPI, CONV><<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
   STB_LAUNCH_CHECK(name);
   return 0;
 }
@@ -210,7 +210,8 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   for (int s = 0; s < a->nseg; ++s) {
     const stb_gemm_seg& g = a->seg[s];
     if (g.K <= 0 || (g.K & 7)) return fail(STB_ERR_ARG, "segment %d: K=%d must be a positive multiple of 8", s, g.K);
-    if (int r = make_token_map(&maps.a[s], g.a, g.K, a->rows_per_batch, a->num_batches, g.a_row_stride, g.a_batch_stride, 128))
+    if (int r = make_token_map(&maps.a[s], g.a, g.K, a->rows_per_batch, a->num_batches, g.a_row_stride, g.a_batch_stride,
+                               stb::GemmCfg<BN>::BM))
       return r;
     if (g.w_kn) {   // [K, N] row-major: contraction index = row; staged as 64 x 64 MN-major boxes
       unsigned long long wd[2] = {(unsigned long long)a->N, (unsigned long long)g.K};
@@ -230,7 +231,6 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   p.num_batches = a->num_batches;
   p.N = a->N;
   p.nseg = a->nseg;
-  p.epi = a->epi;
   p.nan_to_num = a->nan_to_num;
   p.D = static_cast<__nv_bfloat16*>(a->d);
   p.d_batch_stride = a->d_batch_stride;
@@ -244,7 +244,16 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   p.aux = static_cast<__nv_bfloat16*>(a->aux);
   p.aux_batch_stride = a->aux_batch_stride;
   p.aux_row_stride = a->aux_row_stride;
-  return launch_gemm_kernel<BN, false>(maps, p, st, "gemm_bf16_tn");
+  switch (a->epi) {
+    case stb::EPI_STORE: return launch_gemm_kernel<BN, stb::EPI_STORE, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_GELU: return launch_gemm_kernel<BN, stb::EPI_GELU, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_GATE_RES: return launch_gemm_kernel<BN, stb::EPI_GATE_RES, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_MUL_DGELU: return launch_gemm_kernel<BN, stb::EPI_MUL_DGELU, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_ADD_RES: return launch_gemm_kernel<BN, stb::EPI_ADD_RES, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_MUL: return launch_gemm_kernel<BN, stb::EPI_MUL, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_QUICK_GELU: return launch_gemm_kernel<BN, stb::EPI_QUICK_GELU, false>(maps, p, st, "gemm_bf16_tn");
+  }
+  return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -318,15 +327,14 @@ int stb_gemm_bf16(const stb_gemm_args* a, void* stream) {
     return fail(STB_ERR_ARG, "aux must be 16-byte aligned, strides multiple of 8");
   if (a->epi < 0 || a->epi > 6) return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // every sm_90a tile is 128 rows (two 64-row consumer warpgroups); the row-tile request tile_mt is accepted and ignored
+  // a tile's height follows from its width (GemmCfg: 64 x 256, 128 x 128, 128 x 64); the row-tile request tile_mt is
+  // accepted and ignored
   if (a->tile_mt < 0 || a->tile_mt > 3) return fail(STB_ERR_ARG, "unsupported tile config MT=%d", a->tile_mt);
   int bn = a->tile_bn;
   if (bn == 0) {
-    bn = a->N > 128 ? 256 : (a->N > 64 ? 128 : 64);
-    // skinny-M problems (conditioning / modulation GEMMs, M = batch) and short grids: spread the weight stream over
-    // more SMs with narrower tiles while 256-wide tiles would leave SMs idle
-    const long long t256 = (long long)((a->rows_per_batch + 127) / 128) * a->num_batches * ((a->N + 255) / 256);
-    if (bn == 256 && t256 < num_sms()) bn = 128;
+    // 128 x 128 wherever N allows: on H100 it matched or beat 64 x 256 at every Flux projection shape, M = 512 included.
+    // Skinny M (modulation / conditioning GEMMs, a few rows per batch) streams W: 64 x 256 tiles waste no rows.
+    bn = a->N <= 64 ? 64 : (a->rows_per_batch <= 64 && a->N > 128 ? 256 : 128);
   }
   if (bn == 256) return launch_gemm<256>(a, st);
   if (bn == 128) return launch_gemm<128>(a, st);
@@ -890,7 +898,7 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
     unsigned long long d[4] = {(unsigned long long)C_in, (unsigned long long)W, (unsigned long long)H, (unsigned long long)B};
     unsigned long long sb[3] = {(unsigned long long)C_in * 2ull, (unsigned long long)W * C_in * 2ull,
                                 (unsigned long long)H * W * C_in * 2ull};
-    unsigned bx[4] = {64, (unsigned)(128 * stride), 1, 1};  // traversed span: 128 elements at stride `stride`
+    unsigned bx[4] = {64, (unsigned)(stb::GemmCfg<BN>::BM * stride), 1, 1};  // traversed span: BM elements at stride `stride`
     unsigned es[4] = {1, (unsigned)stride, 1, 1};
     if (int r = make_map_strided(&maps.a[0], x, 4, d, sb, bx, es)) return r;
   }
@@ -907,7 +915,6 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   p.N = C_out;
   p.nseg = 1;
   p.kblocks[0] = 9 * (C_in / 64);
-  p.epi = res ? stb::EPI_ADD_RES : stb::EPI_STORE;
   p.D = static_cast<__nv_bfloat16*>(out);
   p.d_batch_stride = (long long)W_out * C_out;
   p.d_row_stride = C_out;
@@ -919,7 +926,8 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   p.conv_stride = stride;
   p.conv_pad = stride == 1 ? 1 : 0;
   p.conv_cblocks = C_in / 64;
-  return launch_gemm_kernel<BN, true>(maps, p, st, "conv3x3_nhwc");
+  if (res) return launch_gemm_kernel<BN, stb::EPI_ADD_RES, true>(maps, p, st, "conv3x3_nhwc");
+  return launch_gemm_kernel<BN, stb::EPI_STORE, true>(maps, p, st, "conv3x3_nhwc");
 }
 
 extern "C" {

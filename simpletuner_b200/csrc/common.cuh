@@ -128,6 +128,13 @@ struct StageRing {
       phase ^= 1u;
     }
   }
+  // n advances at once: a consumer passing over the stages that another consumer takes
+  __device__ __forceinline__ void skip(int n) {
+    stage += n;
+    const int laps = stage / STAGES;
+    stage -= laps * STAGES;
+    phase ^= uint32_t(laps) & 1u;
+  }
   // producer: until the consumers have released the current stage (the first lap passes at once)
   __device__ __forceinline__ void wait_empty(int tag) const { mbar_wait(empty_bar(stage), phase ^ 1u, tag); }
   // consumers: until the current stage's TMA bytes have landed

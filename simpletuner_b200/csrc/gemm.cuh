@@ -9,10 +9,11 @@
 // become extra k-blocks of the same tile instead of extra kernels / extra HBM round trips.
 //
 // Roles (384 threads, three warpgroups): warpgroup 0 = TMA producer (one warp issues), warpgroups 1 and 2 =
-// consumers, each owning 64 rows of the CTA's 128 x BN tile: wgmma m64nBNk16 from shared memory, then the fused
-// epilogue straight from the accumulator registers.  The grid is persistent, so the producer already streams the
-// k-blocks of the next tile while the consumers run the epilogue of the current one.  CONV = true turns the A
-// operand into the shifted NHWC window of a 3x3 convolution (implicit GEMM, VAE encoder).
+// consumers in ping-pong: each owns whole BM x BN tiles (the CTA's tiles alternate between them), runs wgmma
+// m64nBNk16 from shared memory over BM / 64 row blocks, then the fused epilogue straight from the accumulator
+// registers.  While one consumer is in its epilogue the other one's MMAs keep the tensor pipe busy, and the grid is
+// persistent, so the producer streams the next tile's k-blocks meanwhile.  The epilogue kind is a template parameter.
+// CONV = true turns the A operand into the shifted NHWC window of a 3x3 convolution (implicit GEMM, VAE encoder).
 #pragma once
 #include <type_traits>
 #include "common.cuh"
@@ -37,7 +38,6 @@ struct GemmParams {
   int kblocks[3];  // ceil(K_seg / 64)
   int w_kn[3];        // 1: the segment's weight is given as [K, N] row-major (contraction index = row): the B operand is
                       // staged MN-major (64 k-rows x 64 n-columns SWIZZLE_128B boxes) — dgrad reads W itself, no W^T copy
-  int epi;
   int nan_to_num;
   __nv_bfloat16* D;
   long long d_batch_stride, d_row_stride;
@@ -49,25 +49,26 @@ struct GemmParams {
   __nv_bfloat16* aux;  // EPI_GELU / EPI_GATE_RES: written (optional); EPI_MUL_DGELU: read
   long long aux_batch_stride, aux_row_stride;
   // CONV mode (3x3 NHWC implicit GEMM): a "batch" is one output image row, a "row" an output pixel x.
-  // maps.a[0] is then a 4-D map (c, x, y, img) with box (64, 128, 1, 1) and x element-stride = conv_stride;
+  // maps.a[0] is then a 4-D map (c, x, y, img) with box (64, BM, 1, 1) and x element-stride = conv_stride;
   // k-block kb covers tap kb / conv_cblocks (dy = tap / 3, dx = tap % 3) and channels (kb % conv_cblocks) * 64.
   int conv_h_out, conv_stride, conv_pad, conv_cblocks;
 };
 
 struct GemmMaps {
-  CUtensorMap a[3];  // 3-D (k, s, b), box (64, 128, 1), SWIZZLE_128B
+  CUtensorMap a[3];  // 3-D (k, s, b), box (64, BM, 1), SWIZZLE_128B
   CUtensorMap w[3];  // 2-D (k, n),   box (64, BN),      SWIZZLE_128B;  w_kn: 2-D (n, k), box (64, 64)
 };
 
+// A consumer's tile is BM x BN with 128 fp32 accumulators per thread at BN 128 and 256 (64 at BN 64).
 template <int BN>
 struct GemmCfg {
-  static constexpr int BM = 128;
+  static constexpr int BM = BN == 256 ? 64 : 128;
   static constexpr int BK = 64;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int W_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
   static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*ring and order barriers*/;
 };
 
 __device__ __forceinline__ float gemm_bf16r(float x) { return __bfloat162float(__float2bfloat16(x)); }
@@ -94,25 +95,44 @@ __device__ __forceinline__ void ld_bf16x2(const __nv_bfloat16* p, bool two, floa
     b = 0.f;
   }
 }
+// the pair as one word; a lone last column reads one element and leaves the high half zero
+__device__ __forceinline__ uint32_t ld_pair_word(const __nv_bfloat16* p, bool two) {
+  return two ? *reinterpret_cast<const uint32_t*>(p) : uint32_t(__bfloat16_as_ushort(p[0]));
+}
 __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, bool two, float a, float b) {
   if (two) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
   else p[0] = __float2bfloat16(a);
 }
 
-// Fused epilogue of two adjacent columns (n, n+1) of one output row; f = accumulator + bias.
-__device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s, int n, bool two, float f0, float f1) {
+// The epilogues that read an [M, N] operand element for element: res (GATE_RES, ADD_RES) or aux (MUL_DGELU, MUL).
+// The epilogue loads those words ahead, a chunk of column groups at a time, so that their latencies overlap.
+template <int EPI>
+constexpr bool kGemmEpiReadsRows = EPI == EPI_GATE_RES || EPI == EPI_ADD_RES || EPI == EPI_MUL_DGELU || EPI == EPI_MUL;
+template <int EPI>
+__device__ __forceinline__ const __nv_bfloat16* gemm_epi_row_operand(const GemmParams& p, int b, int s, int n) {
+  if constexpr (EPI == EPI_GATE_RES || EPI == EPI_ADD_RES)
+    return p.res + (long long)b * p.res_batch_stride + (long long)s * p.res_row_stride + n;
+  else
+    return p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride + n;
+}
+
+// Fused epilogue of two adjacent columns (n, n+1) of one output row; f = accumulator + bias, x = the pair's res / aux
+// word for the epilogues that read one.
+template <int EPI>
+__device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s, int n, bool two, float f0, float f1,
+                                              uint32_t x) {
   const long long drow = (long long)b * p.d_batch_stride + (long long)s * p.d_row_stride;
   __nv_bfloat16* xp = p.aux ? p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride + n : nullptr;
-  if (p.epi == EPI_GELU) {
+  if constexpr (EPI == EPI_GELU) {
     if (xp) st_bf16x2(xp, two, f0, f1);
     // the activation sees the bf16-rounded pre-activation, as the reference's
     // nn.Linear -> nn.GELU chain does (bf16 tensor between the two modules)
     f0 = gelu_tanh(gemm_bf16r(f0));
     f1 = gelu_tanh(gemm_bf16r(f1));
-  } else if (p.epi == EPI_GATE_RES) {
-    float g0, g1, r0, r1;
+  } else if constexpr (EPI == EPI_GATE_RES) {
+    float g0, g1;
     ld_bf16x2(p.gate + (long long)b * p.gate_batch_stride + n, two, g0, g1);
-    ld_bf16x2(p.res + (long long)b * p.res_batch_stride + (long long)s * p.res_row_stride + n, two, r0, r1);
+    const float r0 = bf16_lo(x), r1 = bf16_hi(x);
     // full fine-tune: keep the (bf16) linear output — the gate gradient is sum_s dOut * y
     if (xp) st_bf16x2(xp, two, f0, f1);
     // reference order: bias -> (bf16 linear output) -> gate * y -> residual + (...)
@@ -130,25 +150,19 @@ __device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s,
     }
     f0 = o[0];
     f1 = o[1];
-  } else if (p.epi == EPI_MUL_DGELU) {
-    float x0, x1;
-    ld_bf16x2(xp, two, x0, x1);
-    f0 *= gelu_tanh_grad(x0);
-    f1 *= gelu_tanh_grad(x1);
-  } else if (p.epi == EPI_MUL) {
-    float x0, x1;
-    ld_bf16x2(xp, two, x0, x1);
-    f0 = gemm_bf16r(f0) * x0;
-    f1 = gemm_bf16r(f1) * x1;
-  } else if (p.epi == EPI_QUICK_GELU) {
+  } else if constexpr (EPI == EPI_MUL_DGELU) {
+    f0 *= gelu_tanh_grad(bf16_lo(x));
+    f1 *= gelu_tanh_grad(bf16_hi(x));
+  } else if constexpr (EPI == EPI_MUL) {
+    f0 = gemm_bf16r(f0) * bf16_lo(x);
+    f1 = gemm_bf16r(f1) * bf16_hi(x);
+  } else if constexpr (EPI == EPI_QUICK_GELU) {
     const float y0 = gemm_bf16r(f0), y1 = gemm_bf16r(f1);
     f0 = y0 / (1.f + __expf(-1.702f * y0));
     f1 = y1 / (1.f + __expf(-1.702f * y1));
-  } else if (p.epi == EPI_ADD_RES) {
-    float r0, r1;
-    ld_bf16x2(p.res + (long long)b * p.res_batch_stride + (long long)s * p.res_row_stride + n, two, r0, r1);
-    f0 += r0;
-    f1 += r1;
+  } else if constexpr (EPI == EPI_ADD_RES) {
+    f0 += bf16_lo(x);
+    f1 += bf16_hi(x);
   }
   st_bf16x2(p.D + drow + n, two, f0, f1);
 }
@@ -160,15 +174,18 @@ __device__ __forceinline__ void gemm_wgmma(float (&acc)[BN / 2], uint64_t a, uin
   else wgmma_ss_n64<0, TB>(acc, a, b, accumulate);
 }
 
-template <int BN, bool CONV = false>
+template <int BN, int EPI, bool CONV = false>
 __global__ void __launch_bounds__(384, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int MI = Cfg::BM / 64;   // m64 row blocks of a tile
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   StageRing<STAGES> ring{smem_base + STAGES * Cfg::STAGE_BYTES};
+  // order[c]: consumer c may start its next mainloop (the other consumer has waited on every stage of the tile before)
+  const uint32_t order_bars = ring.bars + 16u * STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -178,13 +195,18 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   const int tiles_m = tiles_per_batch * p.num_batches;
   const int tiles_n = (p.N + BN - 1) / BN;
   const int num_tiles = tiles_m * tiles_n;
+  int nk = 0;   // k-blocks per tile
+  for (int s = 0; s < p.nseg; ++s) nk += p.kblocks[s];
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nseg; ++s) {
       tma_prefetch_desc(&maps.a[s]);
       tma_prefetch_desc(&maps.w[s]);
     }
-    ring.init(8);
+    ring.init(4);   // each stage belongs to one consumer warpgroup's tile
+    mbar_init(order_bars, 4);
+    mbar_init(order_bars + 8, 4);
+    fence_mbar_init();
   }
   __syncthreads();
 
@@ -231,16 +253,26 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       }
     }
   } else {
-    // ===================== consumers: 64 rows each =====================
+    // ===================== consumers: ping-pong over whole tiles =====================
+    // Consumer cw takes the CTA's tiles cw, cw + 2, ...; the producer fills the ring in tile order, so each consumer
+    // passes over the other's nk stages.  Its epilogue then runs while the other consumer's MMAs use the tensor pipe.
     reg_alloc<232>();
-    const int cw = wg - 1;               // rows [64 cw, 64 cw + 64) of the tile
-    const int wq = warp & 3;             // warp within the warpgroup: rows 16 wq .. 16 wq + 15
-    float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int cw = wg - 1;
+    const int wq = warp & 3;             // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of each m64 block
+    uint32_t order_phase = 0;
+    if (cw == 1) ring.skip(nk);
+    float acc[MI][BN / 2];
+    for (int tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
+      // The other consumer has waited on every stage of the tile before this one, so the producer has filled them all
+      // and this consumer's full-barrier waits are at most one lap ahead of the barriers' phases.
+      if (tile != (int)blockIdx.x) {
+        mbar_wait(order_bars + 8u * cw, order_phase, 4);
+        order_phase ^= 1u;
+      }
       int tm, tn;
       gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
       const int b = tm / tiles_per_batch;
-      const int s0 = (tm - b * tiles_per_batch) * Cfg::BM + cw * 64;
+      const int s0 = (tm - b * tiles_per_batch) * Cfg::BM;
       const int n0 = tn * BN;
       uint32_t accumulate = 0;
       int prev_stage = -1;
@@ -248,46 +280,82 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         const bool wkn = __shfl_sync(0xffffffffu, p.w_kn[seg], 0) != 0;
         for (int kb = 0; kb < p.kblocks[seg]; ++kb) {
           ring.wait_full(3);
-          const uint32_t sa = smem_base + ring.stage * Cfg::STAGE_BYTES + cw * 8192;
-          const uint32_t sw = smem_base + ring.stage * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+          const uint32_t sa = smem_base + ring.stage * Cfg::STAGE_BYTES;
+          const uint32_t sw = sa + Cfg::A_BYTES;
           // K past the end of the segment is zero-filled by TMA, so the last k-block runs all four K steps too
           wg_fence();
           if (wkn) {
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) gemm_wgmma<BN, 1>(acc, sdesc_k(sa, kk * 32), sdesc_mn(sw, kk * 2048, 8192), kk > 0 ? 1u : accumulate);
+            for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+              for (int mi = 0; mi < MI; ++mi)
+                gemm_wgmma<BN, 1>(acc[mi], sdesc_k(sa + mi * 8192, kk * 32), sdesc_mn(sw, kk * 2048, 8192),
+                                  kk > 0 ? 1u : accumulate);
           } else {
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) gemm_wgmma<BN, 0>(acc, sdesc_k(sa, kk * 32), sdesc_k(sw, kk * 32), kk > 0 ? 1u : accumulate);
+            for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+              for (int mi = 0; mi < MI; ++mi)
+                gemm_wgmma<BN, 0>(acc[mi], sdesc_k(sa + mi * 8192, kk * 32), sdesc_k(sw, kk * 32),
+                                  kk > 0 ? 1u : accumulate);
           }
           accumulate = 1;
           wg_commit();
           // keep one k-block in flight; the one before it has retired -> free its slot
           wg_wait<1>();
-          wg_fence_regs(acc);
+#pragma unroll
+          for (int mi = 0; mi < MI; ++mi) wg_fence_regs(acc[mi]);
           if (prev_stage >= 0) ring.release(prev_stage);
           prev_stage = ring.stage;
           ring.advance();
         }
       }
+      // every stage of this tile has landed: the other consumer may start on the next tile
+      if (tile + (int)gridDim.x < num_tiles && lane == 0) mbar_arrive(order_bars + 8u * (cw ^ 1));
+      ring.skip(nk);
       wg_wait<0>();
-      wg_fence_regs(acc);
+#pragma unroll
+      for (int mi = 0; mi < MI; ++mi) wg_fence_regs(acc[mi]);
       ring.release(prev_stage);
 
       // ===================== epilogue from registers =====================
-      // accumulator layout (m64nBN): acc[4 i + 2 h + j] = row 16 wq + lane / 4 + 8 h, column 8 i + 2 (lane % 4) + j
-      const int r_lo = s0 + wq * 16 + (lane >> 2);
+      // accumulator layout (m64nBN): acc[mi][4 i + 2 h + j] = row 64 mi + 16 wq + lane / 4 + 8 h,
+      // column 8 i + 2 (lane % 4) + j
+      constexpr int CH = BN / 8 < 8 ? BN / 8 : 8;   // column groups whose res / aux words are loaded together
+      const bool b_ok = b < p.num_batches;
 #pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int n = n0 + 8 * i + 2 * (lane & 3);
-        if (n < p.N) {
-          const bool two = n + 1 < p.N;
-          float b0 = 0.f, b1 = 0.f;
-          if (p.bias) ld_bf16x2(p.bias + n, two, b0, b1);
+      for (int mi = 0; mi < MI; ++mi) {
+        const int r_lo = s0 + mi * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int s = r_lo + 8 * h;
-            if (s < p.rows_per_batch && b < p.num_batches)
-              gemm_epi_pair(p, b, s, n, two, acc[4 * i + 2 * h] + b0, acc[4 * i + 2 * h + 1] + b1);
+        for (int i0 = 0; i0 < BN / 8; i0 += CH) {
+          uint32_t x[CH][2];
+#pragma unroll
+          for (int c = 0; c < CH; ++c) {
+            const int n = n0 + 8 * (i0 + c) + 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              x[c][h] = 0;
+              if constexpr (kGemmEpiReadsRows<EPI>)
+                if (n < p.N && r_lo + 8 * h < p.rows_per_batch && b_ok)
+                  x[c][h] = ld_pair_word(gemm_epi_row_operand<EPI>(p, b, r_lo + 8 * h, n), n + 1 < p.N);
+            }
+          }
+#pragma unroll
+          for (int c = 0; c < CH; ++c) {
+            const int i = i0 + c;
+            const int n = n0 + 8 * i + 2 * (lane & 3);
+            if (n < p.N) {
+              const bool two = n + 1 < p.N;
+              float b0 = 0.f, b1 = 0.f;
+              if (p.bias) ld_bf16x2(p.bias + n, two, b0, b1);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int s = r_lo + 8 * h;
+                if (s < p.rows_per_batch && b_ok)
+                  gemm_epi_pair<EPI>(p, b, s, n, two, acc[mi][4 * i + 2 * h] + b0, acc[mi][4 * i + 2 * h + 1] + b1,
+                                     x[c][h]);
+              }
+            }
           }
         }
       }

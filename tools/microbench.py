@@ -1,5 +1,8 @@
 #!/usr/bin/env python
-"""Kernel micro-benchmarks (CUDA events, rotating buffers larger than L2) -> bench_out/microbench.json."""
+"""Kernel micro-benchmarks (CUDA events, rotating buffers larger than L2) -> bench_out/microbench.json.
+
+python tools/microbench.py [flux] [gemm] [attn] [--out DIR]; `flux` times the large GEMMs of the batch-1 flux_lora step."""
+import hashlib
 import json
 import sys
 import time
@@ -50,6 +53,112 @@ def bench_gemm(M, N, K, tile, nbuf=3, epi=ops.EPI_STORE):
             "cublas_ms": round(ms_ref, 4), "cublas_tflops": round(2.0 * M * N * K / ms_ref / 1e9, 1)}
 
 
+# The large GEMMs of one batch-1 flux_lora step (1024^2: 4096 image + 512 text tokens; single blocks run both as
+# 4608 rows).  K segments: a trailing 16 is the rank-16 LoRA k-block; w_kn marks the dgrads, which read the forward
+# weight as [K, N].  Columns: block, name, M, N, K segments, w_kn, epilogue, bias, nan_to_num.
+E = ops
+FLUX_GEMMS = [
+    ("single", "qkv", 4608, 9216, [3072, 16], False, E.EPI_STORE, True, False),
+    ("single", "fc1", 4608, 12288, [3072], False, E.EPI_GELU, True, False),
+    ("single", "proj_out", 4608, 3072, [3072, 12288], False, E.EPI_GATE_RES, True, True),
+    ("single", "d_o", 4608, 3072, [3072], True, E.EPI_STORE, False, False),
+    ("single", "d_pre", 4608, 12288, [3072], True, E.EPI_MUL_DGELU, False, False),
+    ("single", "d_nh", 4608, 3072, [12288, 9216, 16], True, E.EPI_STORE, False, False),
+] + [
+    (blk, name, M, N, segs, kn, epi, bias, False)
+    for blk, M in (("double_img", 4096), ("double_txt", 512))
+    for name, N, segs, kn, epi, bias in (
+        ("qkv", 9216, [3072, 16], False, E.EPI_STORE, True),
+        ("out", 3072, [3072, 16], False, E.EPI_GATE_RES, True),
+        ("fc1", 12288, [3072], False, E.EPI_GELU, True),
+        ("fc2", 3072, [12288], False, E.EPI_GATE_RES, True),
+        ("d_pre", 12288, [3072], True, E.EPI_MUL_DGELU, False),
+        ("d_nh2", 3072, [12288], True, E.EPI_STORE, False),
+        ("d_o", 3072, [3072, 16], True, E.EPI_STORE, False),
+        ("d_nh", 3072, [9216, 16], True, E.EPI_STORE, False),
+    )
+]
+
+
+def _digest(t):
+    return hashlib.sha256(t.contiguous().view(torch.uint8).cpu().numpy().tobytes()).hexdigest()[:16]
+
+
+def bench_flux_gemm(blk, name, M, N, segs, kn, epi, bias, nan, nbuf=3, tiles=(0,), iters=20):
+    """Our kernel with the step's epilogue, the same with a plain store (no bias), and torch.matmul at the same M, N and
+    summed K; rotating operand sets.  `digest` fingerprints each output on seeded inputs, for old-vs-new comparison."""
+    g = torch.Generator(device="cuda").manual_seed(1234)
+    rnd = lambda *s, sc=1.0: (torch.randn(*s, device="cuda", generator=g) * sc).bfloat16()  # noqa: E731
+    sets = []
+    for _ in range(nbuf):
+        A = [rnd(M, k) for k in segs]
+        W = [ops.WT(rnd(k, N, sc=0.02)) if kn else rnd(N, k, sc=0.02) for k in segs]
+        sets.append((A, W))
+    K = sum(segs)
+    b = rnd(N) if bias else None
+    gate = rnd(1, N) if epi == E.EPI_GATE_RES else None
+    res = rnd(M, N) if epi == E.EPI_GATE_RES else None
+    aux = rnd(M, N) if epi in (E.EPI_GELU, E.EPI_MUL_DGELU) else None
+    out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+    flop = 2.0 * M * N * K
+    r = {"kind": "flux_gemm", "block": blk, "name": name, "M": M, "N": N, "K": segs, "w_kn": kn, "epi": epi}
+    i = [0]
+
+    def run(j, tile, e, with_bias):
+        A, W = sets[j]
+        ops.gemm(A, W, b if with_bias else None, out=out, epi=e, gate=gate if e == E.EPI_GATE_RES else None,
+                 res=res if e == E.EPI_GATE_RES else None, aux=aux if e in (E.EPI_GELU, E.EPI_MUL_DGELU) else None,
+                 nan_to_num=nan, tile=(0, tile))
+
+    def rot(tile, e, with_bias):
+        def fn():
+            i[0] += 1
+            run(i[0] % nbuf, tile, e, with_bias)
+        return fn
+
+    for tile in tiles:
+        sfx = "" if tile == 0 else f"_bn{tile}"
+        ms = timeit(rot(tile, epi, bias), iters=iters, warm=5)
+        ms_store = timeit(rot(tile, E.EPI_STORE, False), iters=iters, warm=5)
+        run(0, tile, epi, bias)
+        if aux is not None and epi == E.EPI_GELU:
+            r["digest_aux" + sfx] = _digest(aux)
+        r["digest" + sfx] = _digest(out)
+        run(0, tile, E.EPI_STORE, False)
+        r["digest_store" + sfx] = _digest(out)
+        r.update({"ms" + sfx: round(ms, 4), "tflops" + sfx: round(flop / ms / 1e9, 1),
+                  "store_ms" + sfx: round(ms_store, 4), "store_tflops" + sfx: round(flop / ms_store / 1e9, 1)})
+    A2 = [torch.cat(A, 1) for A, _ in sets]
+    W2 = [torch.cat([w.w.t() if kn else w for w in W], 1) for _, W in sets]
+
+    def ref():
+        i[0] += 1
+        j = i[0] % nbuf
+        torch.matmul(A2[j], W2[j].t(), out=out)
+
+    ms_ref = timeit(ref, iters=iters, warm=5)
+    r.update({"cublas_ms": round(ms_ref, 4), "cublas_tflops": round(flop / ms_ref / 1e9, 1)})
+    del sets, A2, W2
+    torch.cuda.empty_cache()
+    return r
+
+
+def flux_gemms():
+    res = []
+    for row in FLUX_GEMMS:
+        # every tile width at M = 512 (text stream), the two wide ones elsewhere: the tile choice in stb_gemm_bf16
+        tiles = (0, 64, 128, 256) if row[2] == 512 else (0, 128, 256)
+        res.append(bench_flux_gemm(*row, tiles=tiles))
+    # per-k-block slope and per-tile intercept: plain store at three depths
+    for N in (3072, 12288):
+        for K in (3072, 6144, 12288):
+            res.append(bench_flux_gemm("ksweep", f"k{K}", 4608, N, [K], False, E.EPI_STORE, False, False))
+    # M = 1 modulation GEMM (6 x 3072 outputs) at every tile width
+    res.append(bench_flux_gemm("mod", "mod", 1, 18432, [3072], False, E.EPI_STORE, True, False, tiles=(0, 64, 128, 256),
+                               iters=100))
+    return res
+
+
 def bench_attn(B, H, S, HD=128, bwd=True):
     q = torch.randn(B, S, H, HD, device="cuda").bfloat16()
     k = torch.randn(B, S, H, HD, device="cuda").bfloat16()
@@ -75,7 +184,17 @@ def bench_attn(B, H, S, HD=128, bwd=True):
 
 def main():
     res = []
-    which = sys.argv[1:] or ["gemm", "attn"]
+    args = sys.argv[1:]
+    out = ROOT / "bench_out"
+    if "--out" in args:
+        k = args.index("--out")
+        out = Path(args[k + 1])
+        del args[k:k + 2]
+    which = args or ["gemm", "attn"]
+    if "flux" in which:
+        for r in flux_gemms():
+            print(json.dumps(r), flush=True)
+            res.append(r)
     if "gemm" in which:
         for (M, N, K) in [(16384, 3072, 3072), (16384, 12288, 3072), (16384, 3072, 12288), (2048, 3072, 3072), (16384, 9216, 3072)]:
             for tile in [(1, 256), (2, 256), (3, 256)]:
@@ -93,8 +212,7 @@ def main():
                 r = {"kind": "attn", "B": B, "H": H, "S": S, "error": str(e)[:200]}
             print(json.dumps(r), flush=True)
             res.append(r)
-    out = ROOT / "bench_out"
-    out.mkdir(exist_ok=True)
+    out.mkdir(parents=True, exist_ok=True)
     (out / f"microbench_{int(time.time())}.json").write_text(json.dumps(res, indent=1))
 
 

@@ -19,7 +19,7 @@ if cfg == "sd3_fullft":
     batches = [bench.synth_batch_sd3(8, dev, hw, seed=i) for i, hw in enumerate(bench.SD3_BUCKETS[:2])]
 else:
     w = bench.build_model(dev)
-    batches = [bench.synth_batch(4, dev, seed=i) for i in range(2)]
+    batches = [bench.synth_batch(1, dev, seed=i) for i in range(2)]   # the bench's flux_lora default batch
 params = [p for p in w._denoiser().parameters() if p.requires_grad]
 opt = AdamWBF16(params, lr=1e-4, weight_decay=1e-2, eps=1e-6, seed=1)
 step = TrainStep(w, opt)
