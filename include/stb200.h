@@ -75,8 +75,10 @@ typedef struct {
   long long res_batch_stride, res_row_stride;
   void* aux;
   long long aux_batch_stride, aux_row_stride;
-  int tile_mt, tile_bn; /* 0 = pick automatically; else BN in {64,128,256}.  MT (0..3) is accepted for compatibility;
-                           every tile is 128 rows */
+  int tile_mt, tile_bn; /* 0 = pick automatically; else BN in {64,128,256} (tiles of 128 rows, 64 at BN 256).
+                           MT: 1 = single CTAs, 2 = 2-CTA clusters multicasting the shared W tile (BN 128 only; other
+                           widths run single CTAs), 0 = automatic (clusters for the GELU / dGELU epilogues at 16 or
+                           more 128-row tiles).  The results are the same bits either way. */
 } stb_gemm_args;
 
 int stb_gemm_bf16(const stb_gemm_args* args, void* stream);

@@ -189,20 +189,49 @@ int set_smem(int bytes) {
 }
 
 // ---------------------------------------------------------------- GEMM
-// One launch of the persistent GEMM for GEMM and conv3x3 alike: one CTA per SM, or one per tile when there are fewer
-template <int BN, int EPI, bool CONV>
+// One launch of the persistent GEMM for GEMM and conv3x3 alike: one CTA per SM, or one per tile when there are fewer.
+// CLUSTER = 2: one 2-CTA cluster per pair tile, at most as many as the device can hold at once (the GPCs' SM counts
+// decide how many pairs of SMs there are, so it is asked, once per kernel).
+template <int BN, int EPI, bool CONV, int CLUSTER = 1>
 int launch_gemm_kernel(const stb::GemmMaps& maps, const stb::GemmParams& p, cudaStream_t st, const char* name) {
   using Cfg = stb::GemmCfg<BN>;
-  if (int r = set_smem<stb::gemm_bf16_tn_kernel<BN, EPI, CONV>>(Cfg::SMEM_BYTES)) return r;
-  const long long tiles = (long long)((p.rows_per_batch + Cfg::BM - 1) / Cfg::BM) * p.num_batches * ((p.N + BN - 1) / BN);
-  const int grid = (int)std::min<long long>(tiles, num_sms());
-  stb::gemm_bf16_tn_kernel<BN, EPI, CONV><<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
+  constexpr auto kernel = stb::gemm_bf16_tn_kernel<BN, EPI, CONV, CLUSTER>;
+  if (int r = set_smem<kernel>(Cfg::SMEM_BYTES)) return r;
+  const long long tiles_m = (long long)((p.rows_per_batch + Cfg::BM - 1) / Cfg::BM) * p.num_batches;
+  const long long units = (tiles_m + CLUSTER - 1) / CLUSTER * ((p.N + BN - 1) / BN);
+  if constexpr (CLUSTER == 1) {
+    const int grid = (int)std::min<long long>(units, num_sms());
+    kernel<<<grid, 384, Cfg::SMEM_BYTES, st>>>(maps, p);
+  } else {
+    cudaLaunchConfig_t cfg;
+    std::memset(&cfg, 0, sizeof cfg);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CLUSTER;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.blockDim = dim3(384);
+    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    static std::atomic<int> max_clusters{0};
+    int mc = max_clusters.load(std::memory_order_acquire);
+    if (mc == 0) {
+      cfg.gridDim = dim3(CLUSTER * (num_sms() / CLUSTER));
+      STB_CUDA(cudaOccupancyMaxActiveClusters(&mc, kernel, &cfg));
+      if (mc < 1) return fail(STB_ERR_CUDA, "%s: no %d-CTA cluster of this kernel fits on the device", name, CLUSTER);
+      max_clusters.store(mc, std::memory_order_release);
+    }
+    cfg.gridDim = dim3((unsigned)(CLUSTER * std::min<long long>(units, mc)));
+    STB_CUDA(cudaLaunchKernelEx(&cfg, kernel, maps, p));
+  }
   STB_LAUNCH_CHECK(name);
   return 0;
 }
 
 template <int BN>
-int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
+int launch_gemm(const stb_gemm_args* a, cudaStream_t st, bool cluster) {
   stb::GemmMaps maps;
   std::memset(&maps, 0, sizeof maps);
   stb::GemmParams p;
@@ -221,7 +250,7 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
     } else {
       unsigned long long wd[2] = {(unsigned long long)g.K, (unsigned long long)a->N};
       unsigned long long ws[1] = {(unsigned long long)g.w_row_stride * 2ull};
-      unsigned wb[2] = {64, (unsigned)BN};
+      unsigned wb[2] = {64, cluster ? 64u : (unsigned)BN};   // a cluster CTA loads half of the W tile's rows
       if (int r = make_map(&maps.w[s], g.w, 2, wd, ws, wb)) return r;
     }
     p.w_kn[s] = g.w_kn ? 1 : 0;
@@ -244,14 +273,21 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st) {
   p.aux = static_cast<__nv_bfloat16*>(a->aux);
   p.aux_batch_stride = a->aux_batch_stride;
   p.aux_row_stride = a->aux_row_stride;
+  // the 2-CTA cluster kernels exist at BN 128 only
+  auto go = [&](auto epi) -> int {
+    constexpr int EPI = decltype(epi)::value;
+    if constexpr (BN == 128)
+      if (cluster) return launch_gemm_kernel<BN, EPI, false, 2>(maps, p, st, "gemm_bf16_tn_cluster");
+    return launch_gemm_kernel<BN, EPI, false>(maps, p, st, "gemm_bf16_tn");
+  };
   switch (a->epi) {
-    case stb::EPI_STORE: return launch_gemm_kernel<BN, stb::EPI_STORE, false>(maps, p, st, "gemm_bf16_tn");
-    case stb::EPI_GELU: return launch_gemm_kernel<BN, stb::EPI_GELU, false>(maps, p, st, "gemm_bf16_tn");
-    case stb::EPI_GATE_RES: return launch_gemm_kernel<BN, stb::EPI_GATE_RES, false>(maps, p, st, "gemm_bf16_tn");
-    case stb::EPI_MUL_DGELU: return launch_gemm_kernel<BN, stb::EPI_MUL_DGELU, false>(maps, p, st, "gemm_bf16_tn");
-    case stb::EPI_ADD_RES: return launch_gemm_kernel<BN, stb::EPI_ADD_RES, false>(maps, p, st, "gemm_bf16_tn");
-    case stb::EPI_MUL: return launch_gemm_kernel<BN, stb::EPI_MUL, false>(maps, p, st, "gemm_bf16_tn");
-    case stb::EPI_QUICK_GELU: return launch_gemm_kernel<BN, stb::EPI_QUICK_GELU, false>(maps, p, st, "gemm_bf16_tn");
+    case stb::EPI_STORE: return go(std::integral_constant<int, stb::EPI_STORE>{});
+    case stb::EPI_GELU: return go(std::integral_constant<int, stb::EPI_GELU>{});
+    case stb::EPI_GATE_RES: return go(std::integral_constant<int, stb::EPI_GATE_RES>{});
+    case stb::EPI_MUL_DGELU: return go(std::integral_constant<int, stb::EPI_MUL_DGELU>{});
+    case stb::EPI_ADD_RES: return go(std::integral_constant<int, stb::EPI_ADD_RES>{});
+    case stb::EPI_MUL: return go(std::integral_constant<int, stb::EPI_MUL>{});
+    case stb::EPI_QUICK_GELU: return go(std::integral_constant<int, stb::EPI_QUICK_GELU>{});
   }
   return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
 }
@@ -327,18 +363,25 @@ int stb_gemm_bf16(const stb_gemm_args* a, void* stream) {
     return fail(STB_ERR_ARG, "aux must be 16-byte aligned, strides multiple of 8");
   if (a->epi < 0 || a->epi > 6) return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // a tile's height follows from its width (GemmCfg: 64 x 256, 128 x 128, 128 x 64); the row-tile request tile_mt is
-  // accepted and ignored
-  if (a->tile_mt < 0 || a->tile_mt > 3) return fail(STB_ERR_ARG, "unsupported tile config MT=%d", a->tile_mt);
+  // a tile's height follows from its width (GemmCfg: 64 x 256, 128 x 128, 128 x 64); tile_mt = 1 / 2 forces single CTAs /
+  // 2-CTA clusters at BN 128, the only width that has the cluster kernel
+  if (a->tile_mt < 0 || a->tile_mt > 2) return fail(STB_ERR_ARG, "unsupported tile config MT=%d", a->tile_mt);
   int bn = a->tile_bn;
   if (bn == 0) {
     // 128 x 128 wherever N allows: on H100 it matched or beat 64 x 256 at every Flux projection shape, M = 512 included.
     // Skinny M (modulation / conditioning GEMMs, a few rows per batch) streams W: 64 x 256 tiles waste no rows.
     bn = a->N <= 64 ? 64 : (a->rows_per_batch <= 64 && a->N > 128 ? 256 : 128);
   }
-  if (bn == 256) return launch_gemm<256>(a, st);
-  if (bn == 128) return launch_gemm<128>(a, st);
-  if (bn == 64) return launch_gemm<64>(a, st);
+  if (bn == 256) return launch_gemm<256>(a, st, false);
+  // Automatic: clusters for the GELU and dGELU epilogues at 16 or more m-tiles, where they measured 7-9 % faster on H100
+  // (Flux fc1 / d_pre at M = 4096 and 4608, DESIGN.md 2.1); single CTAs elsewhere, where clusters were up to 5 % slower.
+  if (bn == 128) {
+    const long long tiles_m = (long long)((a->rows_per_batch + 127) / 128) * a->num_batches;
+    const bool cluster = a->tile_mt == 2 || (a->tile_mt == 0 && tiles_m >= 16 &&
+                                             (a->epi == STB_EPI_GELU || a->epi == STB_EPI_MUL_DGELU));
+    return launch_gemm<128>(a, st, cluster);
+  }
+  if (bn == 64) return launch_gemm<64>(a, st, false);
   return fail(STB_ERR_ARG, "unsupported tile config BN=%d", bn);
 }
 

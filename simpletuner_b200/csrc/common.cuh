@@ -71,6 +71,32 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 
+// ----------------------------------------------------------------------------------------------
+// clusters
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster: release what this thread wrote (barrier init, remote arrives), acquire
+// what the others did
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared offset as `bar` in cluster CTA `rank`.  Default (.release.cta) semantics:
+// the stage it hands back was read by wgmma, complete at the wait_group before it, and .release.cluster would compile to
+// a GPU-wide memory barrier that waits for the epilogue's outstanding global stores.
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t"
+      ".reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
+      "}\n" ::"r"(bar), "r"(rank)
+      : "memory");
+}
+
 // Diagnostics for a wedged pipeline. `tag` identifies the wait site.
 __device__ unsigned int g_stb_wedge[8];
 
@@ -143,6 +169,14 @@ struct StageRing {
   __device__ __forceinline__ void release(int s) const {
     if (lane_id() == 0) mbar_arrive(empty_bar(s));
   }
+  // 2-CTA cluster whose producers each fill stage s in both CTAs: lane 0 of each warp hands s back to both producers
+  // (the empty barriers then count the consumer warps of both CTAs)
+  __device__ __forceinline__ void release_cluster(int s, uint32_t peer) const {
+    if (lane_id() == 0) {
+      mbar_arrive(empty_bar(s));
+      mbar_arrive_remote(empty_bar(s), peer);
+    }
+  }
 };
 
 // ----------------------------------------------------------------------------------------------
@@ -157,6 +191,16 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
       "%4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
+}
+// the box lands at offset `dst` of every cluster CTA in `cta_mask`, and completes bytes on the mbarrier at offset `bar`
+// of each of them
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
+                                               uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, "
+      "{%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0,
@@ -221,17 +265,18 @@ __device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
 // Shared-memory matrix descriptor for wgmma, SWIZZLE_128B layouts.
 //   [0,14) addr>>4  [16,30) LBO>>4  [32,46) SBO>>4  [62,64) layout (1 = SW128)
 // `tile_saddr` is the 1024-byte-aligned base of a SWIZZLE_128B operand tile and `byte_off` a multiple of 16 that
-// selects the K step / atom.
+// selects the K step / atom.  The address field holds bits [4, 18) of the address: in a cluster launch a CTA's shared
+// addresses carry its rank above bit 18, which must not carry into the LBO field.
 //   K-major tile: rows of 64 bf16 (128 B), 8-row groups 1024 B apart (SBO); K step kk -> +kk*32 B.
 __device__ __forceinline__ uint64_t sdesc_k(uint32_t tile_saddr, uint32_t byte_off) {
-  const uint32_t lo = (tile_saddr >> 4) + (byte_off >> 4) + (1u << 16);
+  const uint32_t lo = ((tile_saddr & 0x3ffffu) >> 4) + (byte_off >> 4) + (1u << 16);
   const uint32_t hi = (1024u >> 4) | (1u << 30);
   return (uint64_t(hi) << 32) | lo;
 }
 //   MN-major tile made of [K rows x 64 MN-elements] boxes `lbo` bytes apart; 8-k groups 1024 B apart;
 //   K step of 16 rows -> +2048 B.
 __device__ __forceinline__ uint64_t sdesc_mn(uint32_t tile_saddr, uint32_t byte_off, uint32_t lbo) {
-  const uint32_t lo = (tile_saddr >> 4) + ((byte_off >> 4) + ((lbo >> 4) << 16));
+  const uint32_t lo = ((tile_saddr & 0x3ffffu) >> 4) + ((byte_off >> 4) + ((lbo >> 4) << 16));
   const uint32_t hi = (1024u >> 4) | (1u << 30);
   return (uint64_t(hi) << 32) | lo;
 }

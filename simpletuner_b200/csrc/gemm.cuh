@@ -174,12 +174,21 @@ __device__ __forceinline__ void gemm_wgmma(float (&acc)[BN / 2], uint64_t a, uin
   else wgmma_ss_n64<0, TB>(acc, a, b, accumulate);
 }
 
-template <int BN, int EPI, bool CONV = false>
+// CLUSTER = 2: the CTAs run as 2-CTA clusters.  A cluster's work unit is a pair tile, m-tiles 2 pm and 2 pm + 1 at the
+// same n-tile; CTA rank r computes m-tile 2 pm + r.  The two tiles read the same W tile, so each producer loads rows
+// [64 r, 64 r + 64) of it and multicasts them into the same stage of both CTAs: 24 KB instead of 32 KB of L2 reads per
+// tile and k-block.  Both CTAs walk the same units, so their rings advance in lockstep, and a producer refills a stage
+// only when the consumers of both CTAs have released it (empty barriers of 8 warps, release_cluster).  With an odd
+// tiles_m the last pair's second tile lies past the end (its A box is zero-filled and its stores are skipped by the
+// row / batch guards); that CTA still loads, multicasts, waits on and releases every stage, or its peer would wedge.
+// W maps are then boxes of 64 rows (k-major) or the usual 64 x 64 boxes (w_kn).  CONV supports CLUSTER = 1 only.
+template <int BN, int EPI, bool CONV = false, int CLUSTER = 1>
 __global__ void __launch_bounds__(384, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int MI = Cfg::BM / 64;   // m64 row blocks of a tile
+  static_assert(CLUSTER == 1 || (CLUSTER == 2 && BN == 128 && !CONV), "2-CTA clusters: 128 x 128 GEMM tiles only");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -194,7 +203,12 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   const int tiles_per_batch = (p.rows_per_batch + Cfg::BM - 1) / Cfg::BM;
   const int tiles_m = tiles_per_batch * p.num_batches;
   const int tiles_n = (p.N + BN - 1) / BN;
-  const int num_tiles = tiles_m * tiles_n;
+  // work units: tiles, or pair tiles of a cluster; unit0 / units_stride: this CTA's (cluster's) first unit and stride
+  const int units_m = (tiles_m + CLUSTER - 1) / CLUSTER;
+  const int num_units = units_m * tiles_n;
+  const int unit0 = blockIdx.x / CLUSTER;
+  const int units_stride = gridDim.x / CLUSTER;
+  const uint32_t rank = CLUSTER == 2 ? cluster_ctarank() : 0u;
   int nk = 0;   // k-blocks per tile
   for (int s = 0; s < p.nseg; ++s) nk += p.kblocks[s];
 
@@ -203,20 +217,23 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       tma_prefetch_desc(&maps.a[s]);
       tma_prefetch_desc(&maps.w[s]);
     }
-    ring.init(4);   // each stage belongs to one consumer warpgroup's tile
+    ring.init(4 * CLUSTER);   // each stage belongs to one consumer warpgroup's tile (in every CTA of the cluster)
     mbar_init(order_bars, 4);
     mbar_init(order_bars + 8, 4);
     fence_mbar_init();
   }
-  __syncthreads();
+  // no multicast or remote arrive may reach a CTA before its barriers exist
+  if constexpr (CLUSTER == 2) cluster_sync();
+  else __syncthreads();
 
   if (wg == 0) {
     // ===================== TMA producer (warp 0, one elected lane issues) =====================
     reg_dealloc<40>();
     if (warp == 0) {
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for (int unit = unit0; unit < num_units; unit += units_stride) {
         int tm, tn;
-        gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
+        gemm_tile_coords(unit, units_m, tiles_n, tm, tn);
+        tm = tm * CLUSTER + (int)rank;
         const int b = tm / tiles_per_batch;
         const int s0 = (tm - b * tiles_per_batch) * Cfg::BM;
         const int n0 = tn * BN;
@@ -238,7 +255,13 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
               } else {
                 tma_load_3d(sa, &maps.a[seg], full, kb * 64, s0, b);
               }
-              if (p.w_kn[seg]) {
+              if constexpr (CLUSTER == 2) {
+                // this CTA's half of the W tile, into both CTAs: n-columns [64 r, 64 r + 64), k-major or MN-major
+                const int hn = n0 + 64 * (int)rank;
+                const uint32_t hw = sa + Cfg::A_BYTES + rank * 8192u;
+                if (p.w_kn[seg]) tma_load_2d_mc(hw, &maps.w[seg], full, hn, kb * 64, 0x3);
+                else tma_load_2d_mc(hw, &maps.w[seg], full, kb * 64, hn, 0x3);
+              } else if (p.w_kn[seg]) {
 #pragma unroll
                 for (int g = 0; g < BN / 64; ++g)
                   tma_load_2d(sa + Cfg::A_BYTES + g * 8192, &maps.w[seg], full, n0 + g * 64, kb * 64);
@@ -262,15 +285,16 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     uint32_t order_phase = 0;
     if (cw == 1) ring.skip(nk);
     float acc[MI][BN / 2];
-    for (int tile = blockIdx.x + cw * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
+    for (int unit = unit0 + cw * units_stride; unit < num_units; unit += 2 * units_stride) {
       // The other consumer has waited on every stage of the tile before this one, so the producer has filled them all
       // and this consumer's full-barrier waits are at most one lap ahead of the barriers' phases.
-      if (tile != (int)blockIdx.x) {
+      if (unit != unit0) {
         mbar_wait(order_bars + 8u * cw, order_phase, 4);
         order_phase ^= 1u;
       }
       int tm, tn;
-      gemm_tile_coords(tile, tiles_m, tiles_n, tm, tn);
+      gemm_tile_coords(unit, units_m, tiles_n, tm, tn);
+      tm = tm * CLUSTER + (int)rank;
       const int b = tm / tiles_per_batch;
       const int s0 = (tm - b * tiles_per_batch) * Cfg::BM;
       const int n0 = tn * BN;
@@ -291,6 +315,10 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
               for (int mi = 0; mi < MI; ++mi)
                 gemm_wgmma<BN, 1>(acc[mi], sdesc_k(sa + mi * 8192, kk * 32), sdesc_mn(sw, kk * 2048, 8192),
                                   kk > 0 ? 1u : accumulate);
+            // commit and wait in each branch: a wgmma group still open where the branches join makes ptxas close it
+            // with an extra HGMMA, and the wait below then drains the k-block just issued as well
+            wg_commit();
+            wg_wait<1>();   // keep one k-block in flight; the one before it has retired -> free its slot
           } else {
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
@@ -298,25 +326,26 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
               for (int mi = 0; mi < MI; ++mi)
                 gemm_wgmma<BN, 0>(acc[mi], sdesc_k(sa + mi * 8192, kk * 32), sdesc_k(sw, kk * 32),
                                   kk > 0 ? 1u : accumulate);
+            wg_commit();
+            wg_wait<1>();
           }
           accumulate = 1;
-          wg_commit();
-          // keep one k-block in flight; the one before it has retired -> free its slot
-          wg_wait<1>();
-#pragma unroll
-          for (int mi = 0; mi < MI; ++mi) wg_fence_regs(acc[mi]);
-          if (prev_stage >= 0) ring.release(prev_stage);
+          if (prev_stage >= 0) {
+            if constexpr (CLUSTER == 2) ring.release_cluster(prev_stage, rank ^ 1u);
+            else ring.release(prev_stage);
+          }
           prev_stage = ring.stage;
           ring.advance();
         }
       }
       // every stage of this tile has landed: the other consumer may start on the next tile
-      if (tile + (int)gridDim.x < num_tiles && lane == 0) mbar_arrive(order_bars + 8u * (cw ^ 1));
+      if (unit + units_stride < num_units && lane == 0) mbar_arrive(order_bars + 8u * (cw ^ 1));
       ring.skip(nk);
       wg_wait<0>();
 #pragma unroll
       for (int mi = 0; mi < MI; ++mi) wg_fence_regs(acc[mi]);
-      ring.release(prev_stage);
+      if constexpr (CLUSTER == 2) ring.release_cluster(prev_stage, rank ^ 1u);
+      else ring.release(prev_stage);
 
       // ===================== epilogue from registers =====================
       // accumulator layout (m64nBN): acc[mi][4 i + 2 h + j] = row 64 mi + 16 wq + lane / 4 + 8 h,
@@ -361,6 +390,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       }
     }
   }
+  // the peer may still multicast into this CTA's stages or arrive on its empty barriers until it is done too
+  if constexpr (CLUSTER == 2) cluster_sync();
 }
 
 }  // namespace stb

@@ -84,6 +84,9 @@ def gemm(
     a_list[i]: [B, S, K_i] or [M, K_i];  w_list[i]: [N, K_i] (nn.Linear layout, row stride free) — or, where w_kn[i] is
     set, [K_i, N] (the contraction index is the row: `a @ w`, e.g. the dgrad of a Linear on its forward weight).
     gate: [B, N];  res / aux / out: same leading shape as a_list[0] with last dim N.
+    tile = (mt, bn): bn 64, 128 or 256 forces the tile width (0 = automatic); mt 2 runs 128 x 128 tiles as 2-CTA
+    clusters that share the W tile (the other widths run single CTAs), 1 single CTAs, 0 chooses (clusters for the
+    GELU / dGELU epilogues with at least 16 m-tiles).  Both give the same bits.
     """
     nseg = len(a_list)
     assert 1 <= nseg <= 3 and len(w_list) == nseg
