@@ -96,12 +96,17 @@ typedef struct {
   void* o;
   long long o_b, o_s, o_h;
   float* lse;
-  /* optional additive logit bias shared by the batch (forward / inference only; text encoders: T5 relative position bias
-   * T5Attention.compute_bias, CLIP causal mask — transformers classes called at flux/pipeline.py:1085, 1127):
-   * logit = scale * q.k + bias[h * bias_h + sq * bias_q + sk], bf16, -inf = masked; NULL = none.  Every query row must
-   * keep at least one finite logit among its first 128 keys. */
+  /* optional additive logit bias: logit = scale * q.k + bias[b * bias_b + h * bias_h + sq * bias_q + sk], bf16,
+   * -inf = masked; NULL = none.  A zero stride shares the bias along that dimension.  Two forms:
+   *  - bias_q >= Sk: a [B or 1, H or 1, Sq, Sk] bias (text encoders: T5 relative position bias T5Attention.compute_bias,
+   *    CLIP causal mask — transformers classes called at flux/pipeline.py:1085, 1127);
+   *  - bias_q = bias_h = 0: one row per sample over the keys, [B or 1, Sk] (Flux masked training: the float mask
+   *    `(expand_flux_attention_mask(...) > 0).to(dtype)` that FluxAttnProcessor2_0 adds to the logits, reference
+   *    flux/transformer.py:170-173, 200-207, 227-242).
+   * Every query row must keep at least one finite logit. */
   const void* bias;
   long long bias_h, bias_q;
+  long long bias_b;
 } stb_attn_fwd_args;
 int stb_attn_fwd(const stb_attn_fwd_args* args, void* stream);
 
@@ -131,6 +136,11 @@ typedef struct {
   void *dq, *dk, *dv;
   long long dq_b, dq_s, dq_h, dk_b, dk_s, dk_h, dv_b, dv_s, dv_h;
   const stb_qk_prep* qk_prep; /* NULL: dq / dk are the gradients of the q / k inputs */
+  /* the forward's per-key bias (bias_q = bias_h = 0 form of stb_attn_fwd_args; reference flux/transformer.py:170-173,
+   * 200-207): bf16 bias[b * bias_b + sk], bias_b = 0 shares one row across the batch; NULL = none.  Any other form
+   * returns STB_ERR_UNSUPPORTED.  Keys whose bias is -inf get dk = dv = 0. */
+  const void* bias;
+  long long bias_b;
 } stb_attn_bwd_args;
 int stb_attn_bwd(const stb_attn_bwd_args* args, void* stream);
 

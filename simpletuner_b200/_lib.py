@@ -86,6 +86,7 @@ class AttnFwdArgs(C.Structure):
         ("o_b", C.c_longlong), ("o_s", C.c_longlong), ("o_h", C.c_longlong),
         ("lse", C.c_void_p),
         ("bias", C.c_void_p), ("bias_h", C.c_longlong), ("bias_q", C.c_longlong),
+        ("bias_b", C.c_longlong),
     ]
 
 
@@ -113,6 +114,7 @@ class AttnBwdArgs(C.Structure):
         ("dk_b", C.c_longlong), ("dk_s", C.c_longlong), ("dk_h", C.c_longlong),
         ("dv_b", C.c_longlong), ("dv_s", C.c_longlong), ("dv_h", C.c_longlong),
         ("qk_prep", C.POINTER(QkPrep)),
+        ("bias", C.c_void_p), ("bias_b", C.c_longlong),
     ]
 
 

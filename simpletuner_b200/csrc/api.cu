@@ -296,16 +296,17 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 
 
 }  // namespace
 
-template <int HD, bool BIAS>
+template <int HD, bool BIAS, bool KEY = false>
 static int launch_attn_fwd(const stb::AttnFwdMaps& maps, const stb::AttnFwdParams& p, dim3 grid, cudaStream_t st) {
-  constexpr int SMEM = stb::AttnFwdCfg<HD>::SMEM_BYTES;
-  if (int r = set_smem<stb::attn_fwd_kernel<HD, BIAS>>(SMEM)) return r;
-  stb::attn_fwd_kernel<HD, BIAS><<<grid, 384, SMEM, st>>>(maps, p);
-  STB_LAUNCH_CHECK(BIAS ? "attn_fwd_bias" : "attn_fwd");
+  using Cfg = stb::AttnFwdCfg<HD>;
+  constexpr int SMEM = Cfg::SMEM_BYTES + (KEY ? Cfg::KV_STAGES * 128 * 4 : 0);
+  if (int r = set_smem<stb::attn_fwd_kernel<HD, BIAS, KEY>>(SMEM)) return r;
+  stb::attn_fwd_kernel<HD, BIAS, KEY><<<grid, 384, SMEM, st>>>(maps, p);
+  STB_LAUNCH_CHECK(KEY ? "attn_fwd_key_bias" : (BIAS ? "attn_fwd_bias" : "attn_fwd"));
   return 0;
 }
 
-template <int HD>
+template <int HD, bool BIAS>
 static int launch_attn_bwd(const stb_attn_bwd_args* a, const stb::AttnBwdMaps& maps, const stb::AttnBwdParams& p,
                            cudaStream_t st) {
   {
@@ -315,13 +316,14 @@ static int launch_attn_bwd(const stb_attn_bwd_args* a, const stb::AttnBwdMaps& m
         static_cast<const __nv_bfloat16*>(a->d_o), a->do_b, a->do_s, a->do_h, a->delta, a->B, a->H, a->Sq);
     STB_LAUNCH_CHECK("attn_bwd_delta");
   }
-  constexpr int SMEM1 = stb::AttnBwdCfg<HD>::DKDV_SMEM_BYTES, SMEM2 = stb::AttnBwdCfg<HD>::DQ_SMEM_BYTES;
-  if (int r = set_smem<stb::attn_bwd_dkdv_kernel<HD>>(SMEM1)) return r;
-  if (int r = set_smem<stb::attn_bwd_dq_kernel<HD>>(SMEM2)) return r;
-  stb::attn_bwd_dkdv_kernel<HD><<<dim3((a->Sk + 63) / 64, a->H, a->B), 384, SMEM1, st>>>(maps, p);
-  STB_LAUNCH_CHECK("attn_bwd_dkdv");
-  stb::attn_bwd_dq_kernel<HD><<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM2, st>>>(maps, p);
-  STB_LAUNCH_CHECK("attn_bwd_dq");
+  using Cfg = stb::AttnBwdCfg<HD>;
+  constexpr int SMEM1 = Cfg::DKDV_SMEM_BYTES, SMEM2 = Cfg::DQ_SMEM_BYTES + (BIAS ? Cfg::STAGES * Cfg::KB : 0);
+  if (int r = set_smem<stb::attn_bwd_dkdv_kernel<HD, BIAS>>(SMEM1)) return r;
+  if (int r = set_smem<stb::attn_bwd_dq_kernel<HD, BIAS>>(SMEM2)) return r;
+  stb::attn_bwd_dkdv_kernel<HD, BIAS><<<dim3((a->Sk + 63) / 64, a->H, a->B), 384, SMEM1, st>>>(maps, p);
+  STB_LAUNCH_CHECK(BIAS ? "attn_bwd_dkdv_bias" : "attn_bwd_dkdv");
+  stb::attn_bwd_dq_kernel<HD, BIAS><<<dim3((a->Sq + 127) / 128, a->H, a->B), 384, SMEM2, st>>>(maps, p);
+  STB_LAUNCH_CHECK(BIAS ? "attn_bwd_dq_bias" : "attn_bwd_dq");
   return 0;
 }
 
@@ -405,11 +407,16 @@ int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
   p.o_b = a->o_b; p.o_s = a->o_s; p.o_h = a->o_h;
   p.lse = a->lse;
   p.bias = static_cast<const __nv_bfloat16*>(a->bias);
-  p.bias_h = a->bias_h; p.bias_q = a->bias_q;
+  p.bias_b = a->bias_b; p.bias_h = a->bias_h; p.bias_q = a->bias_q;
   p.inv_scale = a->scale != 0.f ? 1.f / a->scale : 0.f;
   const dim3 grid((a->Sq + 127) / 128, a->H, a->B);
-  if (a->bias) {   // text-encoder instantiation (additive bias / mask); never taken by the training step
-    if (a->scale == 0.f || a->bias_q < a->Sk) return fail(STB_ERR_ARG, "attn_fwd bias: scale must be non-zero and bias_q >= Sk");
+  if (a->bias) {   // additive bias / mask: text encoders, and the per-key bias of Flux masked training
+    const bool key_row = a->bias_q == 0 && a->bias_h == 0;
+    if (a->scale == 0.f || a->bias_b < 0 || a->bias_h < 0 || (a->bias_q < a->Sk && !key_row))
+      return fail(STB_ERR_ARG, "attn_fwd bias: scale must be non-zero, strides non-negative, and bias_q >= Sk "
+                               "(or bias_q = bias_h = 0 for a per-key row)");
+    if (key_row)   // one row per sample: staged per key tile in shared memory
+      return a->HD == 128 ? launch_attn_fwd<128, true, true>(maps, p, grid, st) : launch_attn_fwd<64, true, true>(maps, p, grid, st);
     return a->HD == 128 ? launch_attn_fwd<128, true>(maps, p, grid, st) : launch_attn_fwd<64, true>(maps, p, grid, st);
   }
   return a->HD == 128 ? launch_attn_fwd<128, false>(maps, p, grid, st) : launch_attn_fwd<64, false>(maps, p, grid, st);
@@ -467,8 +474,14 @@ int stb_attn_bwd(const stb_attn_bwd_args* a, void* stream) {
   p.d_o = static_cast<const __nv_bfloat16*>(a->d_o);
   p.q_b = a->q_b; p.q_s = a->q_s; p.q_h = a->q_h;
   p.do_b = a->do_b; p.do_s = a->do_s; p.do_h = a->do_h;
-  if (a->HD == 128) return launch_attn_bwd<128>(a, maps, p, st);
-  return launch_attn_bwd<64>(a, maps, p, st);
+  p.bias = static_cast<const __nv_bfloat16*>(a->bias);
+  p.bias_b = a->bias_b;
+  if (a->bias) {   // per-key only: [B, Sk] rows bias_b apart, or one row shared by the batch (bias_b = 0)
+    if (a->bias_b < 0 || (a->bias_b != 0 && a->bias_b < a->Sk))
+      return fail(STB_ERR_UNSUPPORTED, "attn_bwd bias: only a per-key bias [B or 1, Sk] (bias_b = 0 or >= Sk) is supported");
+    return a->HD == 128 ? launch_attn_bwd<128, true>(a, maps, p, st) : launch_attn_bwd<64, true>(a, maps, p, st);
+  }
+  return a->HD == 128 ? launch_attn_bwd<128, false>(a, maps, p, st) : launch_attn_bwd<64, false>(a, maps, p, st);
 }
 
 int stb_ln_modulate_fwd(const void* x, long long x_b, long long x_s, const void* shift, const void* scale,

@@ -42,6 +42,9 @@ struct AttnBwdParams {
   int s_split;
   const float *cosT, *sinT;          // [S, HD] or null
   float eps;
+  // BIAS instantiations only: the forward's per-key logit bias, bias[b * bias_b + sk] (bf16, -inf = masked key)
+  const __nv_bfloat16* bias;
+  long long bias_b;
 };
 
 struct AttnBwdMaps {
@@ -84,6 +87,7 @@ struct AttnBwdCfg {
   static constexpr int PT = 64 * 64 * 4;     // one fp32 P^T tile handed between the dK / dV warpgroups
   static constexpr int DKDV_SMEM_BYTES = 2 * SMALL + STAGES * (2 * SMALL + STAT) + 2 * PT + 1024 + 256;
   static constexpr int DQ_SMEM_BYTES = 2 * BIG + STAGES * 2 * SMALL + 1024 + 256;
+  static constexpr int KB = 64 * 4;          // per stage (dQ kernel, BIAS): 64 keys x bias * log2(e)
 };
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
@@ -206,7 +210,9 @@ __device__ __forceinline__ void mma_kmajor_n64(float (&d)[32], uint32_t a_tile, 
 //   warpgroup 2: dP^T = V dO^T;  dS^T = P^T o (dP^T - Delta) -> dK += dS^T Q
 // The P^T hand-over is double-buffered (named barriers PT_FULL / PT_EMPTY + buffer), so warpgroup 1 runs up to one
 // query tile ahead and the two warpgroups' MMAs interleave on the tensor pipe.
-template <int HD>
+// BIAS: each thread's two key rows carry a constant bias * log2(e) in the exponent of P^T; a -inf key gets P^T = 0 and
+// with it dS^T = 0, so its dK and dV are exactly 0.
+template <int HD, bool BIAS = false>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams p) {
   using Cfg = AttnBwdCfg<HD>;
@@ -287,6 +293,14 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
     // stat4[4 i + lane % 4] = {LSE * log2(e), Delta} of query columns 8 i + 2 (lane % 4) + {0, 1}
     if (cw == 0) {
       const float sl2 = p.scale * 1.4426950408889634f;
+      float kb[2] = {0.f, 0.f};   // bias * log2(e) of key rows 16 wq + lane / 4 + 8 hh
+      if constexpr (BIAS) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int kv = kv0 + 16 * (t >> 5) + (lane >> 2) + 8 * hh;
+          kb[hh] = kv < p.Sk ? __bfloat162float(p.bias[(long long)b * p.bias_b + kv]) * 1.4426950408889634f : 0.f;
+        }
+      }
       for (int j = 0; j < n_q; ++j) {
         const int stg = j % Cfg::STAGES, buf = j & 1;
         mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 42);
@@ -307,8 +321,13 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
           const float4 sv = stat4[4 * i + (lane & 3)];
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
-            s[4 * i + 2 * hh] = ex2f(fmaf(s[4 * i + 2 * hh], sl2, -sv.x));   // P^T
-            s[4 * i + 2 * hh + 1] = ex2f(fmaf(s[4 * i + 2 * hh + 1], sl2, -sv.z));
+            if constexpr (BIAS) {
+              s[4 * i + 2 * hh] = ex2f(fmaf(s[4 * i + 2 * hh], sl2, kb[hh] - sv.x));   // P^T
+              s[4 * i + 2 * hh + 1] = ex2f(fmaf(s[4 * i + 2 * hh + 1], sl2, kb[hh] - sv.z));
+            } else {
+              s[4 * i + 2 * hh] = ex2f(fmaf(s[4 * i + 2 * hh], sl2, -sv.x));   // P^T
+              s[4 * i + 2 * hh + 1] = ex2f(fmaf(s[4 * i + 2 * hh + 1], sl2, -sv.z));
+            }
           }
         }
         if (j >= 2) named_bar_sync(PT_EMPTY + buf, 256);   // warpgroup 2 has read P^T of tile j - 2
@@ -397,7 +416,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
 // ------------------------------------------------------------------------------------------------
 // dQ
 // ------------------------------------------------------------------------------------------------
-template <int HD>
+// BIAS: the producer stages each key tile's 64 values of bias * log2(e) next to its K / V (s_full then also counts the
+// producer warp's arrive); the consumers fold them into the exponent of P.
+template <int HD, bool BIAS = false>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams p) {
   using Cfg = AttnBwdCfg<HD>;
@@ -408,7 +429,9 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
   const uint32_t q_smem = smem_base, do_smem = smem_base + Cfg::BIG;
   const uint32_t k_smem = smem_base + 2 * Cfg::BIG;                      // STAGES streamed K tiles
   const uint32_t v_smem = k_smem + Cfg::STAGES * Cfg::SMALL;             // STAGES streamed V tiles
-  const uint32_t bar_base = v_smem + Cfg::STAGES * Cfg::SMALL;
+  const uint32_t kb_smem = v_smem + Cfg::STAGES * Cfg::SMALL;            // BIAS: STAGES x 64 fp32 key biases
+  const uint32_t bar_base = kb_smem + (BIAS ? Cfg::STAGES * Cfg::KB : 0);
+  float* kb_rows = reinterpret_cast<float*>(smem_raw + (kb_smem - smem_u32(smem_raw)));
   const uint32_t qd_full = bar_base;
   auto s_full = [&](int s) { return bar_base + 8u * (1 + s); };
   auto s_empty = [&](int s) { return bar_base + 8u * (1 + Cfg::STAGES + s); };
@@ -421,7 +444,7 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
   if (threadIdx.x == 0) {
     mbar_init(qd_full, 1);
     for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(s_full(s), 1);
+      mbar_init(s_full(s), BIAS ? 2 : 1);
       mbar_init(s_empty(s), 8);
     }
     fence_mbar_init();
@@ -450,6 +473,16 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
           }
         }
         __syncwarp();
+        if constexpr (BIAS) {   // keys past Sk: any finite value (their P is forced to 0)
+#pragma unroll
+          for (int r = lane; r < 64; r += 32) {
+            const int kv = j * 64 + r;
+            kb_rows[stg * 64 + r] =
+                kv < p.Sk ? __bfloat162float(p.bias[(long long)b * p.bias_b + kv]) * 1.4426950408889634f : 0.f;
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(s_full(stg));
+        }
       }
     }
   } else {
@@ -489,16 +522,20 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
       wg_wait<1>();   // S
       wg_fence_regs(sc);
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
+      for (int i = 0; i < 8; ++i) {
+        float2 kb2 = make_float2(0.f, 0.f);
+        if constexpr (BIAS) kb2 = reinterpret_cast<const float2*>(kb_rows + stg * 64)[4 * i + (lane & 3)];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const bool ok = j * 64 + 8 * i + 2 * (lane & 3) + e < p.Sk;
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const int x = 4 * i + 2 * hh + e;
-            sc[x] = ok ? ex2f(fmaf(sc[x], sl2, -l2[hh])) : 0.f;   // P
+            if constexpr (BIAS) sc[x] = ok ? ex2f(fmaf(sc[x], sl2, (e ? kb2.y : kb2.x) - l2[hh])) : 0.f;   // P
+            else sc[x] = ok ? ex2f(fmaf(sc[x], sl2, -l2[hh])) : 0.f;
           }
         }
+      }
       wg_wait<0>();   // dP
       wg_fence_regs(dp);
 #pragma unroll

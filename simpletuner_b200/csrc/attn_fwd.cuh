@@ -20,11 +20,14 @@ struct AttnFwdParams {
   __nv_bfloat16* O;   // [B, Sq, H, HD] via strides
   long long o_b, o_s, o_h;
   float* lse;         // [B, H, Sq] natural-log LSE of the scaled scores
-  // BIAS instantiation only: additive logit bias (T5 relative position bias, CLIP causal mask), shared by the batch:
-  // logit = scale * q.k + bias[h * bias_h + sq * bias_q + sk]   (bf16; -inf masks; bias_h = 0 shares it between heads)
+  // BIAS instantiation only: additive logit bias (T5 relative position bias, CLIP causal mask, the Flux per-sample key
+  // bias of masked training):
+  // logit = scale * q.k + bias[b * bias_b + h * bias_h + sq * bias_q + sk]   (bf16; -inf masks; a zero stride shares the
+  // bias along that dimension: bias_b = 0 across the batch, bias_h = bias_q = 0 gives one row per sample over the keys)
   const __nv_bfloat16* bias;
   long long bias_h, bias_q;
   float inv_scale;
+  long long bias_b;
 };
 
 struct AttnFwdMaps {
@@ -55,10 +58,12 @@ __device__ __forceinline__ void wgmma_rs_mn(float (&d)[N / 2], const uint32_t (&
   else wgmma_rs_n64<1>(d, a, b, accumulate);
 }
 
-// BIAS = true (text encoders only): the bias tile is added to the raw scores (pre-divided by the softmax scale).  Every
-// query row needs at least one finite logit in its FIRST key tile (true for a causal mask and for un-masked
-// relative-position biases).
-template <int HD, bool BIAS = false>
+// BIAS = true: the bias tile is added to the raw scores (pre-divided by the softmax scale).  Every query row needs at least
+// one finite logit somewhere; a 128-key tile in which a row is all -inf (at any position) contributes nothing.
+// KEY = true (with BIAS; bias_h = bias_q = 0): one bias row per sample.  The producer warp stages each key tile's 128
+// values in shared memory (ring b_full / b_empty next to K / V) and the consumers read them as float2: per-element global
+// loads of the general form made the forward 1.7x slower at the Flux shape (DESIGN.md 1).
+template <int HD, bool BIAS = false, bool KEY = false>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p) {
   using Cfg = AttnFwdCfg<HD>;
@@ -78,6 +83,9 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
   auto k_empty = [&](int s) { return bar_base + 8u * (1 + NSTG + s); };
   auto v_full = [&](int s) { return bar_base + 8u * (1 + 2 * NSTG + s); };
   auto v_empty = [&](int s) { return bar_base + 8u * (1 + 3 * NSTG + s); };
+  auto b_full = [&](int s) { return bar_base + 8u * (1 + 4 * NSTG + s); };    // KEY only
+  auto b_empty = [&](int s) { return bar_base + 8u * (1 + 5 * NSTG + s); };
+  float* kb_rows = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - smem_u32(smem_raw)));   // KEY: NSTG x 128 fp32
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -97,6 +105,10 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
       mbar_init(k_empty(s), 8);
       mbar_init(v_full(s), 1);
       mbar_init(v_empty(s), 8);
+      if constexpr (KEY) {
+        mbar_init(b_full(s), 1);
+        mbar_init(b_empty(s), 8);
+      }
     }
     fence_mbar_init();
   }
@@ -128,6 +140,14 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
             tma_load_4d(v_smem + stg * TILE + a * ATOM_BYTES, &maps.v, v_full(stg), a * 64, h, j * 128, b);
         }
         __syncwarp();
+        if constexpr (KEY) {   // after the V issue: the bias is needed only once S is done
+          mbar_wait(b_empty(stg), par, 12);
+          const __nv_bfloat16* brow = p.bias + (long long)b * p.bias_b + (long long)j * 128;
+#pragma unroll
+          for (int r = lane; r < 128; r += 32) kb_rows[stg * 128 + r] = j * 128 + r < p.Sk ? __bfloat162float(brow[r]) : 0.f;
+          __syncwarp();
+          if (lane == 0) mbar_arrive(b_full(stg));
+        }
       }
     }
   } else {
@@ -144,10 +164,11 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
     float m_row[2] = {-INFINITY, -INFINITY};   // raw-score row max
     float l_row[2] = {0.f, 0.f};               // this thread's share of the row sum
     const __nv_bfloat16* brow[2] = {nullptr, nullptr};
-    if constexpr (BIAS) {
+    if constexpr (BIAS && !KEY) {
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh)
-        brow[hh] = p.bias + (long long)h * p.bias_h + (long long)min(r_lo + 8 * hh, p.Sq - 1) * p.bias_q;
+        brow[hh] = p.bias + (long long)b * p.bias_b + (long long)h * p.bias_h +
+                   (long long)min(r_lo + 8 * hh, p.Sq - 1) * p.bias_q;
     }
     const uint32_t qa = q_smem + cw * 8192;
     mbar_wait(q_full, 0, 20);
@@ -172,21 +193,30 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
 
       // ---- online softmax (s_acc[4 i + 2 hh + e] = row r_lo + 8 hh, key 8 i + 2 (lane % 4) + e)
       const int kv_valid = p.Sk - j * 128;
+      if constexpr (KEY) mbar_wait(b_full(stg), par, 23);
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
+        float2 kb2 = make_float2(0.f, 0.f);
+        if constexpr (KEY) kb2 = reinterpret_cast<const float2*>(kb_rows + stg * 128)[4 * i + (lane & 3)];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int c = 8 * i + 2 * (lane & 3) + e;
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             float v = s_acc[4 * i + 2 * hh + e];
-            if constexpr (BIAS) {
+            if constexpr (KEY) {
+              if (c < kv_valid) v = fmaf(e ? kb2.y : kb2.x, p.inv_scale, v);
+            } else if constexpr (BIAS) {
               if (c < kv_valid) v = fmaf(__bfloat162float(brow[hh][j * 128 + c]), p.inv_scale, v);
             }
             if (c >= kv_valid) v = -INFINITY;
             s_acc[4 * i + 2 * hh + e] = v;
           }
         }
+      }
+      if constexpr (KEY) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(b_empty(stg));
       }
       float alpha[2], nmb[2];
 #pragma unroll
@@ -197,9 +227,12 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
         m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
         m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
         const float m_new = fmaxf(m_row[hh], m);
-        alpha[hh] = ex2f((m_row[hh] - m_new) * sl2);   // 0 on the first tile
+        // A row that is -inf in every key so far (a bias can do that) exponentiates against 0 instead of -inf: its
+        // exponentials and alpha are then 0, not NaN.  Without a bias every tile has a finite key.
+        const float m_exp = (BIAS && m_new == -INFINITY) ? 0.f : m_new;
+        alpha[hh] = ex2f((m_row[hh] - m_exp) * sl2);   // 0 on the first tile
         m_row[hh] = m_new;
-        nmb[hh] = -m_new * sl2;
+        nmb[hh] = -m_exp * sl2;
         l_row[hh] *= alpha[hh];
       }
 #pragma unroll

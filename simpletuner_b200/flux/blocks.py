@@ -339,9 +339,9 @@ def _qk_fwd(qkv, D, H, hd, img_plan: AttnPlan, txt_plan: Optional[AttnPlan], S_t
     return ops.qk_rmsnorm_rope_fwd(qkv, D, H, hd, img_plan.norm_q, img_plan.norm_k, tq, tk, S_txt, cos, sin, EPS)
 
 
-def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, sin, qk=None):
+def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, sin, qk=None, key_bias=None):
     """Returns d_qkv [B, S, 3D] given d_o.  `qk` = the (q, k) pair saved by the forward (spending 2 B S D bytes per block
-    is cheaper than re-running the RMSNorm + RoPE pass in backward); recomputed when absent."""
+    is cheaper than re-running the RMSNorm + RoPE pass in backward); recomputed when absent.  key_bias: the forward's."""
     B, S, _ = qkv.shape
     q, k = qk if qk is not None else _qk_fwd(qkv, D, H, hd, img_plan, txt_plan, S_txt, cos, sin)
     v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
@@ -349,14 +349,15 @@ def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, s
     dv = d_qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
     if img_plan.norm_q is None and cos is None:
         ops.attn_bwd(q, k, v, o.view(B, S, H, hd), d_o.view(B, S, H, hd), lse,
-                     dq=d_qkv[:, :, 0:D].unflatten(-1, (H, hd)), dk=d_qkv[:, :, D:2 * D].unflatten(-1, (H, hd)), dv=dv)
+                     dq=d_qkv[:, :, 0:D].unflatten(-1, (H, hd)), dk=d_qkv[:, :, D:2 * D].unflatten(-1, (H, hd)), dv=dv,
+                     key_bias=key_bias)
         return d_qkv
     # The backward of RMSNorm + RoPE stays a separate HBM-bound pass.  libstb200 can also run it inside the
     # attention-backward epilogues (ops.attn_bwd(qk_prep=...), tests: attn_bwd_fused_prep*); the step keeps the separate
     # pass because the longer epilogue of the fused form is not overlapped by anything (not measured on H100).
     dq = torch.empty_like(q)
     dk = torch.empty_like(k)
-    ops.attn_bwd(q, k, v, o.view(B, S, H, hd), d_o.view(B, S, H, hd), lse, dq=dq, dk=dk, dv=dv)
+    ops.attn_bwd(q, k, v, o.view(B, S, H, hd), d_o.view(B, S, H, hd), lse, dq=dq, dk=dk, dv=dv, key_bias=key_bias)
     del q, k
     tq = txt_plan.norm_q if txt_plan is not None else None
     tk = txt_plan.norm_k if txt_plan is not None else None
@@ -433,7 +434,7 @@ class DoubleBlockFn(torch.autograd.Function):
         ta: AttnPlan = plans["txt_attn"]
         q, k = _qk_fwd(qkv, D, H, hd, ia, ta, S_txt, cos, sin)
         v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
-        o, lse = ops.attn_fwd(q, k, v)
+        o, lse = ops.attn_fwd(q, k, v, key_bias=st.get("key_bias"))
         keep_qk = SAVE_QK and q.data_ptr() != qkv.data_ptr()      # (views of qkv when the model has neither norm nor RoPE)
         if not keep_qk:
             del q, k
@@ -580,7 +581,8 @@ class DoubleBlockFn(torch.autograd.Function):
                 del nh2a
             del d_qkv2
         # ---- joint attention core
-        d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, plans["img_attn"], plans["txt_attn"], S_txt, cos, sin, qk=qk_saved)
+        d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, plans["img_attn"], plans["txt_attn"], S_txt, cos, sin, qk=qk_saved,
+                               key_bias=st.get("key_bias"))
         del qk_saved, q_saved, k_saved
         dh = torch.empty_like(h)
         for name, sl, mod, base, pre, t_qkv, t_out in streams:
@@ -643,7 +645,7 @@ class SingleBlockFn(torch.autograd.Function):
         qkv, t_qkv = _linear_lora_fwd(nh, ap.w_qkv, ap.b_qkv, pk, drop)
         q, k = ops.qk_rmsnorm_rope_fwd(qkv, D, H, hd, ap.norm_q, ap.norm_k, None, None, 0, cos, sin, EPS)
         v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
-        o, lse = ops.attn_fwd(q, k, v)
+        o, lse = ops.attn_fwd(q, k, v, key_bias=st.get("key_bias"))
         if not SAVE_QK:
             del q, k
         o = o.view(B, S, D)
@@ -708,7 +710,7 @@ class SingleBlockFn(torch.autograd.Function):
                 (grads[8], grads[9]), = _lora_grads(pk_out, torch.cat([o, act], 2), t_out, g, t_up, dr(4))
             del act, t_up
         del g
-        d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, ap, None, 0, cos, sin, qk=qk_saved)
+        d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, ap, None, 0, cos, sin, qk=qk_saved, key_bias=st.get("key_bias"))
         del d_o, qk_saved, q_saved, k_saved
         # d_nh = d_pre W_mlp + d_qkv W_qkv (+ LoRA branches as one more K-segment)
         t_ups, a_ts = [], []

@@ -57,6 +57,8 @@ class Flux:
                                                                        base_image_seq_len=256, max_image_seq_len=4096,
                                                                        base_shift=0.5, max_shift=1.15))
         self.model = transformer if transformer is not None else FluxTransformer2DModel(**transformer_kwargs)
+        # set_attn_processor refuses the flash processors (key-padding semantics) while the additive mask is in use
+        self._denoiser().attention_masked_training = bool(getattr(self.config, "flux_attention_masked_training", False))
 
     # ------------------------------------------------------------------------------------------
     def get_trained_component(self):
@@ -124,8 +126,7 @@ class Flux:
         if tgt not in FLUX_LORA_TARGETS:       # "ai-toolkit" (adaLN linears) / "controlnet" stay on the reference module
             raise NotImplementedError(f"flux_lora_target={tgt!r} is not supported by the libstb200 path "
                                       f"(supported: {sorted(FLUX_LORA_TARGETS)})")
-        if g("flux_attention_masked_training", False):
-            raise NotImplementedError("flux_attention_masked_training is not supported by the libstb200 Flux path (quirk Q2)")
+        check_masked_training(c)
         if g("tread_config", None):
             raise NotImplementedError("TREAD routing is not supported by the libstb200 path")
         if g("flow_cubic_schedule", None) or g("flow_cubic_schedule_weights", None):
@@ -143,10 +144,12 @@ class Flux:
 
     def _check_supported(self, batch: Dict[str, Any]) -> None:
         """Options of the reference wrapper this path does not implement must RAISE, never be ignored, so that a shim can
-        route such a config to the reference class (INTEGRATION.md 2): masked training (flux/model.py:813 passes
-        `encoder_attention_mask`), Kontext conditioning latents (flux/model.py:757-786)."""
-        if getattr(self.config, "flux_attention_masked_training", False):
-            raise NotImplementedError("flux_attention_masked_training is not supported by the libstb200 Flux path (quirk Q2)")
+        route such a config to the reference class (INTEGRATION.md 2): masked training outside `check_masked_training`'s
+        rule or without the batch's `encoder_attention_mask` (flux/model.py:813-822), Kontext conditioning latents
+        (flux/model.py:757-786)."""
+        if check_masked_training(self.config) and batch.get("encoder_attention_mask") is None:
+            raise NotImplementedError("flux_attention_masked_training: the batch has no encoder_attention_mask (the text-embed "
+                                      "cache must carry attention_masks)")
         for k in ("conditioning_packed_latents", "conditioning_ids", "conditioning_latents"):
             if batch.get(k) is not None:
                 raise NotImplementedError(f"Kontext / conditioning input `{k}` is not supported by the libstb200 Flux path")
@@ -177,6 +180,9 @@ class Flux:
         if not hasattr(latents, "to"):
             raise ValueError("Received invalid value for latents.")
         batch["latents"] = latents.to(**kw, non_blocking=True).contiguous()
+        mask = batch.get("encoder_attention_mask")
+        if mask is not None and hasattr(mask, "to"):   # common.py:5911-5913
+            batch["encoder_attention_mask"] = mask.to(**kw, non_blocking=True)
         # noise, then sigma draw — same order and generators as common.py:5938, 5068
         from ..training.noise import sample_noise
         noise, input_noise = sample_noise(c, batch["latents"], state, flow_matching=True)
@@ -237,10 +243,18 @@ class Flux:
         txt_ids = torch.zeros(pb["encoder_hidden_states"].shape[1], 3)
         # side effect kept from the reference: timesteps are overwritten with t / 1000 (flux/model.py:739-745)
         pb["timesteps"] = pb["timesteps"].to(device=dev, dtype=torch.float32) / self.noise_schedule.config.num_train_timesteps
+        attention_mask = None
+        if getattr(self.config, "flux_attention_masked_training", False):   # flux/model.py:813-822
+            attention_mask = pb.get("encoder_attention_mask")
+            if attention_mask is None:
+                raise ValueError("No attention mask was discovered when attempting validation - this means you need to "
+                                 "recreate your text embed cache.")
+            if attention_mask.dim() == 3 and attention_mask.size(1) == 1:
+                attention_mask = attention_mask.squeeze(1)   # [B, 1, S] -> [B, S]
         out = self.model(
             hidden_states=packed, timestep=pb["timesteps"], guidance=self._guidance(B, dev),
             pooled_projections=pb["added_cond_kwargs"]["text_embeds"], encoder_hidden_states=pb["encoder_hidden_states"],
-            txt_ids=txt_ids, img_ids=img_ids, joint_attention_kwargs=None, return_dict=False,
+            txt_ids=txt_ids, img_ids=img_ids, joint_attention_kwargs=None, return_dict=False, attention_mask=attention_mask,
         )[0]
         return self._prediction_dict(out, (B, Cc, Hh, Ww))
 
@@ -306,6 +320,31 @@ class Flux:
 
     def loss_with_logs(self, prepared_batch, model_output, apply_conditioning_mask: bool = True):
         return self.loss(prepared_batch, model_output, apply_conditioning_mask), None
+
+
+def check_masked_training(c) -> bool:
+    """True when `flux_attention_masked_training` is on and this path reproduces the reference's mask semantics; raises
+    NotImplementedError when it is on and the semantics are another's or unknown.
+
+    The reference's default processor (attention_mechanism "diffusers", un-fused QKV: FluxAttnProcessor2_0) passes the
+    float mask `(mask > 0).to(dtype)` to SDPA, which ADDS it to the logits: kept text keys and every image key get +1,
+    padded text keys +0, and nothing is masked out (flux/transformer.py:170-173, 200-207; SURVEY.md quirk Q2).  That is
+    what runs here.  A flash mechanism with fused QKV uses FluxFusedFlashAttnProcessor3, a varlen path with real key
+    padding (flux/model.py:369-380, flux/attention.py:207-210, 307-311); other mechanisms swap SDPA for other kernels."""
+    g = lambda k, d=None: getattr(c, k, d)
+    if not g("flux_attention_masked_training", False):
+        return False
+    mech = g("attention_mechanism", None)
+    if mech is None:
+        raise NotImplementedError("flux_attention_masked_training: the config names no attention_mechanism, so the mask "
+                                  "semantics the reference would apply are unknown; use the reference module")
+    if mech != "diffusers":
+        raise NotImplementedError(f"flux_attention_masked_training with attention_mechanism={mech!r}: only 'diffusers' "
+                                  "(the additive SDPA mask) runs on the libstb200 Flux path")
+    if g("fuse_qkv_projections", False):
+        raise NotImplementedError("flux_attention_masked_training with fuse_qkv_projections: the reference then masks "
+                                  "through a fused processor; only the un-fused 'diffusers' processor runs here")
+    return True
 
 
 def prepare_latent_image_ids(height: int, width: int) -> torch.Tensor:

@@ -275,12 +275,12 @@ class FluxTransformerBlock(nn.Module):
                 if any(l.lokr is not None for l in lins):
                     self._plans.pop(key, None)
 
-    def forward(self, h, silu_temb, cos, sin, S_txt, lora_scaling):
+    def forward(self, h, silu_temb, cos, sin, S_txt, lora_scaling, key_bias=None):
         D = self.dim
         mod_img = self.norm1.linear(silu_temb)
         mod_txt = self.norm1_context.linear(silu_temb)
         st = {"S_txt": S_txt, "H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "lora_drop": getattr(self, "_lora_drop", None)}
+              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias}
         a = self.attn
         attn_l = [a.to_q, a.to_k, a.to_v, a.to_out[0], a.add_q_proj, a.add_k_proj, a.add_v_proj, a.to_add_out]
         mlp_l = [self.ff.net[0].proj, self.ff.net[2], self.ff_context.net[0].proj, self.ff_context.net[2]]
@@ -321,10 +321,10 @@ class FluxSingleTransformerBlock(nn.Module):
         if self._plans and any(l.lokr is not None for l in (a.to_q, a.to_k, a.to_v)):
             self._plans.pop("attn", None)
 
-    def forward(self, h, silu_temb, cos, sin, lora_scaling):
+    def forward(self, h, silu_temb, cos, sin, lora_scaling, key_bias=None):
         mod = self.norm.linear(silu_temb)
         st = {"H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "lora_drop": getattr(self, "_lora_drop", None)}
+              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias}
         a = self.attn
         lora = _lora_list([a.to_q, a.to_k, a.to_v])
         st["lokr_scales"] = _lokr_scales([a.to_q, a.to_k, a.to_v])
@@ -377,6 +377,18 @@ def rope_tables(ids: torch.Tensor, axes_dim, theta: float = 10000.0) -> Tuple[to
     return torch.cat(cos_out, dim=-1).contiguous(), torch.cat(sin_out, dim=-1).contiguous()
 
 
+def flux_key_bias(attention_mask: torch.Tensor, B: int, S: int, dtype, device) -> torch.Tensor:
+    """The per-key logit bias [B, S] of Flux masked training: `expand_flux_attention_mask` (ones over the joint
+    [text | image] sequence, the text mask written into its first L columns) then `(mask > 0).to(dtype)` as
+    FluxAttnProcessor2_0 does before SDPA adds it to the logits (reference flux/transformer.py:170-173, 227-242).  So kept
+    text keys and every image key get +1 and padded text keys +0.  Device ops only: no host sync, CUDA-graph capturable."""
+    if attention_mask.dim() != 2 or attention_mask.shape[0] != B or attention_mask.shape[1] > S:
+        raise ValueError(f"attention_mask must be [B, L] with B = {B} and L <= {S}, got {tuple(attention_mask.shape)}")
+    bias = torch.ones((B, S), device=device, dtype=dtype)
+    bias[:, :attention_mask.shape[1]] = (attention_mask.to(device, non_blocking=True) > 0).to(dtype)
+    return bias
+
+
 class B200FusedAttnProcessor:
     """Marker processor: the attention of this module runs inside the libstb200 block schedule (blocks.py)."""
 
@@ -419,9 +431,14 @@ class AttnProcessorAPI:
         else:
             items = {n: processor for n in mods}
         for n, proc in items.items():
-            if type(proc).__name__ not in _EQUIVALENT_PROCESSORS:
-                raise NotImplementedError(f"attention processor {type(proc).__name__} is not reproduced by the libstb200 "
+            name = type(proc).__name__
+            if name not in _EQUIVALENT_PROCESSORS:
+                raise NotImplementedError(f"attention processor {name} is not reproduced by the libstb200 "
                                           "block schedule; use the reference module for it")
+            if getattr(self, "attention_masked_training", False) and "Flash" in name:
+                # the flash processors mask by key padding (varlen), not by the additive bias the blocks apply
+                raise NotImplementedError(f"attention processor {name} with flux_attention_masked_training applies "
+                                          "key-padding semantics the libstb200 block schedule does not reproduce")
         self.__dict__.setdefault("_attn_processor_store", {}).update(items)
 
     def fuse_qkv_projections(self):
@@ -622,7 +639,7 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
                 controlnet_single_block_samples=None, return_dict: bool = True, attention_mask=None,
                 controlnet_blocks_repeat: bool = False, force_keep_mask=None, hidden_states_buffer=None,
                 grounding_kwargs=None):
-        for nm, v in (("attention_mask", attention_mask), ("timestep_sign", timestep_sign), ("r_timestep", r_timestep),
+        for nm, v in (("timestep_sign", timestep_sign), ("r_timestep", r_timestep),
                       ("controlnet_block_samples", controlnet_block_samples),
                       ("controlnet_single_block_samples", controlnet_single_block_samples),
                       ("force_keep_mask", force_keep_mask), ("grounding_kwargs", grounding_kwargs)):
@@ -666,10 +683,13 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
             img_ids = img_ids[0]
         cos, sin = self._rope(txt_ids, img_ids, dev)[:2]
         scaling = self._lora_scaling
+        # masked training: one per-key bias for every attention of the step (an argument of each block, so the re-run
+        # under gradient checkpointing sees it too)
+        key_bias = None if attention_mask is None else flux_key_bias(attention_mask, B, S_txt + S_img, dt, dev)
         for i, blk in enumerate(self.transformer_blocks):
-            h = self._run_block(i, blk, h, silu_temb, cos, sin, S_txt, scaling)
+            h = self._run_block(i, blk, h, silu_temb, cos, sin, S_txt, scaling, key_bias)
         for i, blk in enumerate(self.single_transformer_blocks):
-            h = self._run_block(i, blk, h, silu_temb, cos, sin, scaling)
+            h = self._run_block(i, blk, h, silu_temb, cos, sin, scaling, key_bias)
         if self._tail_plan is None:
             self._tail_plan = {"w_proj": self.proj_out.weight.detach(), "b_proj": self.proj_out.bias.detach(),
                                "w_proj_t": _wt(self.proj_out.weight.detach())}

@@ -135,9 +135,20 @@ def gemm(
     return out.squeeze(0) if (squeeze and out.dim() == 3) else out
 
 
-def attn_fwd(q, k, v, scale: Optional[float] = None, out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None):
+def _key_bias_stride(key_bias: torch.Tensor, B: int, Sk: int) -> int:
+    """Batch stride of a per-key logit bias bf16 [B or 1, Sk] (keys contiguous); 0 when one row serves the batch."""
+    _chk(key_bias, "key_bias")
+    if key_bias.dim() != 2 or key_bias.shape[0] not in (1, B) or key_bias.shape[1] != Sk or key_bias.stride(1) != 1:
+        raise ValueError(f"key_bias must be [B or 1, Sk] = [{B} or 1, {Sk}] with contiguous keys, got "
+                         f"{tuple(key_bias.shape)} strides {key_bias.stride()}")
+    return 0 if key_bias.shape[0] == 1 else key_bias.stride(0)
+
+
+def attn_fwd(q, k, v, scale: Optional[float] = None, out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None,
+             key_bias: Optional[torch.Tensor] = None):
     """q/k/v: [B, S, H, HD] views (HD contiguous).  Returns (o [B,Sq,H,HD] bf16, lse [B,H,Sq] fp32).
-    bias (forward only): bf16 [H or 1, Sq, Sk] additive logit bias / mask shared by the batch."""
+    bias (forward only): bf16 [H or 1, Sq, Sk] additive logit bias / mask shared by the batch.
+    key_bias: bf16 [B or 1, Sk] additive logit bias per sample and key (Flux masked training); attn_bwd takes it too."""
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _chk(t, n)
     B, Sq, H, HD = q.shape
@@ -156,16 +167,21 @@ def attn_fwd(q, k, v, scale: Optional[float] = None, out: Optional[torch.Tensor]
     a.o = out.data_ptr()
     a.o_b, a.o_s, a.o_h = out.stride(0), out.stride(1), out.stride(2)
     a.lse = lse.data_ptr()
+    if bias is not None and key_bias is not None:
+        raise ValueError("give either bias or key_bias, not both")
     if bias is not None:
         _chk(bias, "bias")
         assert bias.dim() == 3 and bias.shape[0] in (1, H) and bias.shape[1] == Sq and bias.shape[2] == Sk
         a.bias, a.bias_h, a.bias_q = bias.data_ptr(), (0 if bias.shape[0] == 1 else bias.stride(0)), bias.stride(1)
+    if key_bias is not None:
+        a.bias, a.bias_b, a.bias_h, a.bias_q = key_bias.data_ptr(), _key_bias_stride(key_bias, B, Sk), 0, 0
     check(_lib.lib().stb_attn_fwd(C.byref(a), _stream()))
     return out, lse
 
 
-def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=None, dv=None, qk_prep: Optional[dict] = None):
-    """Backward of attn_fwd.  Returns (dq, dk, dv) shaped like q, k, v ([B, S, H, HD], bf16).
+def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=None, dv=None, qk_prep: Optional[dict] = None,
+             key_bias: Optional[torch.Tensor] = None):
+    """Backward of attn_fwd.  Returns (dq, dk, dv) shaped like q, k, v ([B, S, H, HD], bf16).  key_bias: the forward's.
 
     qk_prep (self-attention only): dict(src=[B,S,C] pre-norm projection output, k_off, wq, wk, wq_added, wk_added,
     s_split, cos, sin, eps) — fuses the backward of qk_rmsnorm_rope_fwd into the epilogues, so dq / dk receive the
@@ -207,6 +223,8 @@ def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=No
         f.cos_t, f.sin_t = _ptr(cos), _ptr(sin)
         f.eps = float(qk_prep.get("eps", 1e-6))
         a.qk_prep = C.pointer(f)
+    if key_bias is not None:
+        a.bias, a.bias_b = key_bias.data_ptr(), _key_bias_stride(key_bias, B, Sk)
     check(_lib.lib().stb_attn_bwd(C.byref(a), _stream()))
     return dq, dk, dv
 

@@ -34,16 +34,46 @@ def flash_attn_qkvpacked_func(qkv, dropout_p: float = 0.0, softmax_scale: Option
     return attention_qkvpacked(qkv, softmax_scale)
 
 
+def key_bias_from_mask(attn_mask: torch.Tensor, B: int, H: int, Sq: int, Sk: int, dtype: torch.dtype) -> torch.Tensor:
+    """The [B or 1, Sk] per-key view of an SDPA float `attn_mask` that is constant over heads and queries, decided from
+    its shape and strides alone (values are never read: no device sync).  FluxAttnProcessor2_0 passes such a mask,
+    [B, 1, 1, S] in the activation dtype (reference flux/transformer.py:170-173).  Any other mask raises
+    NotImplementedError, so the override falls back to torch."""
+    if attn_mask.dtype != dtype:
+        raise NotImplementedError(f"libstb200 SDPA: attn_mask must be a float mask in the query dtype {dtype}, "
+                                  f"got {attn_mask.dtype}")
+    if not 1 <= attn_mask.dim() <= 4:
+        raise NotImplementedError(f"libstb200 SDPA: attn_mask must have 1 to 4 dimensions, got {attn_mask.dim()}")
+    m = attn_mask
+    while m.dim() < 4:
+        m = m.unsqueeze(0)
+    mb, mh, mq, mk = m.shape
+    if mb not in (1, B) or mk != Sk or m.stride(3) != 1 or any(n != 1 and s != 0 for n, s in ((mh, m.stride(1)),
+                                                                                             (mq, m.stride(2)))):
+        raise NotImplementedError(f"libstb200 SDPA: only a per-key attn_mask [B or 1, 1, 1, Sk] (heads / queries of size 1 "
+                                  f"or stride 0, contiguous keys) is supported, got {tuple(attn_mask.shape)} strides "
+                                  f"{attn_mask.stride()} for B={B} H={H} Sq={Sq} Sk={Sk}")
+    if mh not in (1, H) or mq not in (1, Sq):
+        raise NotImplementedError(f"libstb200 SDPA: attn_mask {tuple(attn_mask.shape)} does not broadcast to "
+                                  f"[{B}, {H}, {Sq}, {Sk}]")
+    return m[:, 0, 0, :]
+
+
 def b200_sdpa(query, key, value, attn_mask=None, dropout_p=0.0, is_causal=False, scale=None, enable_gqa=False):
-    """`F.scaled_dot_product_attention` signature, layout [B, H, S, D] (what the diffusers processors pass)."""
-    if attn_mask is not None or dropout_p or is_causal or enable_gqa:
-        raise NotImplementedError("libstb200 SDPA: masks / dropout / causal / GQA are not supported")
+    """`F.scaled_dot_product_attention` signature, layout [B, H, S, D] (what the diffusers processors pass).  A float
+    `attn_mask` runs when it is per-key (key_bias_from_mask); any other mask raises."""
+    if dropout_p or is_causal or enable_gqa:
+        raise NotImplementedError("libstb200 SDPA: dropout / causal / GQA are not supported")
     if query.dim() != 4 or key.shape[1] != query.shape[1]:
         raise NotImplementedError("libstb200 SDPA expects [B, H, S, D] with equal head counts")
+    key_bias = None
+    if attn_mask is not None:
+        B, H, Sq, _ = query.shape
+        key_bias = key_bias_from_mask(attn_mask, B, H, Sq, key.shape[2], query.dtype)
     q, k, v = (t.transpose(1, 2) for t in (query, key, value))   # [B, S, H, D] views: the kernels take strides, no copies
     if q.stride(-1) != 1 or k.stride(-1) != 1 or v.stride(-1) != 1:
         raise NotImplementedError("libstb200 SDPA needs a contiguous head dimension")
-    return attention_bshd(q, k, v, scale).transpose(1, 2)
+    return attention_bshd(q, k, v, scale, key_bias=key_bias).transpose(1, 2)
 
 
 def install_sdpa_override() -> None:
