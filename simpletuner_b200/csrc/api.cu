@@ -75,6 +75,12 @@ int check_device() {
     return major == 9 && minor == 0 ? 1 : 0;
   }();
   if (!ok) return fail(STB_ERR_UNSUPPORTED, "libstb200 needs an sm_90 (H100) device; there is no CPU or other-arch fallback");
+  // The tensor-map encoder is a driver call and needs a context current on the calling thread.  A thread whose first CUDA
+  // work is a libstb200 call has none (the autograd engine's device thread, when an attention backward is the first op
+  // it runs); cudaSetDevice makes the primary context of the thread's device current.
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaSetDevice(dev) != cudaSuccess)
+    return fail(STB_ERR_CUDA, "no CUDA context for the calling thread");
   return 0;
 }
 

@@ -1,4 +1,4 @@
-"""Kernel-level parity checks of libstb200 against plain PyTorch fp32 math on the same GPU tensors.
+"""Kernel-level parity checks of libstb200 against plain PyTorch math on the same GPU tensors (fp64 for attention).
 
 Each check is a function returning a dict {"ok": bool, "max_err": ..., "tol": ..., ...}.  They are used
 by the `-m gpu` pytest tests and by tools/run_gpu_checks.py (which runs every check in its own
@@ -47,6 +47,9 @@ def _report(name, got, ref, atol, rtol, extra=None):
         out["col_block_maxerr"] = [round(float(e2[:, j * cb:(j + 1) * cb].max().item()), 4) for j in range(min(8, math.ceil(e2.shape[1] / cb)))]
     if extra:
         out.update(extra)
+    # share of the tolerance the worst element uses (1.0 = at the limit)
+    use = torch.where(err == 0, torch.zeros_like(err), err / tol)
+    out["tol_use"] = round(float(use.max().item()), 4) if use.numel() else 0.0
     return out
 
 
@@ -135,26 +138,105 @@ def check_gemm(M=256, N=256, K=128, B=1, bias=False, epi=ops.EPI_STORE, tile=(0,
 
 
 # --------------------------------------------------------------------------------------------- attention
-def _attn_ref(q, k, v, scale, bias=None):
-    # q,k,v [B,S,H,D] -> fp32 reference in [B,S,H,D]; bias [H or 1, Sq, Sk] is added to the scaled logits
-    qf, kf, vf = (t.float().permute(0, 2, 1, 3) for t in (q, k, v))
-    s = (qf @ kf.transpose(-1, -2)) * scale
-    if bias is not None:
-        s = s + bias.float()
-    lse = torch.logsumexp(s, dim=-1)
-    p = torch.softmax(s, dim=-1)
-    o = p @ vf
-    return o.permute(0, 2, 1, 3), lse
+def _attn_ref(q, k, v, scale, bias=None, key_bias=None, d_o=None, o=None):
+    """fp64 attention on the kernel's own bf16 inputs, one (batch, head) at a time so that memory stays at a few S x S
+    matrices.  q / k / v / d_o [B, S, H, HD]; bias [H or 1, Sq, Sk] shared by the batch, or key_bias [B or 1, Sk].
+    Returns {"o", "lse"} and, with d_o, {"dq", "dk", "dv"} from the explicit formulas:
+      P = softmax(scale Q K^T + bias),  dV = P^T dO,  dS = P o (dO V^T - rowsum(dO o O)),  dQ = scale dS K,  dK = scale dS^T Q
+    o: the forward output the backward is given (bf16), used for O in rowsum(dO o O) as the backward uses it; the exact
+    output when None.  With a peaked softmax dS is the small difference of two nearly equal terms and the forward's bf16
+    rounding of O alone moves dq / dk by several times their tolerance; that error belongs to the forward's o, which
+    the checks compare with the exact one."""
+    B, Sq, H, _ = q.shape
+    o_in = o
+    f64 = lambda t: t.detach().to(torch.float64)
+    ref = {"o": torch.empty(q.shape, dtype=torch.float64, device=q.device),
+           "lse": torch.empty(B, H, Sq, dtype=torch.float64, device=q.device)}
+    if d_o is not None:
+        ref.update(dq=torch.empty_like(ref["o"]), dk=torch.empty(k.shape, dtype=torch.float64, device=q.device),
+                   dv=torch.empty(v.shape, dtype=torch.float64, device=q.device))
+    for b in range(B):
+        for h in range(H):
+            qh, kh, vh = f64(q[b, :, h]), f64(k[b, :, h]), f64(v[b, :, h])
+            s = (qh @ kh.t()) * scale
+            if bias is not None:
+                s += f64(bias[h % bias.shape[0]])
+            if key_bias is not None:
+                s += f64(key_bias[b % key_bias.shape[0]])[None, :]
+            lse = torch.logsumexp(s, -1)
+            p = torch.exp(s - lse[:, None])
+            o = p @ vh
+            ref["o"][b, :, h], ref["lse"][b, h] = o, lse
+            if d_o is not None:
+                g = f64(d_o[b, :, h])
+                ob = o if o_in is None else f64(o_in[b, :, h])
+                ds = p * (g @ vh.t() - (g * ob).sum(-1, keepdim=True))
+                ref["dq"][b, :, h] = scale * (ds @ kh)
+                ref["dk"][b, :, h] = scale * (ds.t() @ qh)
+                ref["dv"][b, :, h] = p.t() @ g
+    return ref
+
+
+# Per-element tolerance atol + rtol |ref| against the fp64 reference.  atol is in units of the RMS of the element's own
+# reference row (one query or key of one head, over the head dim), not of max |ref|: for unit-variance inputs max |ref| is
+# 4-5x the RMS, so a max-scaled atol let typical elements be off by 10 % of the RMS.  Per row rather than over the whole
+# tensor because a per-key bias scales each key's dk / dv (and a peaked softmax each query's dq) by a factor of its own:
+# with an N(0, 2^2) bias a few keys carry most of the tensor's RMS, and a global RMS would be 7x too small an atol for the
+# rest (measured on H100 at the Flux shape, and reproduced by a model of the kernels' bf16 roundings).
+#   o, dq, dk, dv: rtol 2^-7 because the bf16 store alone rounds by up to half an ulp = 2^-8 |x|, which would use all of
+#                  an rtol of 2^-8 on a large element.  The atol covers P (forward) and P^T / dS (backward) rounded to
+#                  bf16 before their MMAs: 2e-2 RMS for o (1e-2 was used up to 0.88 on H100) and 2.5e-2 for the
+#                  gradients (2e-2 was used up to 0.56 with a 64-key tail), so that the unmodified kernels stay at or
+#                  below half of every tolerance.
+#   lse:           fp32 throughout.
+# When every row has a single key (P = 1) the reference gradients dq / dk are 0, and the kernel's are the ~1e-6 residue of
+# dP - Delta (two fp32 dot products of the same values, summed in different orders): hence the floor on the RMS.
+ATTN_TOL = {"o": (2 ** -7, 2e-2), "dq": (2 ** -7, 2.5e-2), "dk": (2 ** -7, 2.5e-2), "dv": (2 ** -7, 2.5e-2)}
+LSE_TOL = 2e-4
+
+
+def _row_rms(ref, floor=1e-3):
+    """RMS of each row of the last dim, floored: the atol scale of attn_compare."""
+    return ref.double().pow(2).mean(-1, keepdim=True).sqrt().clamp_min(floor)
+
+
+def attn_compare(name, got, ref):
+    """got / ref: dicts holding some of o, lse, dq, dk, dv.  One result dict: ok, the worst share of the tolerance used
+    (tol_use, overall and per tensor), max errors, and the element-wise detail of a failing tensor."""
+    out = {"name": name, "ok": True}
+    for nm in ("o", "lse", "dq", "dk", "dv"):
+        if nm not in got:
+            continue
+        if nm == "lse":
+            r = _report(nm, got[nm], ref[nm], atol=LSE_TOL, rtol=LSE_TOL)
+        else:
+            rtol, arms = ATTN_TOL[nm]
+            r = _report(nm, got[nm], ref[nm], atol=arms * _row_rms(ref[nm]), rtol=rtol)
+        out[f"{nm}_tol_use"], out[f"{nm}_max_err"] = r["tol_use"], r["max_err"]
+        if not r["ok"]:
+            out["ok"] = False
+            out[f"{nm}_detail"] = r
+    out["tol_use"] = max(v for n, v in out.items() if n.endswith("_tol_use"))
+    return out
 
 
 def _attn_bias(kind, H, Sq, Sk, keep=None):
-    """Additive logit bias [H or 1, Sq, Sk] (bf16) for the text-encoder instantiation of attn_fwd.  Every query row keeps a
-    finite logit in its first 128-key tile (the kernel's precondition).
+    """Additive logit bias [H or 1, Sq, Sk] (bf16) for the general instantiation of attn_fwd (text encoders).  Every query
+    row needs one finite key anywhere; a 128-key tile that is -inf for a row contributes nothing to it.
       head / shared: dense relative-position-like bias, per head or one for all heads
       causal:        0 on and below the diagonal, -inf above it
-      keypad:        0 for the first `keep` keys, -inf for the rest (whole later key tiles masked)"""
+      keypad:        0 for the first `keep` keys, -inf for the rest (whole later key tiles masked)
+      leftpad:       dense per head, with -inf in front of some rows (left-padded text): rows 3i over the whole first
+                     128-key tile, rows 3i + 1 over every key but the last (in the partial tail tile), rows 3i + 2 over
+                     their first i % 128 keys"""
     if kind in ("head", "shared"):
         return _rand(H if kind == "head" else 1, Sq, Sk, scale=2.0, seed=6)
+    if kind == "leftpad":
+        assert Sk > 128
+        b = _rand(H, Sq, Sk, scale=2.0, seed=6).float().cpu()
+        for r in range(Sq):
+            b[:, r, :(128, Sk - 1, (r // 3) % 128)[r % 3]] = float("-inf")
+        return b.to(torch.bfloat16).to(DEV)
     b = torch.zeros(1, Sq, Sk, dtype=torch.float32)
     if kind == "causal":
         b.masked_fill_(torch.ones(Sq, Sk, dtype=torch.bool).triu(1), float("-inf"))
@@ -165,8 +247,49 @@ def _attn_bias(kind, H, Sq, Sk, keep=None):
     return b.to(torch.bfloat16).to(DEV)
 
 
-def check_attn_fwd(B=1, H=2, Sq=256, Sk=None, HD=128, strided=False, name=None, qscale=1.0, bias=None, keep=None):
-    """bias: None or a _attn_bias kind; the reference is the fp32 softmax of scale * q.k + bias."""
+def _key_bias(kind, B, Sk, seed=0):
+    """Per-key logit bias [B or 1, Sk] (bf16, Flux masked training), different for every sample unless stated:
+      dense:          N(0, 2^2) per (sample, key): a bias taken from the wrong key, row, lane or sample moves every element
+      01 / neg:       ones with one run of 0 / -10000 per sample (the 0/1 mask of the reference and its additive form)
+      inf:            -inf over the first 128-key tile (all keys but the last when Sk <= 128) and over whole 64-key blocks
+      inf_first_tile: dense, -inf over the whole first 128-key tile (Sk > 128)
+      inf_straddle:   dense, -inf runs across the 64- and 128-key boundaries (the backward's and the forward's key tiles)
+      last_key_only:  -inf on every key but Sk - 1 (dense), which lies in the partial tail tile
+      mixed:          sample 0 all zeros, the others dense
+      shared:         one dense [1, Sk] row for the whole batch (batch stride 0)"""
+    g = torch.Generator().manual_seed(seed)
+    bias = torch.randn(B, Sk, generator=g) * 2.0
+    if kind in ("01", "neg", "inf"):
+        bias.fill_(1.0)
+        for b in range(B):
+            n = int(torch.randint(0, Sk, (1,), generator=g)) if Sk > 1 else 0
+            if kind == "inf":
+                bias[b, :min(128, Sk - 1)] = -math.inf
+                for k0 in range(192, Sk - 64, 128 * (b + 1)):
+                    bias[b, k0:k0 + 64] = -math.inf
+            else:
+                bias[b, n:min(Sk, n + 1 + Sk // (b + 2))] = 0.0 if kind == "01" else -10000.0
+    elif kind == "inf_first_tile":
+        assert Sk > 128
+        bias[:, :128] = -math.inf
+    elif kind == "inf_straddle":
+        for b in range(B):
+            for edge in (64, 128, 192, 256, 320):
+                bias[b, max(1, edge - 5 - 3 * b):min(Sk, edge + 7 + 2 * b)] = -math.inf
+    elif kind == "last_key_only":
+        bias[:, :-1] = -math.inf
+    elif kind == "mixed":
+        bias[0] = 0.0
+    elif kind == "shared":
+        bias = bias[:1]
+    elif kind != "dense":
+        raise ValueError(kind)
+    return bias.to(torch.bfloat16).to(DEV)
+
+
+def check_attn_fwd(B=1, H=2, Sq=256, Sk=None, HD=128, strided=False, name=None, qscale=1.0, bias=None, keep=None,
+                   key_bias=None, seed=0):
+    """bias: None or an _attn_bias kind; key_bias: None or a _key_bias kind.  o and lse against the fp64 reference."""
     Sk = Sk or Sq
     if strided:
         # q/k/v as slices of a fused [B, S, 3*H*HD] projection buffer (the layout the model uses)
@@ -181,19 +304,17 @@ def check_attn_fwd(B=1, H=2, Sq=256, Sk=None, HD=128, strided=False, name=None, 
         v = _rand(B, Sk, H, HD, seed=3)
     scale = HD ** -0.5
     bias_t = _attn_bias(bias, H, Sq, Sk, keep) if bias else None
-    o, lse = ops.attn_fwd(q, k, v, scale, bias=bias_t)
+    kb = _key_bias(key_bias, B, Sk, seed) if key_bias else None
+    o, lse = ops.attn_fwd(q, k, v, scale, bias=bias_t, key_bias=kb)
     torch.cuda.synchronize()
-    o_ref, lse_ref = _attn_ref(q, k, v, scale, bias_t)
-    r = _report(name or f"attn_fwd_B{B}_H{H}_Sq{Sq}_Sk{Sk}_HD{HD}", o, o_ref, atol=2e-2 * float(o_ref.abs().max()), rtol=2e-2)
-    r2 = _report("lse", lse, lse_ref, atol=2e-2, rtol=1e-3)
-    r["lse_ok"] = r2["ok"]
-    r["lse_max_err"] = r2["max_err"]
-    r["ok"] = r["ok"] and r2["ok"]
-    return r
+    ref = _attn_ref(q, k, v, scale, bias=bias_t, key_bias=kb)
+    return attn_compare(name or f"attn_fwd_B{B}_H{H}_Sq{Sq}_Sk{Sk}_HD{HD}", {"o": o, "lse": lse}, ref)
 
 
-def check_attn_bwd(B=1, H=2, Sq=256, Sk=None, HD=128, name=None, strided=False, qscale=1.0):
-    """strided: q / k / v are views of a fused [B, S, 3 H HD] projection and dq / dk / dv are written through views of a
+def check_attn_bwd(B=1, H=2, Sq=256, Sk=None, HD=128, name=None, strided=False, qscale=1.0, key_bias=None, seed=0):
+    """Forward then backward; o, lse, dq, dk, dv against the fp64 reference.  key_bias: None or a _key_bias kind; keys it
+    masks with -inf must get dk = dv = 0 exactly.
+    strided: q / k / v are views of a fused [B, S, 3 H HD] projection and dq / dk / dv are written through views of a
     zero-filled fused gradient buffer with a halo of extra rows and columns, which must stay zero."""
     Sk = Sk or Sq
     D = H * HD
@@ -213,23 +334,17 @@ def check_attn_bwd(B=1, H=2, Sq=256, Sk=None, HD=128, name=None, strided=False, 
         dq_o = dk_o = dv_o = None
     d_o = _rand(B, Sq, H, HD, seed=4)
     scale = HD ** -0.5
-    o, lse = ops.attn_fwd(q, k, v, scale)
-    dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse, scale, dq=dq_o, dk=dk_o, dv=dv_o)
+    kb = _key_bias(key_bias, B, Sk, seed) if key_bias else None
+    o, lse = ops.attn_fwd(q, k, v, scale, key_bias=kb)
+    dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse, scale, dq=dq_o, dk=dk_o, dv=dv_o, key_bias=kb)
     torch.cuda.synchronize()
-    qf, kf, vf = (t.float().requires_grad_(True) for t in (q, k, v))
-    o_ref, _ = _attn_ref(qf, kf, vf, scale)
-    o_ref.backward(d_o.float())
-    res = {}
-    ok = True
-    for nm, got, ref in (("dq", dq, qf.grad), ("dk", dk, kf.grad), ("dv", dv, vf.grad)):
-        # with a single key every P is 1 and dS = P (dP - Delta) vanishes identically, so dq = dk = 0 in the reference; the
-        # kernel's two fp32 dot products (dO . v on the tensor core, dO . o in the Delta kernel) cancel to ~1e-6, hence the
-        # floor on the magnitude (it is far below 3e-2 * max|ref| everywhere else, for these unit-scale inputs)
-        r = _report(nm, got, ref, atol=3e-2 * max(float(ref.abs().max()), 1e-3), rtol=3e-2)
-        res[nm] = r
-        ok = ok and r["ok"]
-    out = {"name": name or f"attn_bwd_B{B}_H{H}_Sq{Sq}_Sk{Sk}_HD{HD}", "ok": ok,
-           "max_err": max(res[n]["max_err"] for n in res), **{f"{n}_detail": res[n] for n in res if not res[n]["ok"]}}
+    ref = _attn_ref(q, k, v, scale, key_bias=kb, d_o=d_o, o=o)
+    out = attn_compare(name or f"attn_bwd_B{B}_H{H}_Sq{Sq}_Sk{Sk}_HD{HD}" + (f"_kb_{key_bias}" if key_bias else ""),
+                       {"o": o, "lse": lse, "dq": dq, "dk": dk, "dv": dv}, ref)
+    if kb is not None and bool(torch.isinf(kb.float()).any()):
+        dead = torch.isinf(kb.float())[:, :, None, None].expand(B, Sk, H, HD)
+        out["masked_keys_zero"] = bool((dk[dead] == 0).all()) and bool((dv[dead] == 0).all())
+        out["ok"] = out["ok"] and out["masked_keys_zero"]
     if strided:
         mask = torch.ones_like(gfull, dtype=torch.bool)
         mask[:, 1:Sq + 1, 8:8 + 3 * D] = False
@@ -694,36 +809,44 @@ CHECKS.update({
 
 
 # --------------------------------------------------------------------------------------------- fused q/k-prep backward epilogue
-def check_attn_bwd_fused_prep(B=2, S=333, H=3, HD=128, s_split=77, rope=True, norm_w=True):
-    """attn_bwd(qk_prep=...) == attn_bwd -> qk_rmsnorm_rope_bwd (the two-kernel path) on the same inputs."""
+def check_attn_bwd_fused_prep(B=2, S=333, H=3, HD=128, s_split=77, rope=True, norm_w=True, key_bias=None):
+    """attn_bwd(qk_prep=...) == attn_bwd -> qk_rmsnorm_rope_bwd (the two-kernel path) on the same inputs; dv, which the
+    prep does not touch, bit for bit.  key_bias: None or a _key_bias kind."""
     D = H * HD
     qkv = _rand(B, S, 3 * D, seed=1)
     d_o = _rand(B, S, H, HD, seed=2)
     mk = lambda sd: (1.0 + 0.1 * _rand(HD, seed=sd).float()).bfloat16() if norm_w else None
     wq, wk, wqa, wka = mk(3), mk(4), mk(5), mk(6)
     cos, sin = _rope_tables(S, HD) if rope else (None, None)
+    kb = _key_bias(key_bias, B, S, seed=9) if key_bias else None
     q, k = ops.qk_rmsnorm_rope_fwd(qkv, D, H, HD, wq, wk, wqa, wka, s_split, cos, sin, 1e-6)
     v = qkv[:, :, 2 * D:].unflatten(-1, (H, HD))
-    o, lse = ops.attn_fwd(q, k, v)
+    o, lse = ops.attn_fwd(q, k, v, key_bias=kb)
     # reference: two kernels
-    dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse)
+    dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse, key_bias=kb)
     ref = torch.zeros_like(qkv)
     ops.qk_rmsnorm_rope_bwd(dq, dk, qkv, D, H, HD, wq, wk, wqa, wka, s_split, cos, sin, 1e-6, dsrc=ref)
     ref[:, :, 2 * D:] = dv.reshape(B, S, D)
     got = torch.zeros_like(qkv)
     ops.attn_bwd(q, k, v, o, d_o, lse, dq=got[:, :, 0:D].unflatten(-1, (H, HD)), dk=got[:, :, D:2 * D].unflatten(-1, (H, HD)),
-                 dv=got[:, :, 2 * D:].unflatten(-1, (H, HD)),
+                 dv=got[:, :, 2 * D:].unflatten(-1, (H, HD)), key_bias=kb,
                  qk_prep=dict(src=qkv, k_off=D, wq=wq, wk=wk, wq_added=wqa, wk_added=wka, s_split=s_split, cos=cos, sin=sin, eps=1e-6))
     torch.cuda.synchronize()
-    # the two-kernel path rounds dq / dk to bf16 before the norm backward, the fused one does not
-    return _report(f"attn_bwd_fused_prep_S{S}_HD{HD}_rope{int(rope)}_w{int(norm_w)}", got, ref,
-                   atol=2e-2 * float(ref.float().abs().max()), rtol=2e-2)
+    # Both sides are bf16 and the two-kernel path rounds dq / dk to bf16 before the norm backward, the fused one does not:
+    # the two results may land on neighbouring bf16 values, one ulp = up to 2^-7 |x| apart, hence rtol 2^-6.
+    rows = lambda t: t.unflatten(-1, (3 * H, HD))   # one row per token and head, as attn_compare scales its atol
+    r = _report(f"attn_bwd_fused_prep_S{S}_HD{HD}_rope{int(rope)}_w{int(norm_w)}" + (f"_kb_{key_bias}" if key_bias else ""),
+                rows(got), rows(ref), atol=2e-2 * _row_rms(rows(ref)), rtol=2 ** -6)
+    r["dv_exact"] = bool(torch.equal(got[:, :, 2 * D:], ref[:, :, 2 * D:]))
+    r["ok"] = r["ok"] and r["dv_exact"]
+    return r
 
 
 CHECKS.update({
     "attn_bwd_fused_prep": lambda: check_attn_bwd_fused_prep(),
     "attn_bwd_fused_prep_hd64_norope": lambda: check_attn_bwd_fused_prep(B=1, S=320, H=4, HD=64, s_split=0, rope=False),
     "attn_bwd_fused_prep_now": lambda: check_attn_bwd_fused_prep(B=1, S=256, H=2, HD=128, s_split=0, rope=True, norm_w=False),
+    "attn_bwd_fused_prep_key_bias": lambda: check_attn_bwd_fused_prep(key_bias="dense"),
 })
 
 
@@ -944,6 +1067,48 @@ for _hd in (64, 128):
     CHECKS[f"attn_fwd_bias_ragged_hd{_hd}"] = _case(check_attn_fwd, 1, 2, 150, 333, HD=_hd, bias="head")
 CHECKS["attn_bwd_strided_bigscore"] = lambda: check_attn_bwd(1, 2, 1024, strided=True, qscale=4.0)
 CHECKS["attn_bwd_bigscore_long"] = lambda: check_attn_bwd(1, 2, 4608, qscale=4.0)
+for _hd in (64, 128):
+    # general bias after the all--inf-tile fix: rows -inf over their whole first 128-key tile, or over every key but the
+    # last one; with Sk = 150 every finite key of those rows lies in the partial second tile
+    CHECKS[f"attn_fwd_bias_leftpad_hd{_hd}"] = _case(check_attn_fwd, 2, 3, 200, 333, HD=_hd, bias="leftpad")
+    CHECKS[f"attn_fwd_bias_leftpad_tail_hd{_hd}"] = _case(check_attn_fwd, 1, 2, 129, 150, HD=_hd, bias="leftpad")
+
+
+# --------------------------------------------------------------------------------------------- per-key bias (masked training)
+# Every _key_bias kind meets every key-count tail class: one key, one short of a 64-key tile, whole tiles, one past a
+# tile, ragged.  Sq (1, 7, 65, 129, 333), HD and B in {1, 3} rotate along the grid.  The backward checks also check the
+# forward's o and lse, which the backward reads.
+_KB_KINDS = ("dense", "01", "neg", "inf", "inf_first_tile", "inf_straddle", "last_key_only", "mixed", "shared")
+_KB_SK = ((1,), (63, 127, 191), (64, 128), (65, 129), (333,))
+_KB_SQ = (1, 7, 65, 129, 333)
+for _ki, _kind in enumerate(_KB_KINDS):
+    for _ci, _sks in enumerate(_KB_SK):
+        _sks = [s for s in _sks if _kind != "inf_first_tile" or s > 128]
+        if not _sks:
+            continue
+        _sk, _sq, _hd = _sks[_ki % len(_sks)], _KB_SQ[(_ki + _ci) % 5], (64, 128)[(_ki + _ci) % 2]
+        _b = 1 if (2 * _ci + _ki) % 3 == 0 and _kind not in ("mixed", "shared") else 3
+        CHECKS[f"attn_bwd_kb_{_kind}_sq{_sq}_sk{_sk}_hd{_hd}_b{_b}"] = _case(check_attn_bwd, _b, 2, _sq, _sk, HD=_hd,
+                                                                             key_bias=_kind, seed=_ki + _ci)
+for _hd in (64, 128):
+    for _s in (1, 17, 64, 77, 128, 129):
+        for _kind in ("01", "neg"):
+            CHECKS[f"attn_bwd_kb_{_kind}_self_s{_s}_hd{_hd}"] = _case(check_attn_bwd, 1 + _s % 3, 2, _s, HD=_hd, key_bias=_kind,
+                                                                     seed=_s)
+    for _sq, _sk, _kind in ((100, 300, "01"), (300, 77, "01"), (129, 520, "01"), (100, 300, "inf"), (129, 520, "inf")):
+        CHECKS[f"attn_bwd_kb_{_kind}_cross_sq{_sq}_sk{_sk}_hd{_hd}"] = _case(check_attn_bwd, 3, 3, _sq, _sk, HD=_hd,
+                                                                             key_bias=_kind, seed=_sq + _sk)
+    # the model's layout (fused [B, S, 3 H HD] buffers, halo must stay zero) and a peaked softmax
+    CHECKS[f"attn_bwd_kb_strided_hd{_hd}"] = _case(check_attn_bwd, 2, 3, 333, HD=_hd, strided=True, key_bias="dense")
+    CHECKS[f"attn_bwd_kb_strided_straddle_hd{_hd}"] = _case(check_attn_bwd, 3, 2, 200, HD=_hd, strided=True,
+                                                            key_bias="inf_straddle")
+    CHECKS[f"attn_bwd_kb_bigscore_hd{_hd}"] = _case(check_attn_bwd, 2, 2, 512, HD=_hd, qscale=4.0, key_bias="dense")
+    CHECKS[f"attn_fwd_kb_strided_hd{_hd}"] = _case(check_attn_fwd, 2, 4, 384, HD=_hd, strided=True, key_bias="dense")
+    CHECKS[f"attn_fwd_kb_ragged_hd{_hd}"] = _case(check_attn_fwd, 3, 2, 333, 417, HD=_hd, key_bias="inf_straddle")
+# Flux.1: 24 heads of 128, 512 text + 4096 image tokens; and the HD 64 long shape
+for _kind in ("dense", "01", "inf"):
+    CHECKS[f"attn_bwd_kb_flux_{_kind}"] = _case(check_attn_bwd, 1, 24, 4608, HD=128, key_bias=_kind, seed=7)
+CHECKS["attn_bwd_kb_hd64_long_dense"] = _case(check_attn_bwd, 2, 3, 1255, HD=64, key_bias="dense")
 
 
 # --------------------------------------------------------------------------------------------- entry points without another check
