@@ -180,7 +180,10 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
 /* ---------------------------------------------------------------------------------------------
  * Flow-matching batch prep and loss (Flux 2x2 patchify folded into the index math).
  *   stb_flow_prep_pack : noisy = (1 - sigma) * latents + sigma * noise  (common.py:4975-4992),
- *                        written unpacked (optional) and packed (flux/__init__.py:25-30).
+ *                        written unpacked (optional) and packed (flux/__init__.py:25-30).  Packed batch rows
+ *                        are packed_b elements apart (>= (Hh/2)(Ww/2)*4C; offset `packed` to start at a token), so
+ *                        the tokens can fill a range of a joint sequence.  noise = sigmas = noisy = NULL: a plain
+ *                        pack_latents (Flux Kontext reference latents, flux/__init__.py:64-172).
  *   stb_flow_mse_loss  : mean_b mean_chw (pred.float() - (noise - latents).float())^2
  *                        (common.py:4610-4611, 6286, 6426-6429) with pred in packed layout
  *                        (layout 0: Flux unpack_latents order, flux/__init__.py:33-44; layout 1: SD3
@@ -192,7 +195,7 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
  * per-sample c (constant or the scheduled value of common.py:6168-6215), may be NULL for l2.
  * ------------------------------------------------------------------------------------------- */
 int stb_flow_prep_pack(const void* latents, const void* noise, const float* sigmas, void* noisy,
-                       void* packed, int B, int C, int Hh, int Ww, void* stream);
+                       void* packed, long long packed_b, int B, int C, int Hh, int Ww, void* stream);
 int stb_flow_mse_loss(const void* pred_packed, const void* latents, const void* noise, float* loss_out,
                       void* dpred_packed, float grad_scale, int B, int C, int Hh, int Ww, int layout, int loss_type,
                       const float* huber_c, void* stream);

@@ -132,7 +132,7 @@ SYMBOLS = {
     "stb_ln_modulate_bwd": (_I, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _P, _LL, _LL, _P, _LL, _LL, _I, _I, _I, _F, _P]),
     "stb_qk_rmsnorm_rope_fwd": (_I, [_P, _LL, _LL, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P, _LL, _LL, _I, _I, _I, _I, _F, _P]),
     "stb_qk_rmsnorm_rope_bwd": (_I, [_P, _P, _LL, _LL, _P, _LL, _LL, _I, _P, _P, _P, _P, _I, _P, _P, _P, _LL, _LL, _I, _I, _I, _I, _F, _P, _P]),
-    "stb_flow_prep_pack": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "stb_flow_prep_pack": (_I, [_P, _P, _P, _P, _P, _LL, _I, _I, _I, _I, _P]),
     "stb_flow_mse_loss": (_I, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _I, _I, _I, _P, _P]),
     "stb_ddpm_prep_pack": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "stb_target_mse_loss": (_I, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _I, _I, _I, _P, _P]),

@@ -614,13 +614,16 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
 }
 
 int stb_flow_prep_pack(const void* latents, const void* noise, const float* sigmas, void* noisy,
-                       void* packed, int B, int C, int Hh, int Ww, void* stream) {
+                       void* packed, long long packed_b, int B, int C, int Hh, int Ww, void* stream) {
   if (int r = check_device()) return r;
   if ((Hh & 1) || (Ww & 1)) return fail(STB_ERR_ARG, "latent H and W must be even for 2x2 patchify");
+  if (!noise && (sigmas || noisy)) return fail(STB_ERR_ARG, "flow_prep_pack: sigmas / noisy need noise");
+  if (noise && !sigmas) return fail(STB_ERR_ARG, "flow_prep_pack: noise needs sigmas");
+  if (packed_b < (long long)(Hh / 2) * (Ww / 2) * 4 * C) return fail(STB_ERR_ARG, "flow_prep_pack: packed_b below one sample's tokens");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long n = (long long)B * C * Hh * Ww;
   const int grid = (int)std::min<long long>((n + 255) / 256, (long long)num_sms() * 16);
-  stb::flow_prep_pack_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(latents), static_cast<const __nv_bfloat16*>(noise), sigmas, static_cast<__nv_bfloat16*>(noisy), static_cast<__nv_bfloat16*>(packed), B, C, Hh, Ww);
+  stb::flow_prep_pack_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(latents), static_cast<const __nv_bfloat16*>(noise), sigmas, static_cast<__nv_bfloat16*>(noisy), static_cast<__nv_bfloat16*>(packed), packed_b, B, C, Hh, Ww);
   STB_LAUNCH_CHECK("flow_prep_pack");
   return 0;
 }

@@ -526,12 +526,14 @@ qk_rmsnorm_rope_flat128_kernel(const __nv_bfloat16* __restrict__ g_q, const __nv
 // reference: common.py:4975-4992 (_prepare_flow_noisy_latents: (1-sigma) x + sigma eps),
 //            flux/__init__.py:25-30 (pack_latents).  latents/noise: [B, C, Hh, Ww] contiguous.
 // noisy (bf16, reference tensor dtype) is written both unpacked [B,C,Hh,Ww] and packed
-// [B, (Hh/2)(Ww/2), 4C];  packed index = ((c*2 + dy)*2 + dx).
+// [B, (Hh/2)(Ww/2), 4C];  packed index = ((c*2 + dy)*2 + dx).  Packed batch rows lie packed_b elements
+// apart, so the tokens can land in a token range of a longer joint sequence (Flux Kontext: scene tokens, then
+// each reference image's tokens).  noise == NULL: plain pack_latents of the latents, no noise and no sigma.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 flow_prep_pack_kernel(const __nv_bfloat16* __restrict__ lat, const __nv_bfloat16* __restrict__ noise,
                       const float* __restrict__ sigmas, __nv_bfloat16* __restrict__ noisy,
-                      __nv_bfloat16* __restrict__ packed, int B, int C, int Hh, int Ww) {
+                      __nv_bfloat16* __restrict__ packed, long long packed_b, int B, int C, int Hh, int Ww) {
   const long long n = (long long)B * C * Hh * Ww;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
@@ -540,18 +542,21 @@ flow_prep_pack_kernel(const __nv_bfloat16* __restrict__ lat, const __nv_bfloat16
     const int hh = int(r % Hh); r /= Hh;
     const int c = int(r % C);
     const int b = int(r / C);
-    // reference arithmetic (common.py:4953-4960, 4989-4991): the sigma grid is cast to the latent
-    // dtype (bf16) first, then every op of (1 - g) * x + g * eps is a bf16 tensor op — reproduce
-    // each rounding so the result is bit-identical to the eager chain.
-    const float sg = bf16r(sigmas[b]);
-    const float x = __bfloat162float(lat[i]);
-    const float e = __bfloat162float(noise[i]);
-    const float v = bf16r(bf16r(1.f - sg) * x) + bf16r(sg * e);
-    const __nv_bfloat16 vb = __float2bfloat16(v);
-    if (noisy) noisy[i] = vb;
+    __nv_bfloat16 vb = lat[i];
+    if (noise) {
+      // reference arithmetic (common.py:4953-4960, 4989-4991): the sigma grid is cast to the latent
+      // dtype (bf16) first, then every op of (1 - g) * x + g * eps is a bf16 tensor op — reproduce
+      // each rounding so the result is bit-identical to the eager chain.
+      const float sg = bf16r(sigmas[b]);
+      const float x = __bfloat162float(vb);
+      const float e = __bfloat162float(noise[i]);
+      const float v = bf16r(bf16r(1.f - sg) * x) + bf16r(sg * e);
+      vb = __float2bfloat16(v);
+      if (noisy) noisy[i] = vb;
+    }
     const int ph = hh >> 1, dy = hh & 1, pw = w >> 1, dx = w & 1;
     const long long tok = (long long)ph * (Ww >> 1) + pw;
-    const long long pi = ((long long)b * ((Hh >> 1) * (Ww >> 1)) + tok) * (4 * C) + ((c * 2 + dy) * 2 + dx);
+    const long long pi = (long long)b * packed_b + tok * (4 * C) + ((c * 2 + dy) * 2 + dx);
     packed[pi] = vb;
   }
 }

@@ -306,6 +306,88 @@ def _dgrad_through_gelu(dy, w_t, pack: Optional[LoraPack], drop: Optional[LoraDr
     return ops.mul_dgelu_tanh(d_act, pre, out=d_act), t_up
 
 
+# ------------------------------------------------------------------------------------------------
+# token segments (Flux Kontext): a stream whose tokens fall into segments with their own modulation rows
+# ------------------------------------------------------------------------------------------------
+def _segments(mod: torch.Tensor, counts, n: int):
+    """[(token slice of the stream, modulation rows [B, kD])].  counts None: one segment, `mod` [B, kD]; otherwise `mod`
+    stacks one [B, kD] block per segment (segment-major) and counts[i] tokens follow each other."""
+    if counts is None:
+        return [(slice(0, n), mod)]
+    B = mod.shape[0] // len(counts)
+    out, s0 = [], 0
+    for i, c in enumerate(counts):
+        out.append((slice(s0, s0 + c), mod[i * B:(i + 1) * B]))
+        s0 += c
+    assert s0 == n, (counts, n)
+    return out
+
+
+def _chunk(mod: torch.Tensor, i: int, D: int) -> torch.Tensor:
+    return mod[:, i * D:(i + 1) * D]
+
+
+def _out(x: torch.Tensor, out: Optional[torch.Tensor]) -> torch.Tensor:
+    return out if out is not None else torch.empty(x.shape, device=x.device, dtype=torch.bfloat16)
+
+
+# Each output row of the LayerNorm-modulate, gate and GATE_RES kernels depends on its own row and its sample's
+# modulation row only, so one launch per segment gives the bits of a per-token modulation (reference
+# flux/transformer.py:386-412, the 3-D branches of the adaLN helpers).
+def _lnm_fwd(x, segs, ish: int, isc: int, out=None):
+    if len(segs) == 1:
+        m = segs[0][1]
+        return ops.ln_modulate_fwd(x, _chunk(m, ish, x.shape[2]), _chunk(m, isc, x.shape[2]), EPS, out=out)
+    out = _out(x, out)
+    for sl, m in segs:
+        ops.ln_modulate_fwd(x[:, sl], _chunk(m, ish, x.shape[2]), _chunk(m, isc, x.shape[2]), EPS, out=out[:, sl])
+    return out
+
+
+def _lnm_bwd(d, x, segs, isc: int, add=None, out=None):
+    out = _out(x, out)
+    for sl, m in segs:
+        ops.ln_modulate_bwd(d[:, sl], x[:, sl], _chunk(m, isc, x.shape[2]), add=None if add is None else add[:, sl], eps=EPS,
+                            out=out[:, sl])
+    return out
+
+
+def _gate_mul(x, segs, ig: int):
+    if len(segs) == 1:
+        return ops.gate_mul(x, _chunk(segs[0][1], ig, x.shape[2]))
+    out = _out(x, None)
+    for sl, m in segs:
+        ops.gate_mul(x[:, sl], _chunk(m, ig, x.shape[2]), out=out[:, sl])
+    return out
+
+
+def _gemm_gate_res(a_list, w_list, bias, segs, ig: int, res, out=None, nan_to_num=False):
+    """ops.gemm with the GATE_RES epilogue, one launch per segment (each segment gates with its own rows)."""
+    D = res.shape[2]
+    if len(segs) == 1:
+        return ops.gemm(a_list, w_list, bias, out=out, epi=ops.EPI_GATE_RES, gate=_chunk(segs[0][1], ig, D), res=res,
+                        nan_to_num=nan_to_num)
+    out = _out(res, out)
+    for sl, m in segs:
+        ops.gemm([a[:, sl] for a in a_list], w_list, bias, out=out[:, sl], epi=ops.EPI_GATE_RES, gate=_chunk(m, ig, D),
+                 res=res[:, sl], nan_to_num=nan_to_num)
+    return out
+
+
+def _linear_lora_gate_res(x, w, b, pack, drop, segs, ig: int, res, out, nan_to_num=False):
+    """_linear_lora_fwd with the GATE_RES epilogue over segments: the LoRA down-projection (and its dropout mask) spans
+    the whole stream, the base GEMM runs per segment.  Returns T or None."""
+    if len(segs) == 1:
+        return _linear_lora_fwd(x, w, b, pack, drop, out=out, epi=ops.EPI_GATE_RES, gate=_chunk(segs[0][1], ig, res.shape[2]),
+                                res=res, nan_to_num=nan_to_num)[1]
+    if pack is None or isinstance(pack, LokrPack):
+        _gemm_gate_res([x], [w], b, segs, ig, res, out, nan_to_num)
+        return None
+    t = _lora_down(x, pack, drop)
+    _gemm_gate_res([x, t], [w, pack.b_ext], b, segs, ig, res, out, nan_to_num)
+    return t
+
+
 class LoraLinearFn(torch.autograd.Function):
     """y = x W^T + b + scaling * B A dropout(x) for an adapted Linear outside the block schedules (x_embedder,
     flux_lora_target = "all+ffs+embedder", reference flux/model.py:1320-1338).  x carries no gradient (model input)."""
@@ -399,6 +481,7 @@ class DoubleBlockFn(torch.autograd.Function):
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
         n_lora_in = len(lora)
         lora = list(lora) + [None] * (32 - len(lora))
+        segs = {"txt": _segments(mod_txt, None, S_txt), "img": _segments(mod_img, st.get("img_segs"), S - S_txt)}
         streams = (("txt", slice(0, S_txt), mod_txt, 8), ("img", slice(S_txt, S), mod_img, 0))
         mlp_base = {"img": 24, "txt": 28}
 
@@ -412,10 +495,8 @@ class DoubleBlockFn(torch.autograd.Function):
                 ps.append(None if a is None else (a, b))
             return make_pack(ps, n_out, k_in, scaling, dev, [lsc(base + 2 * m) for m in range(n_members)])
 
-        def mod_shift_scale(name, mod):
-            if name == "txt" and pre_only:
-                return mod[:, D:2 * D], mod[:, 0:D]
-            return mod[:, 0:D], mod[:, D:2 * D]
+        def mod_shift_scale(name):      # chunk indices of (shift, scale)
+            return (1, 0) if name == "txt" and pre_only else (0, 1)
 
         packs = {}
         qkv = torch.empty((B, S, 3 * D), device=dev, dtype=torch.bfloat16)
@@ -426,8 +507,7 @@ class DoubleBlockFn(torch.autograd.Function):
             ap: AttnPlan = plans[name + "_attn"]
             packs[name + "_qkv"] = lp(base, 3, D, D)
             packs[name + "_out"] = lp(base + 6, 1, D, D) if ap.w_out is not None else None
-            sh, sc = mod_shift_scale(name, mod)
-            nh = ops.ln_modulate_fwd(h[:, sl], sh, sc, EPS, out=nh_joint[:, sl] if keep_nh else None)
+            nh = _lnm_fwd(h[:, sl], segs[name], *mod_shift_scale(name), out=nh_joint[:, sl] if keep_nh else None)
             _, t = _linear_lora_fwd(nh, ap.w_qkv, ap.b_qkv, packs[name + "_qkv"], dr(base), out=qkv[:, sl])
             small[name + "_t_qkv"] = t
         ia: AttnPlan = plans["img_attn"]
@@ -448,9 +528,8 @@ class DoubleBlockFn(torch.autograd.Function):
                 h2[:, sl].copy_(h[:, sl])
                 small[name + "_t_out"] = None
                 continue
-            _, t = _linear_lora_fwd(o[:, sl], ap.w_out, ap.b_out, packs[name + "_out"], dr(base + 6), out=h1[:, sl],
-                                    epi=ops.EPI_GATE_RES, gate=mod[:, 2 * D:3 * D], res=h[:, sl])
-            small[name + "_t_out"] = t
+            small[name + "_t_out"] = _linear_lora_gate_res(o[:, sl], ap.w_out, ap.b_out, packs[name + "_out"], dr(base + 6),
+                                                           segs[name], 2, res=h[:, sl], out=h1[:, sl])
         qkv2 = o2 = lse2 = None
         if dual:
             isl = slice(S_txt, S)
@@ -475,7 +554,7 @@ class DoubleBlockFn(torch.autograd.Function):
                 mlp_pre[name] = None
                 continue
             mp: MlpPlan = plans[name + "_mlp"]
-            nh2 = ops.ln_modulate_fwd(h1[:, sl], mod[:, 3 * D:4 * D], mod[:, 4 * D:5 * D], EPS)
+            nh2 = _lnm_fwd(h1[:, sl], segs[name], 3, 4)
             pre = torch.empty((B, sl.stop - sl.start, 4 * D), device=dev, dtype=torch.bfloat16)
             mb = mlp_base[name]
             pk1 = packs[name + "_fc1"] = _pack1(lora[mb], lora[mb + 1], 4 * D, D, scaling, dev, lsc(mb))
@@ -483,9 +562,8 @@ class DoubleBlockFn(torch.autograd.Function):
             act, t = _linear_lora_fwd(nh2, mp.w1, mp.b1, pk1, dr(base + 3), epi=ops.EPI_GELU, aux=pre)
             small[name + "_t_fc1"] = t
             del nh2
-            _, t = _linear_lora_fwd(act, mp.w2, mp.b2, pk2, dr(base + 4), out=h2[:, sl], epi=ops.EPI_GATE_RES,
-                                    gate=mod[:, 5 * D:6 * D], res=h1[:, sl], nan_to_num=(name == "txt" and nan_txt))
-            small[name + "_t_fc2"] = t
+            small[name + "_t_fc2"] = _linear_lora_gate_res(act, mp.w2, mp.b2, pk2, dr(base + 4), segs[name], 5, res=h1[:, sl],
+                                                           out=h2[:, sl], nan_to_num=(name == "txt" and nan_txt))
             del act
             mlp_pre[name] = pre
         ctx.st = st
@@ -519,6 +597,7 @@ class DoubleBlockFn(torch.autograd.Function):
         drop: Optional[LoraDrop] = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
         dh2 = dh2.contiguous()
+        segs = {"txt": _segments(mod_txt, None, S_txt), "img": _segments(mod_img, st.get("img_segs"), S - S_txt)}
         streams = (("txt", slice(0, S_txt), mod_txt, 8, pre_txt, t_qkv_txt, t_out_txt),
                    ("img", slice(S_txt, S), mod_img, 0, pre_img, t_qkv_img, t_out_img))
         mlp_t = {"txt": (28, t_fc1_txt, t_fc2_txt), "img": (24, t_fc1_img, t_fc2_img)}
@@ -533,7 +612,7 @@ class DoubleBlockFn(torch.autograd.Function):
                 continue
             mp: MlpPlan = plans[name + "_mlp"]
             # ---- MLP branch: h2 = h1 + gate_mlp * fc2(gelu(fc1(LNmod(h1))))
-            g2 = ops.gate_mul(dh2[:, sl], mod[:, 5 * D:6 * D])
+            g2 = _gate_mul(dh2[:, sl], segs[name], 5)
             mb, t_fc1, t_fc2 = mlp_t[name]
             pk1, pk2 = packs.get(name + "_fc1"), packs.get(name + "_fc2")
             d_pre, t_up = _dgrad_through_gelu(g2, mp.w2_t, pk2, dr(base + 4), pre)
@@ -544,14 +623,14 @@ class DoubleBlockFn(torch.autograd.Function):
             del g2
             d_nh2, t_up = _linear_lora_dgrad(d_pre, mp.w1_t, pk1, dr(base + 3))
             if pk1 is not None:
-                nh2 = ops.ln_modulate_fwd(h1[:, sl], mod[:, 3 * D:4 * D], mod[:, 4 * D:5 * D], EPS)
+                nh2 = _lnm_fwd(h1[:, sl], segs[name], 3, 4)
                 (grads[mb], grads[mb + 1]), = _lora_grads(pk1, nh2, t_fc1, d_pre, t_up, dr(base + 3))
                 del nh2
             del d_pre
-            ops.ln_modulate_bwd(d_nh2, h1[:, sl], mod[:, 4 * D:5 * D], add=dh2[:, sl], eps=EPS, out=dh1[:, sl])
+            _lnm_bwd(d_nh2, h1[:, sl], segs[name], 4, add=dh2[:, sl], out=dh1[:, sl])
             del d_nh2
             # ---- attention output projection: h1 = h + gate_msa * to_out(o)
-            g1 = ops.gate_mul(dh1[:, sl], mod[:, 2 * D:3 * D])
+            g1 = _gate_mul(dh1[:, sl], segs[name], 2)
             pk = packs[name + "_out"]
             _, t_up = _linear_lora_dgrad(g1, ap.w_out_t, pk, dr(base + 6), out=d_o[:, sl])
             if pk is not None:
@@ -588,17 +667,14 @@ class DoubleBlockFn(torch.autograd.Function):
         for name, sl, mod, base, pre, t_qkv, t_out in streams:
             ap = plans[name + "_attn"]
             pk = packs[name + "_qkv"]
-            if name == "txt" and pre_only:
-                sh_, sc_ = mod[:, D:2 * D], mod[:, 0:D]
-            else:
-                sh_, sc_ = mod[:, 0:D], mod[:, D:2 * D]
+            ish, isc = (1, 0) if name == "txt" and pre_only else (0, 1)
             d_nh, t_up = _linear_lora_dgrad(d_qkv[:, sl], ap.w_qkv_t, pk, dr(base))
             if pk is not None:
-                nh = nh_saved[:, sl] if nh_saved.numel() else ops.ln_modulate_fwd(h[:, sl], sh_, sc_, EPS)
+                nh = nh_saved[:, sl] if nh_saved.numel() else _lnm_fwd(h[:, sl], segs[name], ish, isc)
                 for m, (da, db) in enumerate(_lora_grads(pk, nh, t_qkv, d_qkv[:, sl], t_up, dr(base))):
                     grads[base + 2 * m], grads[base + 2 * m + 1] = da, db
                 del nh
-            ops.ln_modulate_bwd(d_nh, h[:, sl], sc_, add=dh1[:, sl], eps=EPS, out=dh[:, sl])
+            _lnm_bwd(d_nh, h[:, sl], segs[name], isc, add=dh1[:, sl], out=dh[:, sl])
             del d_nh
         if dual:
             isl = slice(S_txt, S)
@@ -641,7 +717,8 @@ class SingleBlockFn(torch.autograd.Function):
             raise NotImplementedError("LoKr on the single blocks' proj_out is not part of the LyCORIS presets supported here")
         drop: Optional[LoraDrop] = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
-        nh = ops.ln_modulate_fwd(h, mod[:, 0:D], mod[:, D:2 * D], EPS)
+        segs = _segments(mod, st.get("segs"), S)
+        nh = _lnm_fwd(h, segs, 0, 1)
         qkv, t_qkv = _linear_lora_fwd(nh, ap.w_qkv, ap.b_qkv, pk, drop)
         q, k = ops.qk_rmsnorm_rope_fwd(qkv, D, H, hd, ap.norm_q, ap.norm_k, None, None, 0, cos, sin, EPS)
         v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
@@ -656,15 +733,14 @@ class SingleBlockFn(torch.autograd.Function):
         # proj_out(cat[attn, mlp]) as two K-segments of one GEMM; gate, residual, nan_to_num in the epilogue
         t_out = None
         if pk_out is None:
-            h_out = ops.gemm([o, act], [mp.w2[:, :D], mp.w2[:, D:]], mp.b2, epi=ops.EPI_GATE_RES,
-                             gate=mod[:, 2 * D:3 * D], res=h, nan_to_num=True)
+            h_out = _gemm_gate_res([o, act], [mp.w2[:, :D], mp.w2[:, D:]], mp.b2, segs, 2, res=h, nan_to_num=True)
         else:
             if drop is None:
                 t_out = ops.gemm([o, act], [pk_out.a_stack[:, :D], pk_out.a_stack[:, D:]])
             else:                       # one mask over the logical [B, S, 5D] input of the adapted Linear
                 t_out = _lora_down(torch.cat([o, act], 2), pk_out, dr(4))
-            h_out = ops.gemm([o, act, t_out], [mp.w2[:, :D], mp.w2[:, D:], pk_out.b_ext], mp.b2, epi=ops.EPI_GATE_RES,
-                             gate=mod[:, 2 * D:3 * D], res=h, nan_to_num=True)
+            h_out = _gemm_gate_res([o, act, t_out], [mp.w2[:, :D], mp.w2[:, D:], pk_out.b_ext], mp.b2, segs, 2, res=h,
+                                   nan_to_num=True)
         del act
         ctx.st = st
         ctx.packs = (pk, pk_mlp, pk_out)
@@ -690,7 +766,8 @@ class SingleBlockFn(torch.autograd.Function):
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
         dh_out = dh_out.contiguous()
         grads: List[Optional[torch.Tensor]] = [None] * 10
-        g = ops.gate_mul(dh_out, mod[:, 2 * D:3 * D])
+        segs = _segments(mod, st.get("segs"), S)
+        g = _gate_mul(dh_out, segs, 2)
         if pk_out is None:
             d_o = ops.gemm([g], [mp.w2_t[:D]], None)
             d_pre = ops.gemm([g], [mp.w2_t[D:]], None, epi=ops.EPI_MUL_DGELU, aux=pre)
@@ -733,7 +810,7 @@ class SingleBlockFn(torch.autograd.Function):
         else:                           # the GEMM takes three K-segments: both rank blocks travel as one
             d_nh = ops.gemm([d_pre, d_qkv, torch.cat(t_ups, 2)], [mp.w1_t, ap.w_qkv_t, torch.cat(a_ts, 1)], None)
         if pk is not None or pk_mlp is not None:
-            nh = nh_saved if nh_saved.numel() else ops.ln_modulate_fwd(h, mod[:, 0:D], mod[:, D:2 * D], EPS)
+            nh = nh_saved if nh_saved.numel() else _lnm_fwd(h, segs, 0, 1)
             if pk is not None:
                 for m, (da, db) in enumerate(_lora_grads(pk, nh, t_qkv, d_qkv, t_up_qkv, drop)):
                     grads[2 * m], grads[2 * m + 1] = da, db
@@ -741,7 +818,7 @@ class SingleBlockFn(torch.autograd.Function):
                 (grads[6], grads[7]), = _lora_grads(pk_mlp, nh, t_mlp, d_pre, t_up_mlp, dr(3))
             del nh
         del d_pre, d_qkv
-        dh = ops.ln_modulate_bwd(d_nh, h, mod[:, D:2 * D], add=dh_out, eps=EPS)
+        dh = _lnm_bwd(d_nh, h, segs, 1, add=dh_out)
         out = [grads[i] if ctx.lora_present[i] else None for i in range(ctx.n_lora_in)]
         return (dh, None, None, None, None, *out)
 
@@ -753,10 +830,11 @@ class TailFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h, mod, st, *lora):
         """h [B, S, D] joint buffer; mod [B, 2D] = (scale | shift) (AdaLayerNormContinuous chunk order).  lora: the final
-        proj_out's (A, B) — PEFT's suffix rule makes the "proj_out" target of "all+ffs" select it too."""
+        proj_out's (A, B) — PEFT's suffix rule makes the "proj_out" target of "all+ffs" select it too.  Rows
+        [S_txt, S_end) are projected (S_end: the end of the Kontext scene tokens, default S)."""
         D = h.shape[2]
-        S_txt = st["S_txt"]
-        x = h[:, S_txt:]
+        S_txt, S_end = st["S_txt"], st.get("S_end") or h.shape[1]
+        x = h[:, S_txt:S_end]
         nx = ops.ln_modulate_fwd(x, mod[:, D:2 * D], mod[:, 0:D], EPS)
         a, b = (lora[0], lora[1]) if len(lora) >= 2 else (None, None)
         pk = _pack1(a, b, st["w_proj"].shape[0], D, st.get("lora_scaling", 1.0), h.device)
@@ -770,15 +848,15 @@ class TailFn(torch.autograd.Function):
         h, mod, t = ctx.saved_tensors
         st, pk = ctx.st, ctx.pack
         D = h.shape[2]
-        S_txt = st["S_txt"]
+        S_txt, S_end = st["S_txt"], st.get("S_end") or h.shape[1]
         d_out = d_out.contiguous()
         d_nx, t_up = _linear_lora_dgrad(d_out, st["w_proj_t"], pk, st.get("lora_drop"))
         lg = [None] * ctx.n_lora_in
         if pk is not None:
-            nx = ops.ln_modulate_fwd(h[:, S_txt:], mod[:, D:2 * D], mod[:, 0:D], EPS)
+            nx = ops.ln_modulate_fwd(h[:, S_txt:S_end], mod[:, D:2 * D], mod[:, 0:D], EPS)
             (lg[0], lg[1]), = _lora_grads(pk, nx, t, d_out, t_up, st.get("lora_drop"))
-        dh = torch.zeros_like(h) if S_txt > 0 else torch.empty_like(h)
-        ops.ln_modulate_bwd(d_nx, h[:, S_txt:], mod[:, 0:D], add=None, eps=EPS, out=dh[:, S_txt:])
+        dh = torch.zeros_like(h) if S_txt > 0 or S_end < h.shape[1] else torch.empty_like(h)
+        ops.ln_modulate_bwd(d_nx, h[:, S_txt:S_end], mod[:, 0:D], add=None, eps=EPS, out=dh[:, S_txt:S_end])
         return (dh, None, None, *lg)
 
 

@@ -127,6 +127,12 @@ class Flux:
             raise NotImplementedError(f"flux_lora_target={tgt!r} is not supported by the libstb200 path "
                                       f"(supported: {sorted(FLUX_LORA_TARGETS)})")
         check_masked_training(c)
+        if is_kontext(c):
+            lt = str(g("loss_type", "l2"))
+            if lt in ("huber", "smooth_l1") and g("huber_schedule", "constant") != "constant":
+                # the reference feeds Kontext's 2-D timesteps [B, S_scene + S_c] to compute_scheduled_huber_c
+                raise NotImplementedError(f"Kontext with loss_type={lt!r} and huber_schedule={g('huber_schedule')!r} is not "
+                                          "supported by the libstb200 path (l2 or a constant huber_c run)")
         if g("tread_config", None):
             raise NotImplementedError("TREAD routing is not supported by the libstb200 path")
         if g("flow_cubic_schedule", None) or g("flow_cubic_schedule_weights", None):
@@ -145,14 +151,20 @@ class Flux:
     def _check_supported(self, batch: Dict[str, Any]) -> None:
         """Options of the reference wrapper this path does not implement must RAISE, never be ignored, so that a shim can
         route such a config to the reference class (INTEGRATION.md 2): masked training outside `check_masked_training`'s
-        rule or without the batch's `encoder_attention_mask` (flux/model.py:813-822), Kontext conditioning latents
-        (flux/model.py:757-786)."""
+        rule or without the batch's `encoder_attention_mask` (flux/model.py:813-822), conditioning latents outside the
+        Kontext flavour, and pre-packed Kontext inputs that `prepare_batch` did not build (flux/model.py:757-786)."""
         if check_masked_training(self.config) and batch.get("encoder_attention_mask") is None:
             raise NotImplementedError("flux_attention_masked_training: the batch has no encoder_attention_mask (the text-embed "
                                       "cache must carry attention_masks)")
+        kontext = is_kontext(self.config)
         for k in ("conditioning_packed_latents", "conditioning_ids", "conditioning_latents"):
-            if batch.get(k) is not None:
-                raise NotImplementedError(f"Kontext / conditioning input `{k}` is not supported by the libstb200 Flux path")
+            if batch.get(k) is None or (kontext and k == "conditioning_latents"):
+                continue
+            if kontext:
+                raise NotImplementedError(f"Kontext input `{k}` without `conditioning_latents`: the libstb200 Flux path "
+                                          "packs the reference latents itself")
+            raise NotImplementedError(f"Kontext / conditioning input `{k}` is not supported by the libstb200 Flux path "
+                                      "outside model_flavour='kontext'")
 
     def _check_loss_supported(self, prepared_batch: Dict[str, Any], apply_conditioning_mask: bool) -> None:
         """common.py:6400-6424: with `apply_conditioning_mask` the reference multiplies the loss by the conditioning mask
@@ -206,12 +218,68 @@ class Flux:
             interp = sigmas if gamma == 0.0 else sigmas + slow * gamma * (1.0 - sigmas)
             batch["mixflow_slowdown_factors"] = slow
             batch["mixflow_interpolation_sigmas"] = interp
-        # fused: noisy = (1 - s) x + s eps  AND  2x2 patchify  (common.py:4975-4992, flux/__init__.py:25-30)
-        noisy, packed = ops.flow_prep_pack(batch["latents"], batch["input_noise"], interp.float().contiguous(),
-                                           want_unpacked=True)
+        cond = self._kontext_conditions(batch, state) if is_kontext(c) else None
+        if cond is None:
+            # fused: noisy = (1 - s) x + s eps  AND  2x2 patchify  (common.py:4975-4992, flux/__init__.py:25-30)
+            noisy, packed = ops.flow_prep_pack(batch["latents"], batch["input_noise"], interp.float().contiguous(),
+                                               want_unpacked=True)
+            batch["noisy_latents"] = noisy
+            batch["_packed_noisy_latents"] = packed
+            return batch
+        # Kontext: the x_embedder input [B, S_scene + S_c, 64] is filled in place, the noisy scene tokens first and then each
+        # reference image's packed tokens (flux/model.py:767-779 concatenates them), with no cat / permute copies
+        conds, ids = cond
+        Hh, Ww = batch["latents"].shape[2:]
+        S_scene = (Hh // 2) * (Ww // 2)
+        S_c = ids.shape[0]
+        joint = torch.empty((bsz, S_scene + S_c, 4 * batch["latents"].shape[1]), device=dev, dtype=torch.bfloat16)
+        noisy, _ = ops.flow_prep_pack(batch["latents"], batch["input_noise"], interp.float().contiguous(), want_unpacked=True,
+                                      out=joint[:, :S_scene])
+        off = S_scene
+        for lat in conds:
+            n = (lat.shape[2] // 2) * (lat.shape[3] // 2)
+            ops.flow_prep_pack(lat, None, None, out=joint[:, off:off + n])
+            off += n
         batch["noisy_latents"] = noisy
-        batch["_packed_noisy_latents"] = packed
+        batch["_packed_noisy_latents"] = joint
+        batch["_kontext_ids"] = ids
+        batch["conditioning_packed_latents"] = joint[:, S_scene:]
+        batch["conditioning_ids"] = ids.to(dev, torch.bfloat16)[None].expand(bsz, -1, -1)   # the reference's dtype
         return batch
+
+    def _kontext_conditions(self, batch: Dict[str, Any], state: Dict[str, Any]):
+        """Flux.prepare_batch_conditions (flux/model.py:522-555) then the base class's list collapse (common.py:4668-4683).
+        Returns None (plain step) or (the conditioning latents on the device, bf16 contiguous [B, 16, h, w] each, in
+        sequence order; their ids [S_c, 3] built on the host from the shapes)."""
+        cond = batch.get("conditioning_latents")
+        if cond is None:
+            return None
+        args = state.get("args", {}) if isinstance(state, dict) else {}
+        mode = args.get("conditioning_multidataset_sampling", "random") if isinstance(args, dict) else \
+            getattr(args, "conditioning_multidataset_sampling", "random")
+        if mode == "random" and isinstance(cond, list) and len(cond) >= 1:
+            cond = cond[0]
+        conds = list(cond) if isinstance(cond, list) else [cond]
+        B, C = batch["latents"].shape[:2]
+        dev = self.accelerator.device
+        out = []
+        for lat in conds:
+            if lat.dim() == 3 and lat.shape[0] == C:          # (C, H, W): one image without a batch dimension
+                lat = lat.unsqueeze(0)
+            if lat.dim() != 4 or lat.shape[1] != C or lat.shape[0] != B or lat.shape[2] % 2 or lat.shape[3] % 2:
+                raise ValueError(f"conditioning latents must be [{B}, {C}, h, w] with even h, w; got {tuple(lat.shape)}")
+            out.append(lat.to(device=dev, dtype=torch.bfloat16, non_blocking=True).contiguous())
+        ids = kontext_ids([tuple(t.shape[2:]) for t in out])
+        cl = batch.get("conditioning_latents")
+        if isinstance(cl, list) and len(cl) > 0:              # common.py:4672-4683
+            types = batch.get("conditioning_latents_type")
+            sel = 0
+            if batch.get("conditioning_type") == "reference_strict" and isinstance(types, list) and "reference_strict" in types:
+                sel = types.index("reference_strict")
+            batch["conditioning_latents"] = cl[sel]
+            if isinstance(types, list) and sel < len(types):
+                batch["conditioning_latents_type"] = types[sel]
+        return out, ids
 
     # ------------------------------------------------------------------------------------------
     def _guidance(self, bsz: int, device) -> Optional[torch.Tensor]:
@@ -242,7 +310,16 @@ class Flux:
         img_ids = prepare_latent_image_ids(Hh, Ww)
         txt_ids = torch.zeros(pb["encoder_hidden_states"].shape[1], 3)
         # side effect kept from the reference: timesteps are overwritten with t / 1000 (flux/model.py:739-745)
-        pb["timesteps"] = pb["timesteps"].to(device=dev, dtype=torch.float32) / self.noise_schedule.config.num_train_timesteps
+        t = pb["timesteps"] = pb["timesteps"].to(device=dev, dtype=torch.float32) / self.noise_schedule.config.num_train_timesteps
+        cond_ids = pb.get("_kontext_ids")
+        S_c = 0 if cond_ids is None else cond_ids.shape[0]
+        if S_c:
+            if t.dim() != 1:
+                raise NotImplementedError("Kontext with token-wise timesteps is not supported by the libstb200 Flux path")
+            # _extend_conditioning_timesteps (flux/model.py:602-618): later readers of the batch see [B, S_scene + S_c]
+            pb["timesteps"] = torch.cat([t[:, None].expand(-1, img_ids.shape[0]),
+                                         torch.zeros(B, S_c, device=dev, dtype=torch.float32)], dim=1)
+            img_ids = torch.cat([img_ids, cond_ids], dim=0)
         attention_mask = None
         if getattr(self.config, "flux_attention_masked_training", False):   # flux/model.py:813-822
             attention_mask = pb.get("encoder_attention_mask")
@@ -252,9 +329,10 @@ class Flux:
             if attention_mask.dim() == 3 and attention_mask.size(1) == 1:
                 attention_mask = attention_mask.squeeze(1)   # [B, 1, S] -> [B, S]
         out = self.model(
-            hidden_states=packed, timestep=pb["timesteps"], guidance=self._guidance(B, dev),
+            hidden_states=packed, timestep=t, guidance=self._guidance(B, dev),
             pooled_projections=pb["added_cond_kwargs"]["text_embeds"], encoder_hidden_states=pb["encoder_hidden_states"],
             txt_ids=txt_ids, img_ids=img_ids, joint_attention_kwargs=None, return_dict=False, attention_mask=attention_mask,
+            **({"conditioning_tokens": S_c} if S_c else {}),
         )[0]
         return self._prediction_dict(out, (B, Cc, Hh, Ww))
 
@@ -316,10 +394,40 @@ class Flux:
         # NB: Flux.model_predict has overwritten `timesteps` with t / 1000 (flux/model.py:739-745) before loss() runs; the
         # reference feeds those scaled values to compute_scheduled_huber_c as they are, and so does this mirror.
         t = prepared_batch["timesteps"]
+        if t.dim() == 2:        # Kontext [B, S_scene + S_c]: validate_config allows only the constant c here
+            t = t[:, 0]
         return lt, compute_scheduled_huber_c(c, self.noise_schedule, t.to(self.accelerator.device), self.PREDICTION_TYPE)
 
     def loss_with_logs(self, prepared_batch, model_output, apply_conditioning_mask: bool = True):
         return self.loss(prepared_batch, model_output, apply_conditioning_mask), None
+
+
+def is_kontext(c) -> bool:
+    """model_flavour "kontext" (flux/model.py:94, black-forest-labs/flux.1-kontext-dev)."""
+    return getattr(c, "model_flavour", None) == "kontext"
+
+
+def kontext_ids(sizes) -> torch.Tensor:
+    """Position ids [S_c, 3] of the Kontext conditioning tokens for latents of the (h, w) `sizes`, in sequence order:
+    build_kontext_inputs (flux/__init__.py:64-172) on the host from shapes alone.  (1, y, x) over each (h/2, w/2) patch
+    grid, offset by the ComfyUI scheme (x0 / y0: the next image goes right of or below what is placed, whichever keeps
+    max(x, y) smaller), then rounded through bf16 as the reference's `.to(weight_dtype)` does (so positions above 256
+    lose their low bits), returned as float32 like the reference's cat with the fp32 scene ids."""
+    x0 = y0 = 0
+    out = []
+    for H, W in sizes:
+        x = y = 0
+        if H + y0 > W + x0:
+            x = x0
+        else:
+            y = y0
+        iy = torch.arange(H // 2) + y // 2
+        ix = torch.arange(W // 2) + x // 2
+        grid = torch.stack(torch.meshgrid(iy, ix, indexing="ij"), dim=-1).reshape(-1, 2)
+        out.append(torch.cat([torch.ones_like(grid[:, :1]), grid], dim=1))
+        x0 = max(x0, W + x)
+        y0 = max(y0, H + y)
+    return torch.cat(out, 0).to(torch.bfloat16).to(torch.float32)
 
 
 def check_masked_training(c) -> bool:

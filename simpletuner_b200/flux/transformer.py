@@ -275,12 +275,18 @@ class FluxTransformerBlock(nn.Module):
                 if any(l.lokr is not None for l in lins):
                     self._plans.pop(key, None)
 
-    def forward(self, h, silu_temb, cos, sin, S_txt, lora_scaling, key_bias=None):
-        D = self.dim
-        mod_img = self.norm1.linear(silu_temb)
-        mod_txt = self.norm1_context.linear(silu_temb)
+    def forward(self, h, silu_temb, cos, sin, S_txt, lora_scaling, key_bias=None, segs=None):
+        """segs (Flux Kontext): (scene, conditioning) token counts of the image stream; silu_temb then stacks the
+        [text | scene | conditioning] rows [3B, D] (FluxTransformer2DModel.forward)."""
+        if segs is None:
+            mod_img = self.norm1.linear(silu_temb)
+            mod_txt = self.norm1_context.linear(silu_temb)
+        else:
+            B = silu_temb.shape[0] // 3
+            mod_img = self.norm1.linear(silu_temb[B:])            # [2B, 6D]: scene rows, conditioning rows
+            mod_txt = self.norm1_context.linear(silu_temb[:B])
         st = {"S_txt": S_txt, "H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias}
+              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias, "img_segs": segs}
         a = self.attn
         attn_l = [a.to_q, a.to_k, a.to_v, a.to_out[0], a.add_q_proj, a.add_k_proj, a.add_v_proj, a.to_add_out]
         mlp_l = [self.ff.net[0].proj, self.ff.net[2], self.ff_context.net[0].proj, self.ff_context.net[2]]
@@ -321,10 +327,11 @@ class FluxSingleTransformerBlock(nn.Module):
         if self._plans and any(l.lokr is not None for l in (a.to_q, a.to_k, a.to_v)):
             self._plans.pop("attn", None)
 
-    def forward(self, h, silu_temb, cos, sin, lora_scaling, key_bias=None):
+    def forward(self, h, silu_temb, cos, sin, lora_scaling, key_bias=None, segs=None):
+        """segs (Flux Kontext): (text, scene, conditioning) token counts; silu_temb then holds those rows [3B, D]."""
         mod = self.norm.linear(silu_temb)
         st = {"H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias}
+              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias, "segs": segs}
         a = self.attn
         lora = _lora_list([a.to_q, a.to_k, a.to_v])
         st["lokr_scales"] = _lokr_scales([a.to_q, a.to_k, a.to_v])
@@ -638,7 +645,12 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
                 joint_attention_kwargs: Optional[Dict[str, Any]] = None, controlnet_block_samples=None,
                 controlnet_single_block_samples=None, return_dict: bool = True, attention_mask=None,
                 controlnet_blocks_repeat: bool = False, force_keep_mask=None, hidden_states_buffer=None,
-                grounding_kwargs=None):
+                grounding_kwargs=None, conditioning_tokens: int = 0):
+        """conditioning_tokens (Flux Kontext): the last `conditioning_tokens` rows of `hidden_states` / `img_ids` are
+        reference-image tokens.  They are conditioned at timestep 0 while `timestep` [B] conditions the scene tokens, as the
+        reference does with its 2-D timesteps (flux/model.py:602-618, flux/transformer.py:245-294, 1068-1085), and the
+        output holds the scene tokens only ([B, S_img - conditioning_tokens, C]; the reference slices them off in
+        model_predict, flux/model.py:846-848)."""
         for nm, v in (("timestep_sign", timestep_sign), ("r_timestep", r_timestep),
                       ("controlnet_block_samples", controlnet_block_samples),
                       ("controlnet_single_block_samples", controlnet_single_block_samples),
@@ -646,13 +658,18 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
             if v is not None:
                 raise NotImplementedError(f"libstb200 Flux path does not support `{nm}`; use the reference module")
         if timestep.ndim != 1:
-            raise NotImplementedError("token-wise timesteps are not supported by the libstb200 Flux path")
+            raise NotImplementedError("token-wise timesteps are not supported by the libstb200 Flux path (Kontext passes "
+                                      "per-sample timesteps and `conditioning_tokens`)")
         if not hidden_states.is_cuda:
             from .._lib import StbError
             raise StbError("FluxTransformer2DModel (libstb200) needs CUDA tensors; there is no CPU fallback")
         dt = self.x_embedder.weight.dtype
         B, S_img, _ = hidden_states.shape
         S_txt = encoder_hidden_states.shape[1]
+        S_c = int(conditioning_tokens or 0)
+        if not 0 <= S_c < S_img:
+            raise ValueError(f"conditioning_tokens must be in [0, {S_img}), got {S_c}")
+        S_scene = S_img - S_c
         D = self.inner_dim
         dev = hidden_states.device
         # joint hidden buffer: [text | image]
@@ -675,8 +692,19 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         g = guidance.to(device=dev, dtype=torch.float32) * 1000 if guidance is not None else None
         if self.config.guidance_embeds and g is None:
             raise ValueError("guidance is required when guidance_embeds=True")
-        temb = self._temb(t, g, pooled_projections.to(dt))
-        silu_temb = F.silu(temb).contiguous()
+        pooled = pooled_projections.to(dt)
+        if S_c == 0:
+            temb = self._temb(t, g, pooled)
+            silu_temb = F.silu(temb).contiguous()
+        else:
+            # _flux_tokenwise_conditioning has two distinct rows per sample, temb(t) over the scene tokens and temb(0) over
+            # the conditioning tokens (same guidance and pooled projection): one pass over 2B rows.  The text stream's
+            # temb.mean(dim=1) over all image tokens is the fp32 mean of those rows with their token counts, rounded once
+            # to bf16 as the reference's bf16 mean is; [B, S, D] is never formed.
+            temb2 = self._temb(torch.cat([t, torch.zeros_like(t)]), None if g is None else torch.cat([g, g]),
+                               torch.cat([pooled, pooled]))
+            temb_txt = ((temb2[:B].float() * S_scene + temb2[B:].float() * S_c) / S_img).to(dt)
+            silu_temb = F.silu(torch.cat([temb_txt, temb2])).contiguous()     # [3B, D]: text, scene, conditioning rows
         if txt_ids.ndim == 3:
             txt_ids = txt_ids[0]
         if img_ids.ndim == 3:
@@ -686,17 +714,20 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         # masked training: one per-key bias for every attention of the step (an argument of each block, so the re-run
         # under gradient checkpointing sees it too)
         key_bias = None if attention_mask is None else flux_key_bias(attention_mask, B, S_txt + S_img, dt, dev)
+        # Kontext token segments: host ints, block arguments like key_bias
+        img_segs = (S_scene, S_c) if S_c else None
+        single_segs = (S_txt, S_scene, S_c) if S_c else None
         for i, blk in enumerate(self.transformer_blocks):
-            h = self._run_block(i, blk, h, silu_temb, cos, sin, S_txt, scaling, key_bias)
+            h = self._run_block(i, blk, h, silu_temb, cos, sin, S_txt, scaling, key_bias, img_segs)
         for i, blk in enumerate(self.single_transformer_blocks):
-            h = self._run_block(i, blk, h, silu_temb, cos, sin, scaling, key_bias)
+            h = self._run_block(i, blk, h, silu_temb, cos, sin, scaling, key_bias, single_segs)
         if self._tail_plan is None:
             self._tail_plan = {"w_proj": self.proj_out.weight.detach(), "b_proj": self.proj_out.bias.detach(),
                                "w_proj_t": _wt(self.proj_out.weight.detach())}
-        mod = self.norm_out.linear(silu_temb)
+        mod = self.norm_out.linear(silu_temb[B:2 * B] if S_c else silu_temb)     # norm_out uses temb_img: the scene rows
         pa, pb = self.proj_out.lora_tensors()
         tail_lora = () if pa is None else (pa, pb)
-        out = TailFn.apply(h, mod, {"S_txt": S_txt, "lora_scaling": scaling, "lora_drop": getattr(self.proj_out, "_lora_drop", None),
+        out = TailFn.apply(h, mod, {"S_txt": S_txt, "S_end": S_txt + S_scene, "lora_scaling": scaling, "lora_drop": getattr(self.proj_out, "_lora_drop", None),
                                     **self._tail_plan}, *tail_lora)
         if not return_dict:
             return (out,)

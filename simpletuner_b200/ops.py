@@ -293,16 +293,29 @@ def qk_rmsnorm_rope_bwd(dq, dk, src, k_off, H, HD, wq, wk, wq_added=None, wk_add
     return dsrc
 
 
-def flow_prep_pack(latents, noise, sigmas, want_unpacked: bool = True):
-    """Returns (noisy [B,C,H,W] or None, packed [B, H/2*W/2, 4C])."""
-    assert latents.is_contiguous() and noise.is_contiguous() and sigmas.dtype == torch.float32
-    _chk(latents, "latents"); _chk(noise, "noise")
+def flow_prep_pack(latents, noise, sigmas, want_unpacked: bool = True, out=None):
+    """Returns (noisy [B,C,H,W] or None, packed [B, H/2*W/2, 4C]).  out: a [B, H/2*W/2, 4C] view with dense tokens
+    (e.g. a token range of a longer joint sequence) that receives the packed tokens.  noise = sigmas = None: plain
+    pack_latents of `latents` (no noisy output)."""
+    assert latents.is_contiguous()
+    _chk(latents, "latents")
+    if noise is not None:
+        assert noise.is_contiguous() and sigmas.dtype == torch.float32
+        _chk(noise, "noise")
+    else:
+        assert sigmas is None
+        want_unpacked = False
     B, Cc, Hh, Ww = latents.shape
     noisy = torch.empty_like(latents) if want_unpacked else None
-    packed = torch.empty((B, (Hh // 2) * (Ww // 2), 4 * Cc), device=latents.device, dtype=torch.bfloat16)
-    check(_lib.lib().stb_flow_prep_pack(latents.data_ptr(), noise.data_ptr(), sigmas.contiguous().data_ptr(),
-                                        _ptr(noisy), packed.data_ptr(), B, Cc, Hh, Ww, _stream()))
-    return noisy, packed
+    shape = (B, (Hh // 2) * (Ww // 2), 4 * Cc)
+    if out is None:
+        out = torch.empty(shape, device=latents.device, dtype=torch.bfloat16)
+    _chk(out, "out")
+    if tuple(out.shape) != shape or out.stride(2) != 1 or out.stride(1) != 4 * Cc or out.dtype != torch.bfloat16:
+        raise ValueError(f"flow_prep_pack: out must be a bf16 {shape} view with dense tokens")
+    check(_lib.lib().stb_flow_prep_pack(latents.data_ptr(), _ptr(noise), _ptr(None if sigmas is None else sigmas.contiguous()),
+                                        _ptr(noisy), out.data_ptr(), out.stride(0), B, Cc, Hh, Ww, _stream()))
+    return noisy, out
 
 
 LOSS_TYPES = {"l2": 0, "huber": 1, "smooth_l1": 2}

@@ -215,6 +215,8 @@ class GraphedTrainStep:
         return ld
 
     def __call__(self, batch: Dict[str, Any]) -> torch.Tensor:
+        if any(batch.get(k) is not None for k in ("conditioning_latents", "conditioning_packed_latents")):
+            raise NotImplementedError("GraphedTrainStep: Flux Kontext batches (conditioning latents) run on the eager TrainStep")
         if not self.capture_prepare:          # eager prepare (host-side draws stay live); its output is the graph's input
             batch = self.step.model.prepare_batch(batch, self.step.state)
         key = tuple((k, tuple(v.shape), v.dtype) for k, v in sorted(batch.items()) if torch.is_tensor(v))
