@@ -21,8 +21,9 @@ def _rand(*shape, scale=1.0, seed=0):
 
 
 def _report(name, got, ref, atol, rtol, extra=None):
-    got = got.float()
-    ref = ref.float()
+    dt = torch.float64 if ref.dtype == torch.float64 else torch.float32   # an fp64 reference is compared in fp64
+    got = got.to(dt)
+    ref = ref.to(dt)
     err = (got - ref).abs()
     tol = atol + rtol * ref.abs()
     bad = err > tol
@@ -53,88 +54,342 @@ def _report(name, got, ref, atol, rtol, extra=None):
     return out
 
 
-# --------------------------------------------------------------------------------------------- GEMM
+# --------------------------------------------------------------------------------------------- GEMM-family reference model
+# The GEMM-family checks (gemm, wgrad_full, skinny_tn, conv3x3_nhwc, conv_in_3ch, colsum2) compare the kernel with an fp64
+# reference computed on the kernel's own bf16 inputs, element by element, in one of two input modes.
+#
+# Realistic inputs (exact=False): N(0, s^2) operands.  Per-element tolerance
+#     tol = rtol |ref| + GEMM_C 2^-24 sqrt(K) (|A| |W|^T)_ij
+# with K the whole contraction length (all segments of a gemm, the tokens of wgrad_full / skinny_tn / colsum2, 9 C_in of a
+# conv).  The second term is the usual scale of an fp32 dot product's rounding error; |A| |W|^T is one more fp64 product,
+# of the absolute values.  rtol is 2^-7 for bf16 outputs, not 2^-8: the bf16 store alone rounds by up to half an ulp =
+# 2^-8 |x|, which would use all of an rtol of 2^-8 (ATTN_TOL has the same reason).  fp32 outputs (skinny_tn, colsum2) have
+# rtol 2^-23, one fp32 ulp.  Epilogues that write the pre-activation (EPI_GELU / EPI_GATE_RES aux) have it checked with
+# this tolerance and the output checked as a function of it: GATE_RES bit for bit, GELU as one of the two bf16 neighbours
+# of fp64 gelu_tanh(aux).  The others propagate the tolerance: |derivative| x atol plus one bf16 ulp (2^-7 |x|) for each
+# rounding.  Each result reports tol_use (the worst element's share of its tolerance) and, where the accumulation term
+# applies directly, c_half: the smallest GEMM_C at which that check's tol_use would be 0.5.
+#   GEMM_C = 0.5, measured on H100 80GB HBM3 (SXM, 700 W limit): the largest c_half of any unmodified kernel was 0.143
+#   (gemm_pair_flux_shape; wgrad 0.104, conv 0.142, colsum2 0.108, skinny_tn 0.073; the largest tol_use 0.498), so every error of the wgmma
+#   accumulation stayed below 0.07 x 2^-24 sqrt(K) sum |a w| where it can be seen through an fp32 output.  This is a
+#   measured value, not a model of the tensor core's rounding.
+#
+# Exact inputs (exact=True): A / dy / L / pixel operands are integers in [-2, 2], W / x operands integers in [-6, 6] times
+# 2^-4 (_gen).  exact_bound_ok asserts on the host, from the drawn values, that every product is a multiple of 2^-4 and
+# sum_k |a_k w_k| < 2^19, so every partial sum in any order is a multiple of 2^-4 below 2^19: 23 significant bits, exact
+# in fp32 (and still exact if the tensor core aligned its addends to fewer bits than fp32, down to 2^-4; unmeasured).  The
+# fp64 accumulation then equals the kernel's fp32 accumulator whatever the tile, split or atomic order, and the epilogue
+# is replayed with fp32 torch ops: the output must be bit-identical.  Bias, gate, res and aux stay ordinary bf16 values.
+# GELU, QuickGELU and dGELU use tanhf / __expf: their output must be one of the two bf16 neighbours of the fp64 value.
+# alpha * acc + old (wgrad_full accumulate, the skinny_tn slab reduce) may be contracted into an FMA: power-of-two alphas
+# are bit-exact either way; a non-power-of-two case accepts either rounding.
+GEMM_C = 0.5
+GEMM_RTOL_BF16 = 2 ** -7
+GEMM_RTOL_F32 = 2 ** -23
+EXACT_BOUND = 2 ** 19
+_U = 2 ** -7          # one bf16 ulp relative to |x| (an upper bound)
+
+
 def gelu_tanh(x):
     return torch.nn.functional.gelu(x, approximate="tanh")
 
 
+def gelu64(x):
+    return 0.5 * x * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (x + 0.044715 * x ** 3)))
+
+
+def dgelu64(x):
+    k0, k1 = math.sqrt(2.0 / math.pi), 0.044715
+    t = torch.tanh(k0 * (x + k1 * x ** 3))
+    return 0.5 * (1.0 + t) + 0.5 * x * (1.0 - t * t) * k0 * (1.0 + 3.0 * k1 * x * x)
+
+
+def quick_gelu64(y):
+    return y * torch.sigmoid(1.702 * y)
+
+
+def dquick_gelu64(y):
+    s = torch.sigmoid(1.702 * y)
+    return s + 1.702 * y * s * (1.0 - s)
+
+
+def _gen(*shape, seed=0, scale=1.0, exact=None):
+    """A bf16 operand on the GPU.  exact None: N(0, scale^2) (_rand); "int": integers in [-2, 2] (A, dy, L, pixels);
+    "frac": integers in [-6, 6] x 2^-4 (W, x)."""
+    if exact is None:
+        return _rand(*shape, scale=scale, seed=seed)
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    hi = 2 if exact == "int" else 6
+    v = torch.randint(-hi, hi + 1, shape, generator=g).float()
+    return (v if exact == "int" else v / 16).to(torch.bfloat16).to(DEV)
+
+
+def exact_bound_ok(ints, fracs, mag):
+    """The exact-input bound from the drawn values: `ints` hold integers, `fracs` multiples of 2^-4, and every
+    mag = sum_k |a_k w_k| (fp64) is below 2^19, which bounds every partial sum of the dot product in any order."""
+    is_int = lambda t: bool((t.double() == t.double().round()).all())
+    return all(is_int(t) for t in ints) and all(is_int(t.double() * 16) for t in fracs) and float(mag.max()) < EXACT_BOUND
+
+
+def _is_pow2(x):
+    return x != 0 and math.frexp(abs(x))[0] == 0.5
+
+
+def _f32(x):
+    """x rounded to fp32, as a Python float (what a float kernel argument holds)."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def gate_res_replay(y, gate, res, nan_to_num=False):
+    """EPI_GATE_RES output from the bf16 linear output y [B, S, N]: res + bf16(gate * y) in fp32, rounded once; with
+    nan_to_num the rounded value maps NaN -> 0 and +-inf -> +-65504 (which is 65536 in bf16)."""
+    out = (res.float() + (gate.float()[:, None, :] * y.float()).bfloat16().float()).bfloat16()
+    if nan_to_num:
+        out = torch.nan_to_num(out, nan=0.0, posinf=65504.0, neginf=-65504.0)
+    return out
+
+
+def replay_epilogue(epi, acc, bias=None, gate=None, res=None, aux=None, nan_to_num=False):
+    """The fp32 epilogue of gemm.cuh on an exact fp32 accumulator acc [B, S, N].  Returns (out, pre), bf16, with
+    pre = bf16(acc + bias) (the aux output of EPI_GELU / EPI_GATE_RES) and out the bits the kernel writes for EPI_STORE,
+    EPI_ADD_RES, EPI_GATE_RES and EPI_MUL; None for the transcendental epilogues, which have no bit-exact replay."""
+    f = acc.float() if bias is None else acc.float() + bias.float()
+    pre = f.bfloat16()
+    out = None
+    if epi == ops.EPI_STORE:
+        out = pre
+    elif epi == ops.EPI_ADD_RES:
+        out = (f + res.float()).bfloat16()
+    elif epi == ops.EPI_GATE_RES:
+        out = gate_res_replay(pre, gate, res, nan_to_num)
+    elif epi == ops.EPI_MUL:
+        out = (pre.float() * aux.float()).bfloat16()
+    return out, pre
+
+
+def _bf16_steps(g):
+    """(next bf16 value below g, next above g) in fp64, for finite bf16 g."""
+    m = g.float().abs().contiguous().view(torch.int32)
+    up_mag = (m + (1 << 16)).view(torch.float32).double()
+    dn_mag = (m - (1 << 16)).clamp_min(0).view(torch.float32).double()
+    gf = g.float()
+    return torch.where(gf > 0, dn_mag, -up_mag), torch.where(gf < 0, -dn_mag, up_mag)
+
+
+def _first(mask, got, ref, out):
+    idx = torch.nonzero(mask)[:8]
+    out["first_bad"] = idx.tolist()
+    out["got"] = [float(got[tuple(i)]) for i in idx.tolist()]
+    out["want"] = [float(ref[tuple(i)]) for i in idx.tolist()]
+
+
+def _bits(name, got, ref):
+    """got and ref (both bf16 or both fp32) hold the same bits, NaN at the same places (payloads not compared)."""
+    iv = torch.int16 if got.dtype == torch.bfloat16 else torch.int32
+    both_nan = torch.isnan(got) & torch.isnan(ref)
+    diff = (got.contiguous().view(iv) != ref.contiguous().view(iv)) & ~both_nan
+    n = int(diff.sum().item())
+    out = {"name": name, "ok": n == 0, "n_diff": n, "numel": got.numel()}
+    if n:
+        _first(diff, got, ref, out)
+    return out
+
+
+def _neighbour(name, got, ref, atol=None):
+    """got (bf16) is one of the two bf16 neighbours of the fp64 ref: no bf16 value lies strictly between them.  atol: an
+    absolute error also accepted (the fp32 formula's own cancellation, see _gelu_atol)."""
+    dn, up = _bf16_steps(got)
+    near = (dn <= ref) & (ref <= up)
+    if atol is not None:
+        near = near | ((got.double() - ref).abs() <= atol)
+    bad = ~(near & torch.isfinite(got))
+    n = int(bad.sum().item())
+    out = {"name": name, "ok": n == 0, "n_bad": n, "numel": got.numel()}
+    if n:
+        _first(bad, got, ref, out)
+    return out
+
+
+def _gelu_atol(x):
+    """For x << 0 the fp32 formulas 0.5 x (1 + tanh u) and its derivative cancel: 1 + tanh u carries the rounding of tanh
+    near -1, about 2^-24, so gelu is off by ~2^-24 |x| absolutely (torch's own fp32 / bf16 GELU too) while its value is
+    tiny.  Allowed: 2^-22 |x| for gelu, 2^-21 (1 + |x| u') for its derivative."""
+    du = math.sqrt(2.0 / math.pi) * (1.0 + 3 * 0.044715 * x * x)
+    return 2.0 ** -22 * x.abs(), 2.0 ** -21 * (1.0 + x.abs() * du)
+
+
+def _slope(deriv, x):
+    """|deriv| over the interval the bf16 rounding of x can move it (x (1 +- 2^-8)): the derivative that propagates the
+    pre-activation's rounding, which a value at x alone understates where the curvature is large."""
+    return torch.maximum(deriv(x).abs(), torch.maximum(deriv(x * (1 + 2 ** -8)).abs(), deriv(x * (1 - 2 ** -8)).abs()))
+
+
+def _acc_unit(mag, K):
+    return 2.0 ** -24 * math.sqrt(K) * mag
+
+
+def _report_acc(name, got, ref, mag, K, rtol):
+    """_report with the accumulation tolerance rtol |ref| + GEMM_C 2^-24 sqrt(K) mag, plus c_half."""
+    unit = _acc_unit(mag, K)
+    r = _report(name, got, ref, atol=GEMM_C * unit, rtol=rtol)
+    err = (got.double() - ref).abs()
+    need = torch.where(unit > 0, (2 * err - rtol * ref.abs()) / unit.clamp_min(1e-300), torch.zeros_like(err))
+    r["c_half"] = round(float(need.max().clamp_min(0).item()), 3) if need.numel() else 0.0
+    return r
+
+
+def _combine(name, parts, **extra):
+    """One result from the parts of a check: ok if every part is, the largest tol_use / c_half, failing parts in full."""
+    out = {"name": name, "ok": all(p["ok"] for p in parts) and all(v for v in extra.values() if isinstance(v, bool))}
+    for key in ("tol_use", "c_half"):
+        vals = [p[key] for p in parts if key in p]
+        if vals:
+            out[key] = max(vals)
+    for p in parts:
+        out[f"{p['name']}_ok"] = p["ok"]
+        if not p["ok"]:
+            out[f"{p['name']}_detail"] = p
+    out.update(extra)
+    return out
+
+
+def _pad8(n):
+    return (n + 7) // 8 * 8
+
+
 def check_gemm(M=256, N=256, K=128, B=1, bias=False, epi=ops.EPI_STORE, tile=(0, 0), segs=None, strided=False,
-               nan_to_num=False, name=None, w_kn=None):
+               nan_to_num=False, name=None, w_kn=None, exact=False, aux_out=None, res_special=False):
     """segs: list of extra K sizes appended as additional segments.  w_kn[i]: hand segment i's weight over as [K, N]
-    (the contraction index is the row — what a dgrad reads from the forward weight) instead of [N, K]."""
+    (the contraction index is the row — what a dgrad reads from the forward weight) instead of [N, K].
+    exact: the exact-input mode (bit for bit).  aux_out: give EPI_GELU / EPI_GATE_RES an aux output (default: GELU yes,
+    GATE_RES no).  res_special (GATE_RES, with aux): res holds +inf, -inf and NaN, and +-bf16 max in columns whose gate
+    (2^120) pushes res + gate y past it; out must match the replay from the kernel's aux bit for bit.
+    strided, or odd N: out is a view of a wider zero-filled buffer whose halo must stay zero; with odd N gate / res / aux
+    are views of wider buffers too (row strides must be multiples of 8 elements)."""
     Ks = [K] + list(segs or [])
     S = M
+    ea, ew = ("int", "frac") if exact else (None, None)
+    NP = _pad8(N) + 8                      # row length of the padded buffers
+    if aux_out is None:
+        aux_out = epi == ops.EPI_GELU
+    assert not res_special or (epi == ops.EPI_GATE_RES and aux_out)
     a_list, w_list = [], []
     for i, k in enumerate(Ks):
         if strided:
-            full = _rand(B, S + 3, k + 16, seed=10 + i)
-            a_list.append(full[:, 1:S + 1, 8:8 + k])
-            wfull = _rand(N, k + 8, scale=0.5, seed=20 + i)
-            w_list.append(wfull[:, :k])
+            a_list.append(_gen(B, S + 3, k + 16, seed=10 + i, exact=ea)[:, 1:S + 1, 8:8 + k])
+            w_list.append(_gen(N, k + 8, scale=0.5, seed=20 + i, exact=ew)[:, :k])
         else:
-            a_list.append(_rand(B, S, k, seed=10 + i))
-            w_list.append(_rand(N, k, scale=0.5, seed=20 + i))
+            a_list.append(_gen(B, S, k, seed=10 + i, exact=ea))
+            w_list.append(_gen(N, k, scale=0.5, seed=20 + i, exact=ew))
     bias_t = _rand(N, seed=30) if bias else None
-    acc = sum(a.float() @ w.float().t() for a, w in zip(a_list, w_list))
-    if bias_t is not None:
-        acc = acc + bias_t.float()
+
+    def rows(seed=None):
+        """[B, S, N] bf16 (zeros without a seed); a view of a [B, S, NP] buffer when N is odd."""
+        t = _rand(B, S, N, seed=seed) if seed is not None else torch.zeros(B, S, N, dtype=torch.bfloat16, device=DEV)
+        if N % 2 == 0:
+            return t
+        full = torch.zeros(B, S, NP, dtype=torch.bfloat16, device=DEV)
+        full[..., :N] = t
+        return full[..., :N]
+
     gate = res = aux = None
-    kw = {}
-    if epi == ops.EPI_STORE:
-        ref = acc
-    elif epi == ops.EPI_GELU:
-        aux = torch.zeros(B, S, N, dtype=torch.bfloat16, device=DEV)
-        ref = gelu_tanh(acc.bfloat16().float())
-    elif epi == ops.EPI_GATE_RES:
-        gate = _rand(B, N, seed=31)
-        res = _rand(B, S, N, seed=32)
-        y = acc.bfloat16().float()
-        ref = res.float() + (gate.float()[:, None, :] * y).bfloat16().float()
-    elif epi == ops.EPI_MUL_DGELU:
-        aux = _rand(B, S, N, seed=33)
-        x = aux.float().requires_grad_(True)
-        gelu_tanh(x).sum().backward()
-        ref = acc * x.grad
+    if epi == ops.EPI_GATE_RES:
+        gfull = torch.zeros(B, NP, dtype=torch.bfloat16, device=DEV)
+        gfull[:, :N] = _rand(B, N, seed=31)
+        gate = gfull[:, :N] if N % 2 else gfull[:, :N].contiguous()
+        res = rows(32)
     elif epi == ops.EPI_ADD_RES:
-        res = _rand(B, S, N, seed=32)
-        ref = acc + res.float()
+        res = rows(32)
+    elif epi == ops.EPI_MUL_DGELU:
+        aux = rows(33)
     elif epi == ops.EPI_MUL:
-        aux = _rand(B, S, N, seed=34)
-        ref = acc.bfloat16().float() * aux.float()
-    elif epi == ops.EPI_QUICK_GELU:
-        y = acc.bfloat16().float()
-        ref = y * torch.sigmoid(1.702 * y)
-    else:
-        raise ValueError(f"no reference for epilogue {epi}")
+        aux = rows(34)
+    if aux_out:
+        aux = rows()
+    if res_special:
+        big = torch.finfo(torch.bfloat16).max
+        res[..., 0::8] = float("inf")
+        res[..., 1::8] = float("-inf")
+        res[..., 2::8] = float("nan")
+        res[:, 0::2, 3::8] = big
+        res[:, 1::2, 3::8] = -big
+        gate[:, 3::8] = 2.0 ** 120
     out = None
-    if strided:
-        outfull = torch.zeros(B, S + 2, N + 8, dtype=torch.bfloat16, device=DEV)
+    padded = strided or N % 2 == 1
+    if padded:
+        outfull = torch.zeros(B, S + 2, NP, dtype=torch.bfloat16, device=DEV)
         out = outfull[:, 1:S + 1, :N]
     w_pass = list(w_list)
     if w_kn is not None:
         for i, flag in enumerate(w_kn):
             if flag:                      # [K, N] storage; with `strided` a column range of a wider matrix (row stride > N)
                 if strided:
-                    wide = torch.zeros(w_list[i].shape[1], N + 24, dtype=torch.bfloat16, device=DEV)
+                    wide = torch.zeros(w_list[i].shape[1], _pad8(N) + 24, dtype=torch.bfloat16, device=DEV)
                     wide[:, 8:8 + N] = w_list[i].t()
                     w_pass[i] = wide[:, 8:8 + N]
                 else:
                     w_pass[i] = w_list[i].t().contiguous()
-    got = ops.gemm(a_list, w_pass, bias_t, out=out, epi=epi, gate=gate, res=res, aux=aux, nan_to_num=nan_to_num, tile=tile, w_kn=w_kn)
+    got = ops.gemm(a_list, w_pass, bias_t, out=out, epi=epi, gate=gate, res=res, aux=aux, nan_to_num=nan_to_num, tile=tile,
+                   w_kn=w_kn)
     torch.cuda.synchronize()
-    scale = float(ref.abs().max().item())
-    r = _report(name or f"gemm_M{M}_N{N}_K{Ks}_B{B}_epi{epi}_tile{tile}", got, ref, atol=scale * 6e-3, rtol=1.6e-2)
-    if epi == ops.EPI_GELU:
-        r2 = _report("aux", aux, acc, atol=float(acc.abs().max()) * 6e-3, rtol=1.6e-2)
-        r["aux_ok"] = r2["ok"]
-        r["ok"] = r["ok"] and r2["ok"]
-    if strided:
+
+    acc64 = sum(a.double() @ w.double().t() for a, w in zip(a_list, w_list))
+    mag = sum(a.double().abs() @ w.double().abs().t() for a, w in zip(a_list, w_list))
+    Kt = sum(Ks)
+    parts, extra = [], {}
+    if exact:
+        extra["exact_bound"] = exact_bound_ok(a_list, w_list, mag)
+        want, pre = replay_epilogue(epi, acc64.float(), bias_t, gate, res, aux, nan_to_num)
+        if aux_out:
+            parts.append(_bits("aux", aux, pre))
+        if want is not None:
+            parts.append(_bits("out", got, want))
+        elif epi == ops.EPI_GELU:
+            parts.append(_neighbour("out", got, gelu64(pre.double()), _gelu_atol(pre.double())[0]))
+        elif epi == ops.EPI_QUICK_GELU:
+            parts.append(_neighbour("out", got, quick_gelu64(pre.double())))
+        elif epi == ops.EPI_MUL_DGELU:
+            f = acc64.float() if bias_t is None else acc64.float() + bias_t.float()
+            parts.append(_neighbour("out", got, f.double() * dgelu64(aux.double()),
+                                    f.double().abs() * _gelu_atol(aux.double())[1]))
+    else:
+        f64 = acc64 if bias_t is None else acc64 + bias_t.double()
+        atol = GEMM_C * _acc_unit(mag, Kt)
+        if aux_out:
+            parts.append(_report_acc("aux", aux, f64, mag, Kt, GEMM_RTOL_BF16))
+        if epi == ops.EPI_STORE:
+            parts.append(_report_acc("out", got, f64, mag, Kt, GEMM_RTOL_BF16))
+        elif epi == ops.EPI_ADD_RES:
+            parts.append(_report_acc("out", got, f64 + res.double(), mag, Kt, GEMM_RTOL_BF16))
+        elif epi == ops.EPI_GATE_RES and aux_out:
+            parts.append(_bits("out", got, gate_res_replay(aux, gate, res, nan_to_num)))
+        elif epi == ops.EPI_GATE_RES:
+            g = gate.double()[:, None, :]
+            ref = res.double() + g * f64
+            parts.append(_report("out", got, ref, atol=g.abs() * atol + 2 * _U * (g * f64).abs(), rtol=_U))
+        elif epi == ops.EPI_GELU and aux_out:
+            parts.append(_neighbour("out", got, gelu64(aux.double()), _gelu_atol(aux.double())[0]))
+        elif epi == ops.EPI_GELU:
+            parts.append(_report("out", got, gelu64(f64), atol=_slope(dgelu64, f64) * (atol + _U * f64.abs()) + _gelu_atol(f64)[0],
+                                 rtol=_U))
+        elif epi == ops.EPI_MUL:
+            x = aux.double()
+            parts.append(_report("out", got, f64 * x, atol=x.abs() * (atol + _U * f64.abs()), rtol=_U))
+        elif epi == ops.EPI_QUICK_GELU:
+            parts.append(_report("out", got, quick_gelu64(f64), atol=_slope(dquick_gelu64, f64) * (atol + _U * f64.abs()),
+                                 rtol=_U))
+        elif epi == ops.EPI_MUL_DGELU:
+            d = dgelu64(aux.double())
+            parts.append(_report("out", got, f64 * d, atol=d.abs() * atol + f64.abs() * _gelu_atol(aux.double())[1], rtol=_U))
+        else:
+            raise ValueError(f"no reference for epilogue {epi}")
+    if padded:
         # nothing outside the view may be touched
         mask = torch.ones_like(outfull, dtype=torch.bool)
         mask[:, 1:S + 1, :N] = False
-        r["halo_clean"] = bool((outfull[mask] == 0).all().item())
-        r["ok"] = r["ok"] and r["halo_clean"]
-    return r
+        extra["halo_clean"] = bool((outfull[mask] == 0).all().item())
+    mode = "_exact" if exact else ""
+    return _combine(name or f"gemm_M{M}_N{N}_K{Ks}_B{B}_epi{epi}_tile{tile}{mode}", parts, **extra)
 
 
 # --------------------------------------------------------------------------------------------- attention
@@ -516,14 +771,35 @@ class _deterministic:
         ops.set_deterministic(self.prev)
 
 
-def check_skinny(B=2, S=300, R=16, N=3072, deterministic=None):
-    L = _rand(B, S, R, seed=1)
-    Rm = _rand(B, S, N, seed=2)
+def check_skinny(B=2, S=300, R=16, N=3072, deterministic=None, exact=False, accumulate=False, alpha=0.5):
+    """out[r, n] += alpha sum_m L[m, r] Rm[m, n] (fp32).  deterministic: True = slab workspace + ordered reduce, False =
+    fp32 atomics; R or N not a multiple of 8 takes the CUDA-core kernel.  accumulate: out starts non-zero (N(0, 1), or
+    integers x 2^-4 with exact inputs, so that atomics in any order stay exact).  A non-power-of-two alpha (slab path
+    only with exact inputs) accepts alpha acc + out rounded once (FMA) or twice."""
+    L = _gen(B, S, R, seed=1, exact="int" if exact else None)
+    Rm = _gen(B, S, N, seed=2, exact="frac" if exact else None)
+    out0 = None
+    if accumulate:
+        g = torch.Generator(device="cpu").manual_seed(3)
+        out0 = (torch.randint(-64, 65, (R, N), generator=g).float() / 16 if exact else torch.randn(R, N, generator=g)).to(DEV)
     with _deterministic(deterministic):
-        out = ops.skinny_tn(L, Rm, alpha=0.5)
+        out = ops.skinny_tn(L, Rm, alpha=alpha, out=out0.clone() if accumulate else None)
         torch.cuda.synchronize()
-    ref = 0.5 * (L.float().reshape(-1, R).t() @ Rm.float().reshape(-1, N))
-    return _report(f"skinny_tn_B{B}_S{S}_R{R}_N{N}_det{deterministic}", out, ref, atol=1e-3 * float(ref.abs().max()), rtol=1e-3)
+    L2, R2 = L.double().reshape(-1, R), Rm.double().reshape(-1, N)
+    acc64, mag = L2.t() @ R2, L2.abs().t() @ R2.abs()
+    a32 = _f32(alpha)
+    base = out0.double() if accumulate else torch.zeros_like(acc64)
+    name = f"skinny_tn_B{B}_S{S}_R{R}_N{N}_det{deterministic}" + ("_accum" if accumulate else "") + ("_exact" if exact else "")
+    if not exact:
+        r = _report_acc("out", out, base + a32 * acc64, abs(a32) * mag + base.abs(), B * S, GEMM_RTOL_F32)
+        return _combine(name, [r])
+    bound = exact_bound_ok([L], [Rm], mag)
+    if _is_pow2(a32):
+        return _combine(name, [_bits("out", out, (base + a32 * acc64).float())], exact_bound=bound)
+    once, twice = (base + a32 * acc64).float(), base.float() + a32 * acc64.float()
+    either = ((out == once) | (out == twice)).all().item()
+    return _combine(name, [], exact_bound=bound, fma_or_two_roundings=bool(either),
+                    n_fma=int((out == once).sum().item()), n_twice=int((out == twice).sum().item()))
 
 
 def check_skinny_repeatable(B=4, S=4608, R=48, N=9216):
@@ -622,36 +898,59 @@ CHECKS["skinny_r24"] = lambda: check_skinny(B=1, S=300, R=24, N=512)
 
 
 # --------------------------------------------------------------------------------------------- VAE encode kernels
-def check_conv3x3(B=2, H=24, W=40, Ci=64, Co=128, stride=1, bias=True, res=False):
+def check_conv3x3(B=2, H=24, W=40, Ci=64, Co=128, stride=1, bias=True, res=False, exact=False):
+    """Implicit-GEMM 3x3 conv (K = 9 Ci): the fp64 conv of the same bf16 inputs; exact: bf16((acc + bias) + res)."""
     import torch.nn.functional as F
-    x = _rand(B, H, W, Ci, seed=1)
-    w = _rand(Co, Ci, 3, 3, scale=(9 * Ci) ** -0.5, seed=2)
+    x = _gen(B, H, W, Ci, seed=1, exact="int" if exact else None)
+    w = _gen(Co, Ci, 3, 3, scale=(9 * Ci) ** -0.5, seed=2, exact="frac" if exact else None)
     bv = _rand(Co, scale=0.1, seed=3) if bias else None
     Ho, Wo = (H, W) if stride == 1 else (H // 2, W // 2)
     rv = _rand(B, Ho, Wo, Co, seed=4) if res else None
     w9 = w.permute(0, 2, 3, 1).reshape(Co, -1).contiguous()
     out = ops.conv3x3_nhwc(x, w9, bv, rv, stride)
     torch.cuda.synchronize()
-    xn = x.float().permute(0, 3, 1, 2)
-    if stride == 1:
-        ref = F.conv2d(xn, w.float(), bv.float() if bias else None, padding=1)
-    else:
-        ref = F.conv2d(F.pad(xn, (0, 1, 0, 1)), w.float(), bv.float() if bias else None, stride=2)
-    ref = ref.permute(0, 2, 3, 1)
-    if res:
-        ref = ref + rv.float()
-    return _report(f"conv3x3_s{stride}_{Ci}to{Co}_{H}x{W}", out, ref, atol=2e-2, rtol=1e-2)
+
+    def conv(xt, wt):
+        xn = xt.double().permute(0, 3, 1, 2)
+        if stride == 1:
+            return F.conv2d(xn, wt.double(), padding=1).permute(0, 2, 3, 1)
+        return F.conv2d(F.pad(xn, (0, 1, 0, 1)), wt.double(), stride=2).permute(0, 2, 3, 1)
+
+    acc64, mag = conv(x, w), conv(x.abs(), w.abs())
+    name = f"conv3x3_s{stride}_{Ci}to{Co}_{H}x{W}" + ("_exact" if exact else "")
+    if exact:
+        f = acc64.float() + (bv.float() if bias else 0.0)
+        want = (f + rv.float() if res else f).bfloat16()
+        return _combine(name, [_bits("out", out, want)], exact_bound=exact_bound_ok([x], [w], mag))
+    ref = acc64 + (bv.double() if bias else 0.0) + (rv.double() if res else 0.0)
+    return _combine(name, [_report_acc("out", out, ref, mag, 9 * Ci, GEMM_RTOL_BF16)])
 
 
-def check_conv_in(B=2, H=20, W=36, C=128):
+def check_conv_in(B=2, H=20, W=36, C=128, exact=False):
+    """RGB stem conv (K = 27).  C = 64 / 128 / 256: the tensor-core kernel, bf16(acc + bias); other C: the CUDA-core
+    kernel, which starts from the bias and adds the 27 taps in (channel, dy, dx) order, replayed as such when exact."""
     import torch.nn.functional as F
-    x = _rand(B, 3, H, W, seed=1)
-    w = _rand(C, 3, 3, 3, scale=27 ** -0.5, seed=2)
+    x = _gen(B, 3, H, W, seed=1, exact="int" if exact else None)
+    w = _gen(C, 3, 3, 3, scale=27 ** -0.5, seed=2, exact="frac" if exact else None)
     bv = _rand(C, scale=0.1, seed=3)
     out = ops.conv_in_3ch(x, w, bv)
     torch.cuda.synchronize()
-    ref = F.conv2d(x.float(), w.float(), bv.float(), padding=1).permute(0, 2, 3, 1)
-    return _report("conv_in_3ch", out, ref, atol=1e-2, rtol=1e-2)
+    acc64 = F.conv2d(x.double(), w.double(), padding=1).permute(0, 2, 3, 1)
+    mag = F.conv2d(x.double().abs(), w.double().abs(), padding=1).permute(0, 2, 3, 1)
+    name = f"conv_in_3ch_C{C}_{H}x{W}" + ("_exact" if exact else "")
+    if not exact:
+        return _combine(name, [_report_acc("out", out, acc64 + bv.double(), mag, 27, GEMM_RTOL_BF16)])
+    if C in (64, 128, 256):
+        want = (acc64.float() + bv.float()).bfloat16()
+    else:
+        xp = F.pad(x.float(), (1, 1, 1, 1))
+        acc = bv.float().expand(B, H, W, C).clone()
+        for c in range(3):
+            for dy in range(3):
+                for dx in range(3):
+                    acc = acc + xp[:, c, dy:dy + H, dx:dx + W, None] * w.float()[:, c, dy, dx]
+        want = acc.bfloat16()
+    return _combine(name, [_bits("out", out, want)], exact_bound=exact_bound_ok([x], [w], mag))
 
 
 def check_groupnorm(B=2, H=16, W=24, C=128, G=32, silu=True, mean=0.0):
@@ -870,33 +1169,63 @@ CHECKS.update({
 
 
 # --------------------------------------------------------------------------------------------- full-rank weight gradient
-def check_wgrad_full(B=2, S=300, N=256, K=320, strided=False, accumulate=False, alpha=1.0):
+def wgrad_tile_width(N, K, sms=132):
+    """The tile width stb_wgrad_full picks: 256 unless that leaves more than half of the SMs idle, and always for K <= 128."""
+    return 256 if ((N + 127) // 128) * ((K + 255) // 256) >= sms // 2 or K <= 128 else 128
+
+
+def check_wgrad_full(B=2, S=300, N=256, K=320, strided=False, accumulate=False, alpha=1.0, exact=False):
+    """dW [N, K] = alpha sum_tokens dy[:, n] x[:, k] (+ dW): contraction over the B S tokens.  exact: bf16(alpha acc + old)
+    bit for bit; a non-power-of-two alpha with accumulate accepts the FMA or the two-rounding result per element."""
+    ed, ex = ("int", "frac") if exact else (None, None)
     if strided:   # row ranges / column ranges of larger buffers, like the joint hidden buffer and the fused qkv gradient
-        dyf = _rand(B, S + 5, N + 64, seed=41)
-        xf = _rand(B, S + 9, K + 32, seed=42)
+        dyf = _gen(B, S + 5, N + 64, seed=41, exact=ed)
+        xf = _gen(B, S + 9, K + 32, seed=42, exact=ex)
         dy, x = dyf[:, 3:S + 3, 32:32 + N], xf[:, 4:S + 4, 8:8 + K]
     else:
-        dy, x = _rand(B, S, N, seed=41), _rand(B, S, K, seed=42)
-    ref = alpha * torch.einsum("bsn,bsk->nk", dy.float(), x.float())
-    out = None
+        dy, x = _gen(B, S, N, seed=41, exact=ed), _gen(B, S, K, seed=42, exact=ex)
+    out = old = None
     if accumulate:
         out = _rand(N, K, seed=43)
-        ref = ref + out.float()
+        old = out.clone()
     got = ops.wgrad_full(dy, x, out=out, alpha=alpha, accumulate=accumulate)
     torch.cuda.synchronize()
-    return _report(f"wgrad_full_B{B}_S{S}_N{N}_K{K}", got, ref, atol=float(ref.abs().max()) * 6e-3, rtol=1.6e-2)
+    acc64 = torch.einsum("bsn,bsk->nk", dy.double(), x.double())
+    mag = torch.einsum("bsn,bsk->nk", dy.double().abs(), x.double().abs())
+    a32 = _f32(alpha)
+    name = f"wgrad_full_B{B}_S{S}_N{N}_K{K}_bn{wgrad_tile_width(N, K)}" + ("_accum" if accumulate else "") + \
+        ("_exact" if exact else "")
+    base = old.double() if accumulate else torch.zeros_like(acc64)
+    if not exact:
+        return _combine(name, [_report_acc("dw", got, base + a32 * acc64, abs(a32) * mag, B * S, GEMM_RTOL_BF16)])
+    bound = exact_bound_ok([dy], [x], mag)
+    twice = ((a32 * acc64.float() + old.float()) if accumulate else a32 * acc64.float()).bfloat16()
+    if _is_pow2(a32) or not accumulate:
+        return _combine(name, [_bits("dw", got, twice)], exact_bound=bound)
+    once = (base + a32 * acc64).float().bfloat16()
+    either = ((got.view(torch.int16) == once.view(torch.int16)) | (got.view(torch.int16) == twice.view(torch.int16))).all()
+    return _combine(name, [], exact_bound=bound, fma_or_two_roundings=bool(either.item()),
+                    n_fma=int((got == once).sum().item()), n_twice=int((got == twice).sum().item()))
 
 
-def check_colsum2(B=3, S=333, D=1536):
-    dyf, zf = _rand(B, S + 3, D + 16, seed=51), _rand(B, S, D, seed=52)
+def check_colsum2(B=3, S=333, D=1536, exact=False):
+    """sum_s dy and sum_s dy z (fp32, atomics over row chunks) against fp64; exact: bit for bit."""
+    dyf = _gen(B, S + 3, D + 16, seed=51, exact="int" if exact else None)
+    zf = _gen(B, S, D, seed=52, exact="frac" if exact else None)
     dy = dyf[:, 1:S + 1, 8:8 + D]
     sm, dt = ops.colsum2(dy, zf)
-    torch.cuda.synchronize()
-    r1 = _report("colsum", sm, dy.float().sum(1), atol=0.05, rtol=1e-3)
-    r2 = _report("coldot", dt, (dy.float() * zf.float()).sum(1), atol=0.05, rtol=1e-3)
     only = ops.colsum2(dy, None)[0]
-    return {"name": f"colsum2_B{B}_S{S}_D{D}", "ok": r1["ok"] and r2["ok"] and bool(torch.allclose(only, sm, atol=1e-3)),
-            "max_err": max(r1["max_err"], r2["max_err"])}
+    torch.cuda.synchronize()
+    d64, z64 = dy.double(), zf.double()
+    s_ref, s_mag = d64.sum(1), d64.abs().sum(1)
+    p_ref, p_mag = (d64 * z64).sum(1), (d64 * z64).abs().sum(1)
+    name = f"colsum2_B{B}_S{S}_D{D}" + ("_exact" if exact else "")
+    if exact:
+        parts = [_bits("colsum", sm, s_ref.float()), _bits("coldot", dt, p_ref.float()), _bits("colsum_only", only, s_ref.float())]
+        return _combine(name, parts, exact_bound=exact_bound_ok([dy], [zf], p_mag) and float(s_mag.max()) < EXACT_BOUND)
+    parts = [_report_acc("colsum", sm, s_ref, s_mag, S, GEMM_RTOL_F32), _report_acc("coldot", dt, p_ref, p_mag, S, GEMM_RTOL_F32),
+             _report_acc("colsum_only", only, s_ref, s_mag, S, GEMM_RTOL_F32)]
+    return _combine(name, parts)
 
 
 CHECKS.update({
@@ -1137,4 +1466,101 @@ CHECKS.update({
     "skinny_repeatable_flux_lora": lambda: check_skinny_repeatable(),
     "flow_loss_full_size": lambda: check_loss_full_size("flow"),
     "target_loss_full_size": lambda: check_loss_full_size("target"),
+})
+
+
+# --------------------------------------------------------------------------------------------- GEMM family, exact inputs
+# The exact-input mode over the grid above: every epilogue at every tile width and weight layout, 2-CTA clusters with an
+# odd m-tile count, ring-7 segments, skinny M and the Flux shapes (K = 12288; segments 3072 + 12288 and 12288 + 9216 + 48).
+for _en, (_epi, _nan) in _EPIS.items():
+    for _bn in _BNS:
+        for _kn in (False, True):
+            CHECKS[f"gemm_epi_{_en}_bn{_bn}" + ("_wkn" if _kn else "") + "_exact"] = _case(
+                check_gemm, 200, 328, 200, B=2, bias=True, epi=_epi, nan_to_num=_nan, tile=(0, _bn),
+                w_kn=[True] if _kn else None, exact=True)
+for _en in ("store", "gelu", "gate_res_nan", "mul_dgelu", "mul", "quick_gelu"):
+    _epi, _nan = _EPIS[_en]
+    CHECKS[f"gemm_cluster_odd_mtiles_{_en}_exact"] = _case(check_gemm, 300, 328, 200, B=3, segs=[72, 16], bias=True, epi=_epi,
+                                                           nan_to_num=_nan, tile=(2, 128), exact=True)
+for _bn in _BNS:
+    CHECKS[f"gemm_ring7_bn{_bn}_exact"] = _case(check_gemm, 4608, 3072, 200, B=1, segs=[72, 16], bias=True, tile=(0, _bn),
+                                                exact=True)
+CHECKS["gemm_ring7_bn128_wkn_mixed_exact"] = _case(check_gemm, 4608, 3072, 200, B=1, segs=[72, 16], w_kn=[True, False, True],
+                                                   tile=(0, 128), exact=True)
+for _m in (1, 2, 65, 129):
+    for _b in (1, 4):
+        CHECKS[f"gemm_skinny_m{_m}_b{_b}_exact"] = _case(check_gemm, _m, 18432, 3072, B=_b, bias=True, exact=True)
+CHECKS["gemm_k12288_exact"] = _case(check_gemm, 4608, 3072, 12288, B=1, bias=True, exact=True)
+CHECKS["gemm_seg2_3072_12288_gate_res_exact"] = _case(check_gemm, 4608, 3072, 3072, B=1, segs=[12288], bias=True,
+                                                      epi=E.EPI_GATE_RES, nan_to_num=True, exact=True)
+CHECKS["gemm_seg3_dgrad_12288_9216_48_exact"] = _case(check_gemm, 4608, 3072, 12288, B=1, segs=[9216, 48], exact=True)
+CHECKS["gemm_wkn_flux_dgrad_exact"] = _case(check_gemm, 4608, 3072, 9216, w_kn=[True], tile=(0, 256), exact=True)
+
+# --------------------------------------------------------------------------------------------- GEMM paths without a reference before
+for _x in (False, True):
+    _s = "_exact" if _x else ""
+    for _bn in _BNS:
+        # the bf16 linear output full fine-tune keeps for the gate gradient
+        CHECKS[f"gemm_gate_res_aux_bn{_bn}{_s}"] = _case(check_gemm, 200, 328, 200, B=2, bias=True, epi=E.EPI_GATE_RES,
+                                                         nan_to_num=True, aux_out=True, tile=(0, _bn), exact=_x)
+        # nan_to_num on +-inf / NaN in res and on res + gate y pushed past the bf16 maximum; without it they pass through
+        for _nan in (True, False):
+            CHECKS[f"gemm_gate_res_nonfinite_nan{int(_nan)}_bn{_bn}{_s}"] = _case(
+                check_gemm, 200, 328, 200, B=2, bias=True, epi=E.EPI_GATE_RES, nan_to_num=_nan, aux_out=True,
+                res_special=True, tile=(0, _bn), exact=_x)
+        CHECKS[f"gemm_gelu_noaux_bn{_bn}{_s}"] = _case(check_gemm, 200, 328, 200, B=2, bias=True, epi=E.EPI_GELU,
+                                                       aux_out=False, tile=(0, _bn), exact=_x)
+    CHECKS[f"gemm_gelu_noaux_cluster{_s}"] = _case(check_gemm, 300, 328, 200, B=3, bias=True, epi=E.EPI_GELU, aux_out=False,
+                                                   tile=(2, 128), exact=_x)
+    # odd N: the lone last column of every row (bias, gate, res / aux words and the store of one element)
+    for _n in (1, 3, 65, 327):
+        for _en, _kw in (("store", dict(epi=E.EPI_STORE)), ("gate_res_aux", dict(epi=E.EPI_GATE_RES, nan_to_num=True, aux_out=True)),
+                         ("mul", dict(epi=E.EPI_MUL)), ("gelu", dict(epi=E.EPI_GELU)), ("add_res", dict(epi=E.EPI_ADD_RES))):
+            CHECKS[f"gemm_odd_n{_n}_{_en}{_s}"] = _case(check_gemm, 200, _n, 200, B=2, bias=True, **_kw, exact=_x)
+    CHECKS[f"gemm_odd_n327_gelu_cluster{_s}"] = _case(check_gemm, 300, 327, 200, B=3, bias=True, epi=E.EPI_GELU,
+                                                      tile=(2, 128), exact=_x)
+    CHECKS[f"gemm_odd_n65_bn256{_s}"] = _case(check_gemm, 200, 65, 200, B=2, bias=True, tile=(0, 256), exact=_x)
+
+    # skinny_tn into a non-zero out: slab workspace, fp32 atomics, CUDA-core kernel (N % 8 != 0)
+    CHECKS[f"skinny_ws_accum{_s}"] = _case(check_skinny, B=2, S=700, R=48, N=1536, deterministic=True, accumulate=True, exact=_x)
+    CHECKS[f"skinny_atomic_accum{_s}"] = _case(check_skinny, B=2, S=700, R=48, N=1536, deterministic=False, accumulate=True,
+                                                exact=_x)
+    CHECKS[f"skinny_cuda_core_accum{_s}"] = _case(check_skinny, B=2, S=100, R=16, N=250, accumulate=True, exact=_x)
+    # wgrad_full with N % 128 != 0 at both tile widths (K <= 128 forces 256; 520 gives 128 on 132 SMs)
+    for _n in (200, 136):
+        for _k in (120, 520):
+            CHECKS[f"wgrad_full_n{_n}_k{_k}{_s}"] = _case(check_wgrad_full, B=2, S=300, N=_n, K=_k, exact=_x)
+    CHECKS[f"wgrad_full_n200_accum{_s}"] = _case(check_wgrad_full, B=2, S=300, N=200, K=520, accumulate=True, alpha=0.25, exact=_x)
+    # conv3x3 with C_out not a multiple of the tile width (72 at 128, 136 and 200 at 256)
+    for _co in (72, 136, 200):
+        CHECKS[f"conv3x3_co{_co}{_s}"] = _case(check_conv3x3, B=2, H=24, W=40, Ci=64, Co=_co, res=_co == 136, exact=_x)
+    CHECKS[f"conv3x3_s2_co200{_s}"] = _case(check_conv3x3, B=1, H=32, W=48, Ci=128, Co=200, stride=2, exact=_x)
+
+# exact mode of the existing weight-gradient, LoRA-gradient, reduction and conv checks
+CHECKS.update({
+    "skinny_exact": lambda: check_skinny(exact=True),
+    "skinny_flux_exact": lambda: check_skinny(B=4, S=4608, R=48, N=9216, exact=True),
+    "skinny_ragged_exact": lambda: check_skinny(B=3, S=333, R=16, N=200, exact=True),
+    "skinny_r64_ws_exact": lambda: check_skinny(B=2, S=700, R=64, N=1536, deterministic=True, exact=True),
+    "skinny_r128_atomic_exact": lambda: check_skinny(B=2, S=700, R=128, N=1536, deterministic=False, exact=True),
+    "skinny_ws_accum_alpha0.3_exact": lambda: check_skinny(B=2, S=700, R=48, N=1536, deterministic=True, accumulate=True,
+                                                           alpha=0.3, exact=True),
+    "wgrad_full_basic_exact": lambda: check_wgrad_full(exact=True),
+    "wgrad_full_strided_accum_exact": lambda: check_wgrad_full(B=3, S=231, N=384, K=200, strided=True, accumulate=True,
+                                                               alpha=0.5, exact=True),
+    "wgrad_full_accum_alpha0.3_exact": lambda: check_wgrad_full(B=3, S=231, N=384, K=200, accumulate=True, alpha=0.3,
+                                                                exact=True),
+    "wgrad_full_sd3_qkv_exact": lambda: check_wgrad_full(B=2, S=1255, N=4608, K=1536, exact=True),
+    "wgrad_full_narrow_exact": lambda: check_wgrad_full(B=1, S=1000, N=128, K=64, exact=True),
+    "wgrad_full_flux_mlp_exact": lambda: check_wgrad_full(B=1, S=4608, N=3072, K=12288, exact=True),
+    "colsum2_exact": lambda: check_colsum2(exact=True),
+    "colsum2_small_exact": lambda: check_colsum2(B=1, S=7, D=64, exact=True),
+    "conv3x3_s1_res_exact": lambda: check_conv3x3(Ci=128, Co=256, res=True, exact=True),
+    "conv3x3_out32_exact": lambda: check_conv3x3(B=2, H=16, W=16, Ci=512, Co=32, exact=True),
+    "conv3x3_pair_oddrows_exact": lambda: check_conv3x3(B=1, H=149, W=120, Ci=128, Co=128, res=True, exact=True),
+    "conv3x3_pair_s2_wide_exact": lambda: check_conv3x3(B=1, H=160, W=600, stride=2, Ci=64, Co=256, exact=True),
+    "conv3x3_s1_512_exact": lambda: check_conv3x3(B=1, H=16, W=16, Ci=512, Co=512, res=True, exact=True),
+    "conv_in_3ch_exact": lambda: check_conv_in(exact=True),
+    "conv_in_3ch_wide_exact": lambda: check_conv_in(B=2, H=9, W=300, C=128, exact=True),
+    "conv_in_3ch_c8_cuda_core_exact": lambda: check_conv_in(B=1, H=12, W=20, C=8, exact=True),
 })
