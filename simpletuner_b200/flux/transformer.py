@@ -285,17 +285,24 @@ class FluxTransformerBlock(nn.Module):
             B = silu_temb.shape[0] // 3
             mod_img = self.norm1.linear(silu_temb[B:])            # [2B, 6D]: scene rows, conditioning rows
             mod_txt = self.norm1_context.linear(silu_temb[:B])
-        st = {"S_txt": S_txt, "H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias, "img_segs": segs}
         a = self.attn
         attn_l = [a.to_q, a.to_k, a.to_v, a.to_out[0], a.add_q_proj, a.add_k_proj, a.add_v_proj, a.to_add_out]
         mlp_l = [self.ff.net[0].proj, self.ff.net[2], self.ff_context.net[0].proj, self.ff_context.net[2]]
-        lora = _lora_list(attn_l)
-        mlp = _lora_list(mlp_l)
-        st["lokr_scales"] = _lokr_scales(attn_l + [None] * 4 + mlp_l)
-        if any(t is not None for t in mlp):
-            lora = lora + [None] * 8 + mlp          # [16..23] = the SD3.5 second attention, unused here
-        return DoubleBlockFn.apply(h, mod_img, mod_txt, cos, sin, st, *lora)
+        return run_double_block(self, h, mod_img, mod_txt, cos, sin, S_txt, lora_scaling, key_bias, segs, attn_l, mlp_l)
+
+
+def run_double_block(blk, h, mod_img, mod_txt, cos, sin, S_txt, lora_scaling, key_bias, segs, attn_l, mlp_l, **flags):
+    """DoubleBlockFn over one joint block: `attn_l` = the image q, k, v, out then text q, k, v, out Linears, `mlp_l` = the
+    image fc1, fc2 then text fc1, fc2 Linears; `blk` provides heads, head_dim, plans() and the step's dropout state.
+    Shared by the Flux and Qwen-Image double blocks; `flags` are DoubleBlockFn's `st` switches (e.g. nan_to_num_txt)."""
+    st = {"S_txt": S_txt, "H": blk.heads, "hd": blk.head_dim, "plans": blk.plans(), "lora_scaling": lora_scaling,
+          "lora_drop": getattr(blk, "_lora_drop", None), "key_bias": key_bias, "img_segs": segs, **flags}
+    lora = _lora_list(attn_l)
+    mlp = _lora_list(mlp_l)
+    st["lokr_scales"] = _lokr_scales(attn_l + [None] * 4 + mlp_l)
+    if any(t is not None for t in mlp):
+        lora = lora + [None] * 8 + mlp          # [16..23] = the SD3.5 second attention, unused here
+    return DoubleBlockFn.apply(h, mod_img, mod_txt, cos, sin, st, *lora)
 
 
 class FluxSingleTransformerBlock(nn.Module):
@@ -482,7 +489,92 @@ class LoraDropoutAPI:
         return p
 
 
-class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
+class AdapterModelAPI:
+    """Gradient checkpointing and the PEFT adapter surface shared by the denoisers built on the Flux blocks.  A model sets
+    `_DEFAULT_LORA_TARGETS` and `_lora_adaptable(name)` (the Linears its block schedules can adapt)."""
+
+    _DEFAULT_LORA_TARGETS: Sequence[str] = ()
+
+    @staticmethod
+    def _lora_adaptable(name: str) -> bool:
+        raise NotImplementedError
+
+    def enable_gradient_checkpointing(self):
+        """common.py:3550-3636 / flux/transformer.py:1240-1287: blocks selected by `gradient_checkpointing_interval`
+        (every block when None) are re-run in backward instead of keeping their saved set (block input only is kept),
+        through torch.utils.checkpoint like the reference.  Off by default: the block schedules already keep a minimal
+        activation set; on an 80 GB H100 that holds one 1024^2 sample next to the Flux.1-dev weights, and larger batches need
+        recompute."""
+        self.gradient_checkpointing = True
+
+    def disable_gradient_checkpointing(self):
+        self.gradient_checkpointing = False
+
+    def _run_block(self, index: int, blk, *args):
+        interval = getattr(self, "gradient_checkpointing_interval", None)
+        if self.gradient_checkpointing and torch.is_grad_enabled() and (interval is None or index % interval == 0):
+            from torch.utils.checkpoint import checkpoint
+            return checkpoint(blk, *args, use_reentrant=False)
+        return blk(*args)
+
+    def set_gradient_checkpointing_interval(self, value: int):
+        self.gradient_checkpointing_interval = value
+
+    def lora_linears(self) -> Dict[str, Linear]:
+        return {n: m for n, m in self.named_modules() if isinstance(m, Linear) and m.lora_A is not None}
+
+    def add_adapter(self, lora_config=None, adapter_name: str = "default", *, rank: Optional[int] = None,
+                    lora_alpha: Optional[float] = None, target_modules: Optional[Sequence[str]] = None,
+                    lora_dropout: float = 0.0):
+        """PeftAdapterMixin.add_adapter (reference common.py:1117).  Accepts a peft.LoraConfig-like object
+        (attributes r, lora_alpha, target_modules, lora_dropout) or keyword arguments."""
+        if lora_config is not None:
+            rank = getattr(lora_config, "r", rank)
+            lora_alpha = getattr(lora_config, "lora_alpha", lora_alpha)
+            target_modules = getattr(lora_config, "target_modules", target_modules)
+            lora_dropout = getattr(lora_config, "lora_dropout", lora_dropout)
+        if rank is None:
+            raise ValueError("LoRA rank is required")
+        if getattr(self, "_lycoris_network", None) is not None:
+            raise NotImplementedError("a LyCORIS network is attached: PEFT LoRA and LoKr adapters cannot be mixed on this path")
+        lora_dropout = self._check_dropout_p(lora_dropout)
+        if not 1 <= rank <= 128:
+            raise NotImplementedError("fused LoRA path supports rank 1..128 (one 128-wide rank block per adapted Linear)")
+        lora_alpha = float(lora_alpha) if lora_alpha is not None else float(rank)  # common.py:1090-1093
+        targets = list(target_modules) if target_modules is not None else list(self._DEFAULT_LORA_TARGETS)
+        n = 0
+        chosen = []
+        for name, mod in self.named_modules():
+            if not isinstance(mod, Linear) or not _peft_match(name, targets):
+                continue
+            if not self._lora_adaptable(name):
+                raise NotImplementedError(f"LoRA target {name} is not supported by the fused path (adaLN / embedder linears: "
+                                          "use the reference module, e.g. for flux_lora_target=ai-toolkit)")
+            chosen.append(mod)
+        for mod in chosen:
+            mod.add_lora(rank, lora_alpha, adapter_name)
+            n += 1
+        if n == 0:
+            raise ValueError(f"no module matched LoRA targets {targets}")
+        self._lora_scaling = lora_alpha / rank
+        self._lora_dropout_p = lora_dropout
+        self.peft_config[adapter_name] = SimpleNamespace(r=rank, lora_alpha=lora_alpha, target_modules=targets,
+                                                         lora_dropout=lora_dropout)
+        return n
+
+    def disable_lora(self):
+        for m in self.lora_linears().values():
+            m.lora_enabled = False
+
+    def enable_lora(self):
+        for m in self.lora_linears().values():
+            m.lora_enabled = True
+
+    def trainable_parameters(self):
+        return [p for p in self.parameters() if p.requires_grad]
+
+
+class FluxTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, nn.Module):
     _no_split_modules = ["FluxTransformerBlock", "FluxSingleTransformerBlock"]
     _supports_gradient_checkpointing = True
 
@@ -515,27 +607,12 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         self._lora_scaling = 1.0
         self.peft_config: Dict[str, Any] = {}
 
-    # ---- reference-facing utilities ---------------------------------------------------------
-    def enable_gradient_checkpointing(self):
-        """common.py:3550-3636 / flux/transformer.py:1240-1287: blocks selected by `gradient_checkpointing_interval`
-        (every block when None) are re-run in backward instead of keeping their saved set (block input only is kept),
-        through torch.utils.checkpoint like the reference.  Off by default: the block schedules already keep a minimal
-        activation set; on an 80 GB H100 that holds one 1024^2 sample next to the Flux.1-dev weights, and larger batches need
-        recompute."""
-        self.gradient_checkpointing = True
+    _DEFAULT_LORA_TARGETS = FLUX_LORA_TARGETS["all"]
 
-    def disable_gradient_checkpointing(self):
-        self.gradient_checkpointing = False
-
-    def _run_block(self, index: int, blk, *args):
-        interval = getattr(self, "gradient_checkpointing_interval", None)
-        if self.gradient_checkpointing and torch.is_grad_enabled() and (interval is None or index % interval == 0):
-            from torch.utils.checkpoint import checkpoint
-            return checkpoint(blk, *args, use_reentrant=False)
-        return blk(*args)
-
-    def set_gradient_checkpointing_interval(self, value: int):
-        self.gradient_checkpointing_interval = value
+    @staticmethod
+    def _lora_adaptable(name: str) -> bool:
+        # adaLN linears ("ai-toolkit") stay on the reference module: their gradients need d loss / d modulation
+        return name.endswith(_ADAPTABLE_SUFFIXES) or name in ("proj_out", "x_embedder")
 
     def invalidate_plans(self):
         """Call after base weights change (load_state_dict / .to()); derived layouts are rebuilt lazily."""
@@ -560,59 +637,6 @@ class FluxTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         if getattr(self, "_lycoris_network", None) is not None:
             for blk in list(self.transformer_blocks) + list(self.single_transformer_blocks):
                 blk.drop_adapted_plans()
-
-    def lora_linears(self) -> Dict[str, Linear]:
-        return {n: m for n, m in self.named_modules() if isinstance(m, Linear) and m.lora_A is not None}
-
-    def add_adapter(self, lora_config=None, adapter_name: str = "default", *, rank: Optional[int] = None,
-                    lora_alpha: Optional[float] = None, target_modules: Optional[Sequence[str]] = None,
-                    lora_dropout: float = 0.0):
-        """PeftAdapterMixin.add_adapter (reference common.py:1117).  Accepts a peft.LoraConfig-like object
-        (attributes r, lora_alpha, target_modules, lora_dropout) or keyword arguments."""
-        if lora_config is not None:
-            rank = getattr(lora_config, "r", rank)
-            lora_alpha = getattr(lora_config, "lora_alpha", lora_alpha)
-            target_modules = getattr(lora_config, "target_modules", target_modules)
-            lora_dropout = getattr(lora_config, "lora_dropout", lora_dropout)
-        if rank is None:
-            raise ValueError("LoRA rank is required")
-        if getattr(self, "_lycoris_network", None) is not None:
-            raise NotImplementedError("a LyCORIS network is attached: PEFT LoRA and LoKr adapters cannot be mixed on this path")
-        lora_dropout = self._check_dropout_p(lora_dropout)
-        if not 1 <= rank <= 128:
-            raise NotImplementedError("fused LoRA path supports rank 1..128 (one 128-wide rank block per adapted Linear)")
-        lora_alpha = float(lora_alpha) if lora_alpha is not None else float(rank)  # common.py:1090-1093
-        targets = list(target_modules) if target_modules is not None else FLUX_LORA_TARGETS["all"]
-        n = 0
-        chosen = []
-        for name, mod in self.named_modules():
-            if not isinstance(mod, Linear) or not _peft_match(name, targets):
-                continue
-            if not (name.endswith(_ADAPTABLE_SUFFIXES) or name in ("proj_out", "x_embedder")):
-                raise NotImplementedError(f"LoRA target {name} is not supported by the fused path (adaLN / embedder linears: "
-                                          "use the reference module, e.g. for flux_lora_target=ai-toolkit)")
-            chosen.append(mod)
-        for mod in chosen:
-            mod.add_lora(rank, lora_alpha, adapter_name)
-            n += 1
-        if n == 0:
-            raise ValueError(f"no module matched LoRA targets {targets}")
-        self._lora_scaling = lora_alpha / rank
-        self._lora_dropout_p = lora_dropout
-        self.peft_config[adapter_name] = SimpleNamespace(r=rank, lora_alpha=lora_alpha, target_modules=targets,
-                                                         lora_dropout=lora_dropout)
-        return n
-
-    def disable_lora(self):
-        for m in self.lora_linears().values():
-            m.lora_enabled = False
-
-    def enable_lora(self):
-        for m in self.lora_linears().values():
-            m.lora_enabled = True
-
-    def trainable_parameters(self):
-        return [p for p in self.parameters() if p.requires_grad]
 
     # ---- forward ------------------------------------------------------------------------------
     def _rope(self, txt_ids, img_ids, device):

@@ -62,8 +62,18 @@ def _pixart_step():
     return PixartSigma
 
 
+def _qwen_image():
+    from ..qwen_image.transformer import QwenImageTransformer2DModel
+    return QwenImageTransformer2DModel
+
+
+def _qwen_image_step():
+    from ..qwen_image.model import QwenImage
+    return QwenImage
+
+
 FAMILIES: Dict[str, FamilySpec] = {
-    # registry keys: flux/model.py:1504, sd3/model.py:900, pixart/model.py:858 ("pixart_sigma")
+    # registry keys: flux/model.py:1504, sd3/model.py:900, pixart/model.py:858 ("pixart_sigma"), qwen_image/model.py:1874
     "flux": FamilySpec("flux", "simpletuner.helpers.models.flux.model", "Flux", _flux, _flux_step,
                        ("patch_size", "in_channels", "num_layers", "num_single_layers", "attention_head_dim",
                         "num_attention_heads", "joint_attention_dim", "pooled_projection_dim", "guidance_embeds",
@@ -77,6 +87,21 @@ FAMILIES: Dict[str, FamilySpec] = {
                                 "cross_attention_dim", "sample_size", "patch_size", "caption_channels", "interpolation_scale",
                                 "use_additional_conditions", "norm_eps")),
 }
+# Opt-in families: `install()` registers them only when named (`install(["qwen_image"])`), so an existing setup that calls
+# `install()` keeps exactly the families it had.
+OPT_IN_FAMILIES: Dict[str, FamilySpec] = {
+    "qwen_image": FamilySpec("qwen_image", "simpletuner.helpers.models.qwen_image.model", "QwenImage", _qwen_image,
+                             _qwen_image_step,
+                             ("patch_size", "in_channels", "out_channels", "num_layers", "attention_head_dim",
+                              "num_attention_heads", "joint_attention_dim", "guidance_embeds", "axes_dims_rope")),
+}
+
+
+def family_spec(family: str) -> FamilySpec:
+    spec = FAMILIES.get(family) or OPT_IN_FAMILIES.get(family)
+    if spec is None:
+        raise KeyError(f"unknown family {family!r}; known: {sorted(FAMILIES) + sorted(OPT_IN_FAMILIES)}")
+    return spec
 
 
 def _cfg_get(cfg: Any, key: str, default=None):
@@ -113,7 +138,7 @@ class B200FoundationMixin:
     def _b200_install(self):
         import torch
 
-        spec = FAMILIES[self.B200_FAMILY]
+        spec = family_spec(self.B200_FAMILY)
         ref = self.model
         if ref is None:
             raise NotImplementedError("no denoiser loaded")
@@ -187,8 +212,7 @@ class B200FoundationMixin:
 
 def make_b200_family(reference_cls: type, family: str) -> type:
     """`class <Ref>B200(B200FoundationMixin, reference_cls)` with B200_FAMILY set."""
-    if family not in FAMILIES:
-        raise KeyError(f"unknown family {family!r}; known: {sorted(FAMILIES)}")
+    family_spec(family)
     return type(reference_cls.__name__ + "B200", (B200FoundationMixin, reference_cls), {"B200_FAMILY": family})
 
 
@@ -232,7 +256,7 @@ def install(families: Optional[Sequence[str]] = None) -> Dict[str, type]:
     registry = importlib.import_module("simpletuner.helpers.models.registry").ModelRegistry
     out = {}
     for fam in (families or list(FAMILIES)):
-        spec = FAMILIES[fam]
+        spec = family_spec(fam)
         ref_cls = getattr(importlib.import_module(spec.reference_module), spec.reference_class)
         cls = make_b200_family(ref_cls, fam)
         registry.register(spec.registry_key, cls)
