@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -524,7 +525,8 @@ int stb_ln_modulate_bwd(const void* dy, long long dy_b, long long dy_s, const vo
                         float eps, void* stream) {
   if (int r = check_device()) return r;
   if ((D & 7) || D > 4096) return fail(STB_ERR_ARG, "D=%d must be a multiple of 8 and <= 4096", D);
-  if (!aligned16(x) || !aligned16(dy) || !aligned16(dx) || !aligned16(scale) || (add && !aligned16(add)))
+  if (!aligned16(x) || !aligned16(dy) || !aligned16(dx) || !aligned16(scale) || (add && !aligned16(add)) || (dy_b & 7) ||
+      (dy_s & 7) || (x_b & 7) || (x_s & 7) || (mod_b & 7) || (add && ((add_b & 7) || (add_s & 7))) || (dx_b & 7) || (dx_s & 7))
     return fail(STB_ERR_ARG, "ln_modulate_bwd alignment");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int rows = B * S;
@@ -547,6 +549,17 @@ int stb_ln_modulate_bwd(const void* dy, long long dy_b, long long dy_s, const vo
   return 0;
 }
 
+// The warp-per-token q/k kernels load and store HD / 32 consecutive bf16 per lane: 8 bytes at HD 128, 4 at HD 64.
+static bool qk_rows_aligned(int HD, std::initializer_list<const void*> ptrs, std::initializer_list<long long> strides) {
+  const uintptr_t pmask = HD == 128 ? 7 : 3;
+  const long long emask = HD == 128 ? 3 : 1;
+  for (const void* p : ptrs)
+    if (reinterpret_cast<uintptr_t>(p) & pmask) return false;
+  for (long long s : strides)
+    if (s & emask) return false;
+  return true;
+}
+
 int stb_qk_rmsnorm_rope_fwd(const void* src, long long src_b, long long src_s, int k_off, const void* wq,
                             const void* wk, const void* wq_added, const void* wk_added, int s_split,
                             const float* cos_t, const float* sin_t, void* q_out, void* k_out,
@@ -554,7 +567,7 @@ int stb_qk_rmsnorm_rope_fwd(const void* src, long long src_b, long long src_s, i
                             void* stream) {
   if (int r = check_device()) return r;
   if (HD != 128 && HD != 64) return fail(STB_ERR_UNSUPPORTED, "head_dim %d not supported", HD);
-  if ((src_s & 3) || (src_b & 3) || (k_off & 3) || (dst_s & 3) || (dst_b & 3)) return fail(STB_ERR_ARG, "qk_rmsnorm_rope alignment");
+  if (!qk_rows_aligned(HD, {src, q_out, k_out}, {src_s, src_b, k_off, dst_s, dst_b})) return fail(STB_ERR_ARG, "qk_rmsnorm_rope alignment");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long warps = (long long)B * S;  // one warp per token
   const unsigned grid = (unsigned)((warps + 7) / 8);
@@ -577,6 +590,8 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
                             int H, int HD, float eps, float* dw, void* stream) {
   if (int r = check_device()) return r;
   if (HD != 128 && HD != 64) return fail(STB_ERR_UNSUPPORTED, "head_dim %d not supported", HD);
+  if (!qk_rows_aligned(HD, {dq, dk, src, dsrc}, {d_b, d_s, src_b, src_s, k_off, ds_b, ds_s}))
+    return fail(STB_ERR_ARG, "qk_rmsnorm_rope_bwd alignment");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long warps = (long long)B * S;  // one warp per token
   const unsigned grid = (unsigned)((warps + 7) / 8);
