@@ -201,7 +201,7 @@ int set_smem(int bytes) {
 // decide how many pairs of SMs there are, so it is asked, once per kernel).
 template <int BN, int EPI, bool CONV, int CLUSTER = 1>
 int launch_gemm_kernel(const stb::GemmMaps& maps, const stb::GemmParams& p, cudaStream_t st, const char* name) {
-  using Cfg = stb::GemmCfg<BN>;
+  using Cfg = stb::GemmCfg<BN, stb::kGemmSmemEpi<BN, CONV>>;
   constexpr auto kernel = stb::gemm_bf16_tn_kernel<BN, EPI, CONV, CLUSTER>;
   if (int r = set_smem<kernel>(Cfg::SMEM_BYTES)) return r;
   const long long tiles_m = (long long)((p.rows_per_batch + Cfg::BM - 1) / Cfg::BM) * p.num_batches;
@@ -280,6 +280,21 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st, bool cluster) {
   p.aux = static_cast<__nv_bfloat16*>(a->aux);
   p.aux_batch_stride = a->aux_batch_stride;
   p.aux_row_stride = a->aux_row_stride;
+  if constexpr (stb::kGemmSmemEpi<BN, false>) {
+    // the shared-memory epilogue's maps: 64-column x 128-row boxes of D, of the [M, N] operand it reads and of the aux
+    // output.  stb_gemm_bf16's alignment rules for D, res and aux (16-byte bases, strides of 8 elements) are TMA's.
+    const bool reads_res = a->epi == stb::EPI_GATE_RES || a->epi == stb::EPI_ADD_RES;
+    const bool reads_aux = a->epi == stb::EPI_MUL_DGELU || a->epi == stb::EPI_MUL;
+    int r = make_token_map(&maps.d, a->d, a->N, a->rows_per_batch, a->num_batches, a->d_row_stride, a->d_batch_stride,
+                           128);
+    if (!r && reads_res)
+      r = make_token_map(&maps.x, a->res, a->N, a->rows_per_batch, a->num_batches, a->res_row_stride,
+                         a->res_batch_stride, 128);
+    if (!r && a->aux)
+      r = make_token_map(reads_aux ? &maps.x : &maps.aux, a->aux, a->N, a->rows_per_batch, a->num_batches,
+                         a->aux_row_stride, a->aux_batch_stride, 128);
+    if (r) return r;
+  }
   // the 2-CTA cluster kernels exist at BN 128 only
   auto go = [&](auto epi) -> int {
     constexpr int EPI = decltype(epi)::value;

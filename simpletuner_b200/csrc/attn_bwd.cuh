@@ -90,12 +90,6 @@ struct AttnBwdCfg {
   static constexpr int KB = 64 * 4;          // per stage (dQ kernel, BIAS): 64 keys x bias * log2(e)
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 
 // fp32 accumulator (64 x HD, wgmma layout) of this warpgroup -> shared-memory rows [64][HD + 4] (multiplied by `mul`)
 template <int HD>

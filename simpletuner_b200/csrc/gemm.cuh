@@ -10,8 +10,8 @@
 //
 // Roles (384 threads, three warpgroups): warpgroup 0 = TMA producer (one warp issues), warpgroups 1 and 2 =
 // consumers in ping-pong: each owns whole BM x BN tiles (the CTA's tiles alternate between them), runs wgmma
-// m64nBNk16 from shared memory over BM / 64 row blocks, then the fused epilogue straight from the accumulator
-// registers.  While one consumer is in its epilogue the other one's MMAs keep the tensor pipe busy, and the grid is
+// m64nBNk16 from shared memory over BM / 64 row blocks, then the fused epilogue (through a shared-memory buffer and TMA
+// at 128 x 128, straight from the accumulator registers otherwise).  While one consumer is in its epilogue the other one's MMAs keep the tensor pipe busy, and the grid is
 // persistent, so the producer streams the next tile's k-blocks meanwhile.  The epilogue kind is a template parameter.
 // CONV = true turns the A operand into the shifted NHWC window of a 3x3 convolution (implicit GEMM, VAE encoder).
 #pragma once
@@ -57,18 +57,30 @@ struct GemmParams {
 struct GemmMaps {
   CUtensorMap a[3];  // 3-D (k, s, b), box (64, BM, 1), SWIZZLE_128B
   CUtensorMap w[3];  // 2-D (k, n),   box (64, BN),      SWIZZLE_128B;  w_kn: 2-D (n, k), box (64, 64)
+  // shared-memory epilogue (kGemmSmemEpi): 3-D (n, s, b), box (64, 128, 1), SWIZZLE_128B, over D, the [M, N] operand the
+  // epilogue reads (res or aux) and the aux output of EPI_GELU / EPI_GATE_RES
+  CUtensorMap d, x, aux;
 };
 
-// A consumer's tile is BM x BN with 128 fp32 accumulators per thread at BN 128 and 256 (64 at BN 64).
-template <int BN>
+// 128 x 128 tiles of the plain GEMM stage the epilogue through shared memory (a TMA load of the operand, TMA stores of
+// the results); the other widths and CONV keep the epilogue from registers.
+template <int BN, bool CONV>
+constexpr bool kGemmSmemEpi = BN == 128 && !CONV;
+
+// A consumer's tile is BM x BN with 128 fp32 accumulators per thread at BN 128 and 256 (64 at BN 64).  SMEM_EPI: one
+// BM x BN bf16 epilogue buffer per consumer warpgroup, paid for with one ring stage (5 instead of 6 at 128 x 128).
+template <int BN, bool SMEM_EPI = false>
 struct GemmCfg {
   static constexpr int BM = BN == 256 ? 64 : 128;
   static constexpr int BK = 64;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int W_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
-  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*ring and order barriers*/;
+  static constexpr int EPI_BYTES = SMEM_EPI ? BM * BN * 2 : 0;
+  static constexpr int STAGES = SMEM_EPI ? 5 : (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
+  static constexpr int SMEM_BYTES =
+      STAGES * STAGE_BYTES + 2 * EPI_BYTES + 1024 /*align*/ + 256 /*ring, order and epilogue barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ float gemm_bf16r(float x) { return __bfloat162float(__float2bfloat16(x)); }
@@ -105,7 +117,7 @@ __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, bool two, float a, f
 }
 
 // The epilogues that read an [M, N] operand element for element: res (GATE_RES, ADD_RES) or aux (MUL_DGELU, MUL).
-// The epilogue loads those words ahead, a chunk of column groups at a time, so that their latencies overlap.
+// The register epilogue loads those words ahead, a chunk of column groups at a time, so that their latencies overlap.
 template <int EPI>
 constexpr bool kGemmEpiReadsRows = EPI == EPI_GATE_RES || EPI == EPI_ADD_RES || EPI == EPI_MUL_DGELU || EPI == EPI_MUL;
 template <int EPI>
@@ -116,25 +128,18 @@ __device__ __forceinline__ const __nv_bfloat16* gemm_epi_row_operand(const GemmP
     return p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride + n;
 }
 
-// Fused epilogue of two adjacent columns (n, n+1) of one output row; f = accumulator + bias, x = the pair's res / aux
-// word for the epilogues that read one.
+// Fused epilogue arithmetic of two adjacent columns of one output row: f = accumulator + bias in, D out; x = the pair's
+// res / aux word for the epilogues that read one, g = the pair's gate (EPI_GATE_RES).  The aux output of EPI_GELU /
+// EPI_GATE_RES is f itself, written by the caller.
 template <int EPI>
-__device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s, int n, bool two, float f0, float f1,
-                                              uint32_t x) {
-  const long long drow = (long long)b * p.d_batch_stride + (long long)s * p.d_row_stride;
-  __nv_bfloat16* xp = p.aux ? p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride + n : nullptr;
+__device__ __forceinline__ void gemm_epi_math(const GemmParams& p, float& f0, float& f1, float g0, float g1, uint32_t x) {
   if constexpr (EPI == EPI_GELU) {
-    if (xp) st_bf16x2(xp, two, f0, f1);
     // the activation sees the bf16-rounded pre-activation, as the reference's
     // nn.Linear -> nn.GELU chain does (bf16 tensor between the two modules)
     f0 = gelu_tanh(gemm_bf16r(f0));
     f1 = gelu_tanh(gemm_bf16r(f1));
   } else if constexpr (EPI == EPI_GATE_RES) {
-    float g0, g1;
-    ld_bf16x2(p.gate + (long long)b * p.gate_batch_stride + n, two, g0, g1);
     const float r0 = bf16_lo(x), r1 = bf16_hi(x);
-    // full fine-tune: keep the (bf16) linear output — the gate gradient is sum_s dOut * y
-    if (xp) st_bf16x2(xp, two, f0, f1);
     // reference order: bias -> (bf16 linear output) -> gate * y -> residual + (...)
     // (flux/transformer.py:464-465, 584-586, 652-653); each step is a bf16 tensor there.
     float o[2] = {r0 + gemm_bf16r(g0 * gemm_bf16r(f0)), r1 + gemm_bf16r(g1 * gemm_bf16r(f1))};
@@ -164,6 +169,20 @@ __device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s,
     f0 += bf16_lo(x);
     f1 += bf16_hi(x);
   }
+}
+
+// Register epilogue of one pair (n, n+1) of output row s, stored straight to global memory.
+template <int EPI>
+__device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int b, int s, int n, bool two, float f0, float f1,
+                                              uint32_t x) {
+  const long long drow = (long long)b * p.d_batch_stride + (long long)s * p.d_row_stride;
+  __nv_bfloat16* xp = p.aux ? p.aux + (long long)b * p.aux_batch_stride + (long long)s * p.aux_row_stride + n : nullptr;
+  float g0 = 0.f, g1 = 0.f;
+  if constexpr (EPI == EPI_GATE_RES) ld_bf16x2(p.gate + (long long)b * p.gate_batch_stride + n, two, g0, g1);
+  // full fine-tune (GATE_RES): keep the (bf16) linear output — the gate gradient is sum_s dOut * y
+  if constexpr (EPI == EPI_GELU || EPI == EPI_GATE_RES)
+    if (xp) st_bf16x2(xp, two, f0, f1);
+  gemm_epi_math<EPI>(p, f0, f1, g0, g1, x);
   st_bf16x2(p.D + drow + n, two, f0, f1);
 }
 
@@ -185,16 +204,21 @@ __device__ __forceinline__ void gemm_wgmma(float (&acc)[BN / 2], uint64_t a, uin
 template <int BN, int EPI, bool CONV = false, int CLUSTER = 1>
 __global__ void __launch_bounds__(384, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
-  using Cfg = GemmCfg<BN>;
+  constexpr bool SMEM_EPI = kGemmSmemEpi<BN, CONV>;
+  using Cfg = GemmCfg<BN, SMEM_EPI>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int MI = Cfg::BM / 64;   // m64 row blocks of a tile
   static_assert(CLUSTER == 1 || (CLUSTER == 2 && BN == 128 && !CONV), "2-CTA clusters: 128 x 128 GEMM tiles only");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  StageRing<STAGES> ring{smem_base + STAGES * Cfg::STAGE_BYTES};
+  // shared memory: the ring's stages, the consumers' epilogue buffers (SMEM_EPI), then the barriers
+  const uint32_t epi_smem = smem_base + STAGES * Cfg::STAGE_BYTES;
+  StageRing<STAGES> ring{epi_smem + 2 * Cfg::EPI_BYTES};
   // order[c]: consumer c may start its next mainloop (the other consumer has waited on every stage of the tile before)
   const uint32_t order_bars = ring.bars + 16u * STAGES;
+  // epi_full[c] (SMEM_EPI, epilogues that read an operand): the res / aux block of consumer c's tile is in its buffer
+  const uint32_t epi_full_bars = order_bars + 16u;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -217,9 +241,15 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       tma_prefetch_desc(&maps.a[s]);
       tma_prefetch_desc(&maps.w[s]);
     }
+    if constexpr (SMEM_EPI) {
+      tma_prefetch_desc(&maps.d);
+      if constexpr (kGemmEpiReadsRows<EPI>) tma_prefetch_desc(&maps.x);
+    }
     ring.init(4 * CLUSTER);   // each stage belongs to one consumer warpgroup's tile (in every CTA of the cluster)
     mbar_init(order_bars, 4);
     mbar_init(order_bars + 8, 4);
+    mbar_init(epi_full_bars, 1);
+    mbar_init(epi_full_bars + 8, 1);
     fence_mbar_init();
   }
   // no multicast or remote arrive may reach a CTA before its barriers exist
@@ -284,6 +314,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
     const int wq = warp & 3;             // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of each m64 block
     uint32_t order_phase = 0;
     if (cw == 1) ring.skip(nk);
+    uint32_t epi_phase = 0;   // SMEM_EPI: phase of this warpgroup's epi_full barrier
     float acc[MI][BN / 2];
     for (int unit = unit0 + cw * units_stride; unit < num_units; unit += 2 * units_stride) {
       // The other consumer has waited on every stage of the tile before this one, so the producer has filled them all
@@ -334,6 +365,19 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
             if constexpr (CLUSTER == 2) ring.release_cluster(prev_stage, rank ^ 1u);
             else ring.release(prev_stage);
           }
+          if constexpr (SMEM_EPI && kGemmEpiReadsRows<EPI>) {
+            // the tile's res / aux block, two 64-column boxes (past the N, row or batch end TMA fills zeros), loaded by
+            // the warpgroup's first thread a few k-blocks into the mainloop, when the previous tile's stores have long
+            // read the buffer
+            if (seg == 0 && kb == min(3, p.kblocks[0] - 1) && (threadIdx.x & 127) == 0) {
+              const uint32_t ebuf = epi_smem + cw * Cfg::EPI_BYTES, epi_full = epi_full_bars + 8u * cw;
+              tma_store_wait_read<0>();   // the previous tile's stores have read the buffer
+              mbar_arrive_expect_tx(epi_full, Cfg::EPI_BYTES);
+              tma_load_3d(ebuf, &maps.x, epi_full, n0, s0, b);
+              tma_load_3d(ebuf + Cfg::EPI_BYTES / 2, &maps.x, epi_full, n0 + 64, s0, b);
+            }
+            __syncwarp();
+          }
           prev_stage = ring.stage;
           ring.advance();
         }
@@ -347,11 +391,86 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
       if constexpr (CLUSTER == 2) ring.release_cluster(prev_stage, rank ^ 1u);
       else ring.release(prev_stage);
 
-      // ===================== epilogue from registers =====================
       // accumulator layout (m64nBN): acc[mi][4 i + 2 h + j] = row 64 mi + 16 wq + lane / 4 + 8 h,
       // column 8 i + 2 (lane % 4) + j
-      constexpr int CH = BN / 8 < 8 ? BN / 8 : 8;   // column groups whose res / aux words are loaded together
       const bool b_ok = b < p.num_batches;
+      if constexpr (SMEM_EPI) {
+        // ===================== epilogue through shared memory =====================
+        // The buffer holds the tile as two 64-column halves of 128 rows x 128 B in TMA's SWIZZLE_128B layout: the 16-byte
+        // chunk c of row r sits at chunk position c ^ (r % 8).  Column 8 i + 2 (lane % 4) of row r is then at half i / 8,
+        // chunk (i % 8) ^ (lane / 4), byte 4 (lane % 4), and a warp's 8 rows x 4 words of one column group hit all 32
+        // banks once.  Every thread reads (res / aux) and writes (D, then aux) only its own words; the TMA stores clip
+        // the tile at the N, row and batch ends, so tail elements are computed but never leave shared memory.  The
+        // warpgroup's first thread issues the stores.
+        const uint32_t ebuf = epi_smem + cw * Cfg::EPI_BYTES;
+        const bool epi_leader = (threadIdx.x & 127) == 0;
+        const uint32_t wrow = ebuf + (wq * 16 + (lane >> 2)) * 128 + 4 * (lane & 3);
+        // fill(false): the epilogue's D over the buffer; fill(true): the aux output acc + bias
+        auto fill = [&](auto aux_pass) {
+          constexpr bool AUX = decltype(aux_pass)::value;
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i) {
+            const int n = n0 + 8 * i + 2 * (lane & 3);
+            const bool col_ok = n < p.N && b_ok;
+            const bool two = n + 1 < p.N;
+            float b0 = 0.f, b1 = 0.f, g0 = 0.f, g1 = 0.f;
+            if (p.bias && col_ok) ld_bf16x2(p.bias + n, two, b0, b1);
+            if constexpr (EPI == EPI_GATE_RES && !AUX)
+              if (col_ok) ld_bf16x2(p.gate + (long long)b * p.gate_batch_stride + n, two, g0, g1);
+            const uint32_t wcol = wrow + (i >> 3) * (Cfg::EPI_BYTES / 2) + (((i & 7) ^ (lane >> 2)) << 4);
+#pragma unroll
+            for (int mi = 0; mi < MI; ++mi)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t w = wcol + (mi * 64 + 8 * h) * 128;
+                float f0 = acc[mi][4 * i + 2 * h] + b0, f1 = acc[mi][4 * i + 2 * h + 1] + b1;
+                if constexpr (!AUX) gemm_epi_math<EPI>(p, f0, f1, g0, g1, kGemmEpiReadsRows<EPI> ? ld_shared_u32(w) : 0u);
+                st_shared_u32(w, pack_bf16x2(f0, f1));
+              }
+          }
+        };
+        // the buffer's words -> global: every thread's writes made visible to the async proxy, then one thread stores
+        auto store = [&](const CUtensorMap* m) {
+          fence_proxy_async_smem();
+          named_bar_sync(1 + cw, 128);
+          if (epi_leader && b_ok) {
+            tma_store_3d(m, ebuf, n0, s0, b);
+            tma_store_3d(m, ebuf + Cfg::EPI_BYTES / 2, n0 + 64, s0, b);
+            tma_store_commit();
+          }
+        };
+        // before the buffer is written again: the stores issued from it have read it
+        auto reuse = [&]() {
+          if (epi_leader) tma_store_wait_read<0>();
+          named_bar_sync(1 + cw, 128);
+        };
+        if constexpr (kGemmEpiReadsRows<EPI>) {
+          mbar_wait(epi_full_bars + 8u * cw, epi_phase, 5);
+          epi_phase ^= 1u;
+        } else {
+          reuse();
+        }
+        // GELU's aux output (the pre-activation) goes first; GATE_RES's after D, which is computed over the res it reads
+        if constexpr (EPI == EPI_GELU)
+          if (p.aux) {
+            fill(std::true_type{});
+            store(&maps.aux);
+            reuse();
+          }
+        fill(std::false_type{});
+        store(&maps.d);
+        if constexpr (EPI == EPI_GATE_RES)
+          if (p.aux) {
+            reuse();
+            fill(std::true_type{});
+            store(&maps.aux);
+          }
+        __syncwarp();
+        continue;   // next tile
+      }
+
+      // ===================== epilogue from registers =====================
+      constexpr int CH = BN / 8 < 8 ? BN / 8 : 8;   // column groups whose res / aux words are loaded together
 #pragma unroll
       for (int mi = 0; mi < MI; ++mi) {
         const int r_lo = s0 + mi * 64 + wq * 16 + (lane >> 2);
@@ -389,6 +508,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
         }
       }
     }
+    // the last tile's stores have completed before the CTA's shared memory goes away
+    if constexpr (SMEM_EPI)
+      if ((threadIdx.x & 127) == 0) tma_store_wait<0>();
   }
   // the peer may still multicast into this CTA's stages or arrive on its empty barriers until it is done too
   if constexpr (CLUSTER == 2) cluster_sync();
