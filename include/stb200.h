@@ -48,7 +48,9 @@ enum stb_gemm_epilogue {
   STB_EPI_ADD_RES = 4,   /* D = acc + bias + res                                               */
   STB_EPI_MUL = 5,       /* D = bf16(acc + bias) * aux[b, s, n]  (aux read) — T5 gated-GELU feed-forward, transformers
                             T5DenseGatedActDense (called through flux/pipeline.py:1085)             */
-  STB_EPI_QUICK_GELU = 6 /* D = y * sigmoid(1.702 y), y = bf16(acc + bias) — CLIP text MLP (flux/pipeline.py:1127) */
+  STB_EPI_QUICK_GELU = 6, /* D = y * sigmoid(1.702 y), y = bf16(acc + bias) — CLIP text MLP (flux/pipeline.py:1127) */
+  STB_EPI_SILU = 7        /* D = y * sigmoid(y), y = bf16(acc + bias) — Chroma approximator layers, PixArtAlphaTextProjection
+                             with act_fn "silu" (chroma/transformer.py:297-313)                                       */
 };
 
 typedef struct {
@@ -107,6 +109,13 @@ typedef struct {
   const void* bias;
   long long bias_h, bias_q;
   long long bias_b;
+  /* optional, per-key bias only: its live list, int32 rows kv_live_b elements apart (0 = one row for the batch), each
+   * {n_live, the indices of the n_live live 128-key tiles in ascending order padded to n_tiles slots, one 0/1 live flag
+   * per tile}, n_tiles = ceil(Sk / 128).  A tile is dead when the bias of every key in it is -inf (past Sk counts as
+   * -inf).  The kernels then skip the dead tiles, with the same results; a row with no live tile is outside the contract
+   * above.  NULL = process every tile.  Built on the device by simpletuner_b200.ops.key_bias_live_list. */
+  const int* kv_live;
+  long long kv_live_b;
 } stb_attn_fwd_args;
 int stb_attn_fwd(const stb_attn_fwd_args* args, void* stream);
 
@@ -141,6 +150,10 @@ typedef struct {
    * returns STB_ERR_UNSUPPORTED.  Keys whose bias is -inf get dk = dv = 0. */
   const void* bias;
   long long bias_b;
+  /* optional: the forward's live list (stb_attn_fwd_args.kv_live).  dk = dv = 0 is written for the keys of dead tiles
+   * without computing them, and dq iterates over the live tiles only.  NULL = process every tile. */
+  const int* kv_live;
+  long long kv_live_b;
 } stb_attn_bwd_args;
 int stb_attn_bwd(const stb_attn_bwd_args* args, void* stream);
 

@@ -87,6 +87,7 @@ class AttnFwdArgs(C.Structure):
         ("lse", C.c_void_p),
         ("bias", C.c_void_p), ("bias_h", C.c_longlong), ("bias_q", C.c_longlong),
         ("bias_b", C.c_longlong),
+        ("kv_live", C.c_void_p), ("kv_live_b", C.c_longlong),
     ]
 
 
@@ -115,6 +116,7 @@ class AttnBwdArgs(C.Structure):
         ("dv_b", C.c_longlong), ("dv_s", C.c_longlong), ("dv_h", C.c_longlong),
         ("qk_prep", C.POINTER(QkPrep)),
         ("bias", C.c_void_p), ("bias_b", C.c_longlong),
+        ("kv_live", C.c_void_p), ("kv_live_b", C.c_longlong),
     ]
 
 

@@ -310,6 +310,7 @@ int launch_gemm(const stb_gemm_args* a, cudaStream_t st, bool cluster) {
     case stb::EPI_ADD_RES: return go(std::integral_constant<int, stb::EPI_ADD_RES>{});
     case stb::EPI_MUL: return go(std::integral_constant<int, stb::EPI_MUL>{});
     case stb::EPI_QUICK_GELU: return go(std::integral_constant<int, stb::EPI_QUICK_GELU>{});
+    case stb::EPI_SILU: return go(std::integral_constant<int, stb::EPI_SILU>{});
   }
   return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
 }
@@ -385,7 +386,7 @@ int stb_gemm_bf16(const stb_gemm_args* a, void* stream) {
   if ((a->epi == STB_EPI_MUL_DGELU || a->epi == STB_EPI_MUL) && !a->aux) return fail(STB_ERR_ARG, "MUL_DGELU / MUL need aux");
   if (a->aux && (!aligned16(a->aux) || (a->aux_row_stride & 7) || (a->aux_batch_stride & 7)))
     return fail(STB_ERR_ARG, "aux must be 16-byte aligned, strides multiple of 8");
-  if (a->epi < 0 || a->epi > 6) return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
+  if (a->epi < 0 || a->epi > STB_EPI_SILU) return fail(STB_ERR_ARG, "unknown epilogue %d", a->epi);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // a tile's height follows from its width (GemmCfg: 64 x 256, 128 x 128, 128 x 64); tile_mt = 1 / 2 forces single CTAs /
   // 2-CTA clusters at BN 128, the only width that has the cluster kernel
@@ -431,7 +432,11 @@ int stb_attn_fwd(const stb_attn_fwd_args* a, void* stream) {
   p.bias = static_cast<const __nv_bfloat16*>(a->bias);
   p.bias_b = a->bias_b; p.bias_h = a->bias_h; p.bias_q = a->bias_q;
   p.inv_scale = a->scale != 0.f ? 1.f / a->scale : 0.f;
+  p.kv_live = a->kv_live;
+  p.kv_live_b = a->kv_live_b;
   const dim3 grid((a->Sq + 127) / 128, a->H, a->B);
+  if (a->kv_live && (!a->bias || a->bias_q != 0 || a->bias_h != 0 || a->kv_live_b < 0))
+    return fail(STB_ERR_ARG, "attn_fwd kv_live: only with a per-key bias (bias_q = bias_h = 0), kv_live_b >= 0");
   if (a->bias) {   // additive bias / mask: text encoders, and the per-key bias of Flux masked training
     const bool key_row = a->bias_q == 0 && a->bias_h == 0;
     if (a->scale == 0.f || a->bias_b < 0 || a->bias_h < 0 || (a->bias_q < a->Sk && !key_row))
@@ -498,6 +503,10 @@ int stb_attn_bwd(const stb_attn_bwd_args* a, void* stream) {
   p.do_b = a->do_b; p.do_s = a->do_s; p.do_h = a->do_h;
   p.bias = static_cast<const __nv_bfloat16*>(a->bias);
   p.bias_b = a->bias_b;
+  p.kv_live = a->kv_live;
+  p.kv_live_b = a->kv_live_b;
+  if (a->kv_live && (!a->bias || a->kv_live_b < 0))
+    return fail(STB_ERR_ARG, "attn_bwd kv_live: only with a per-key bias, kv_live_b >= 0");
   if (a->bias) {   // per-key only: [B, Sk] rows bias_b apart, or one row shared by the batch (bias_b = 0)
     if (a->bias_b < 0 || (a->bias_b != 0 && a->bias_b < a->Sk))
       return fail(STB_ERR_UNSUPPORTED, "attn_bwd bias: only a per-key bias [B or 1, Sk] (bias_b = 0 or >= Sk) is supported");

@@ -45,6 +45,10 @@ struct AttnBwdParams {
   // BIAS instantiations only: the forward's per-key logit bias, bias[b * bias_b + sk] (bf16, -inf = masked key)
   const __nv_bfloat16* bias;
   long long bias_b;
+  // BIAS instantiations only, optional: the bias's live list (attn_fwd.cuh, kv_tile_at), rows kv_live_b apart.  The
+  // dK/dV kernel writes zeros for a 64-key tile inside a dead 128-key tile; the dQ kernel iterates over live tiles only.
+  const int* kv_live;
+  long long kv_live_b;
 };
 
 struct AttnBwdMaps {
@@ -232,6 +236,19 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
   const int kv0 = blockIdx.x * 64, h = blockIdx.y, b = blockIdx.z;
   const int n_q = (p.Sq + 63) / 64;
+  if constexpr (BIAS) {
+    // every key of a dead tile has P^T = 0, so its dK and dV are 0: write them without loading anything
+    if (p.kv_live && p.kv_live[(long long)b * p.kv_live_b + 1 + (p.Sk + 127) / 128 + (kv0 >> 7)] == 0) {
+      for (int i = threadIdx.x; i < 64 * (HD / 2); i += blockDim.x) {
+        const int kv = kv0 + i / (HD / 2), c = 2 * (i % (HD / 2));
+        if (kv < p.Sk) {
+          *reinterpret_cast<uint32_t*>(p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h + c) = 0u;
+          *reinterpret_cast<uint32_t*>(p.dv + (long long)b * p.dv_b + (long long)kv * p.dv_s + (long long)h * p.dv_h + c) = 0u;
+        }
+      }
+      return;
+    }
+  }
 
   if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
@@ -433,7 +450,17 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);   // warp-uniform for the compiler (wgmma needs converged warpgroups)
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
-  const int n_kv = (p.Sk + 63) / 64;
+  int n_kv = (p.Sk + 63) / 64;
+  const int* live = nullptr;   // BIAS with a live list: the 64-key halves of the live 128-key tiles only
+  if constexpr (BIAS) {
+    if (p.kv_live) {
+      live = p.kv_live + (long long)b * p.kv_live_b;
+      const int n_live = live[0];
+      // the last live tile may be the tail tile with a single 64-key half
+      n_kv = n_live > 0 ? 2 * n_live - (2 * live[n_live] + 1 >= n_kv ? 1 : 0) : 0;
+    }
+  }
+  auto tile64 = [&](int t) { return live ? 2 * live[1 + (t >> 1)] + (t & 1) : t; };
 
   if (threadIdx.x == 0) {
     mbar_init(qd_full, 1);
@@ -456,9 +483,10 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
         }
       }
       __syncwarp();
-      for (int j = 0; j < n_kv; ++j) {
-        const int stg = j % Cfg::STAGES;
-        mbar_wait(s_empty(stg), ((j / Cfg::STAGES) & 1) ^ 1u, 50);
+      for (int t = 0; t < n_kv; ++t) {
+        const int j = tile64(t);
+        const int stg = t % Cfg::STAGES;
+        mbar_wait(s_empty(stg), ((t / Cfg::STAGES) & 1) ^ 1u, 50);
         if (elect_one()) {
           mbar_arrive_expect_tx(s_full(stg), 2 * Cfg::SMALL);
           for (int a = 0; a < ATOMS; ++a) {
@@ -498,18 +526,19 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
     // fragments stay live until then, so dP is issued only after it: all of them together exceed the 168 registers of
     // a 384-thread CTA); exp(S) runs while dP is on the tensor pipe.  A stage goes back to the producer once the dQ MMA
     // reading its K has retired.
-    for (int j = 0; j < n_kv; ++j) {
-      const int stg = j % Cfg::STAGES;
-      mbar_wait(s_full(stg), (j / Cfg::STAGES) & 1, 52);
+    for (int t = 0; t < n_kv; ++t) {
+      const int j = tile64(t);
+      const int stg = t % Cfg::STAGES;
+      mbar_wait(s_full(stg), (t / Cfg::STAGES) & 1, 52);
       const uint32_t ka = k_smem + stg * Cfg::SMALL, va = v_smem + stg * Cfg::SMALL;
       float sc[32], dp[32];
       wg_fence();
       mma_kmajor_n64<HD>(sc, q_smem + cw * 8192, BIG_ATOM, ka, SMALL_ATOM);    // S  = Q K^T
       wg_commit();
       wg_wait<1>();   // the previous tile's dQ
-      if (j > 0) {
+      if (t > 0) {
         __syncwarp();
-        if (lane == 0) mbar_arrive(s_empty((j - 1) % Cfg::STAGES));
+        if (lane == 0) mbar_arrive(s_empty((t - 1) % Cfg::STAGES));
       }
       mma_kmajor_n64<HD>(dp, do_smem + cw * 8192, BIG_ATOM, va, SMALL_ATOM);   // dP = dO V^T
       wg_commit();
@@ -539,7 +568,7 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
       for (int kk = 0; kk < 4; ++kk) {   // 64 keys / 16
         uint32_t a[4];
         acc_to_afrag(dp, kk, a);
-        wgmma_rs_mn<HD>(dq_acc, a, sdesc_mn(ka, kk * 2048, SMALL_ATOM), (j > 0 || kk > 0) ? 1u : 0u);
+        wgmma_rs_mn<HD>(dq_acc, a, sdesc_mn(ka, kk * 2048, SMALL_ATOM), (t > 0 || kk > 0) ? 1u : 0u);
       }
       wg_commit();
     }

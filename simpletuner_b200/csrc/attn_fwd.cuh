@@ -28,7 +28,17 @@ struct AttnFwdParams {
   long long bias_h, bias_q;
   float inv_scale;
   long long bias_b;
+  // KEY instantiation only, optional: the live list of the per-key bias (kv_live_row): row b at kv_live + b * kv_live_b
+  // holds {n_live, the n_live live 128-key tile indices in ascending order, ...}.  Null: every tile is processed.
+  const int* kv_live;
+  long long kv_live_b;
 };
+
+// Live list of a per-key bias, one row per bias row: [n_live, live tile indices ascending (n_tiles slots, the first
+// n_live used), live flag per tile (n_tiles)], n_tiles = ceil(Sk / 128).  A 128-key tile is dead when every key of it
+// has bias -inf (the padding past Sk counts as -inf).  Skipping a dead tile gives the bits of processing it: its keys
+// have p = 0, which adds nothing to l or O, and the row max either stays (alpha = 1) or stays -inf (alpha = 0).
+__device__ __forceinline__ int kv_tile_at(const int* live, int t) { return live ? live[1 + t] : t; }
 
 struct AttnFwdMaps {
   CUtensorMap q, k, v;  // 4-D (d, h, s, b), box (64, 1, 128, 1), SWIZZLE_128B
@@ -93,7 +103,14 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
   const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
-  const int n_kv = (p.Sk + 127) / 128;
+  int n_kv = (p.Sk + 127) / 128;
+  const int* live = nullptr;   // KEY with a live list: iterate over the live tiles only
+  if constexpr (KEY) {
+    if (p.kv_live) {
+      live = p.kv_live + (long long)b * p.kv_live_b;
+      n_kv = live[0];
+    }
+  }
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&maps.q);
@@ -123,9 +140,10 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
         for (int a = 0; a < ATOMS; ++a) tma_load_4d(q_smem + a * ATOM_BYTES, &maps.q, q_full, a * 64, h, q0, b);
       }
       __syncwarp();
-      for (int j = 0; j < n_kv; ++j) {
-        const int stg = j % NSTG;
-        const uint32_t par = ((j / NSTG) & 1) ^ 1u;
+      for (int t = 0; t < n_kv; ++t) {
+        const int j = kv_tile_at(live, t);
+        const int stg = t % NSTG;
+        const uint32_t par = ((t / NSTG) & 1) ^ 1u;
         mbar_wait(k_empty(stg), par, 10);
         if (elect_one()) {
           mbar_arrive_expect_tx(k_full(stg), TILE);
@@ -173,9 +191,10 @@ attn_fwd_kernel(const __grid_constant__ AttnFwdMaps maps, const AttnFwdParams p)
     const uint32_t qa = q_smem + cw * 8192;
     mbar_wait(q_full, 0, 20);
 
-    for (int j = 0; j < n_kv; ++j) {
-      const int stg = j % NSTG;
-      const uint32_t par = (j / NSTG) & 1;
+    for (int t = 0; t < n_kv; ++t) {
+      const int j = kv_tile_at(live, t);
+      const int stg = t % NSTG;
+      const uint32_t par = (t / NSTG) & 1;
       // ---- S = Q K^T
       mbar_wait(k_full(stg), par, 21);
       const uint32_t ka = k_smem + stg * TILE;

@@ -28,6 +28,7 @@ enum GemmEpi : int {
   EPI_ADD_RES = 4,      // D = acc + bias + res                (gradient accumulation; residual add of the text encoders)
   EPI_MUL = 5,          // D = (acc + bias) * aux              (T5 gated feed-forward: gelu(x wi_0) * (x wi_1))
   EPI_QUICK_GELU = 6,   // D = y * sigmoid(1.702 y), y = bf16(acc + bias)   (CLIP text model activation)
+  EPI_SILU = 7,         // D = y * sigmoid(y), y = bf16(acc + bias)           (Chroma approximator: nn.Linear -> SiLU)
 };
 
 struct GemmParams {
@@ -165,6 +166,10 @@ __device__ __forceinline__ void gemm_epi_math(const GemmParams& p, float& f0, fl
     const float y0 = gemm_bf16r(f0), y1 = gemm_bf16r(f1);
     f0 = y0 / (1.f + __expf(-1.702f * y0));
     f1 = y1 / (1.f + __expf(-1.702f * y1));
+  } else if constexpr (EPI == EPI_SILU) {
+    const float y0 = gemm_bf16r(f0), y1 = gemm_bf16r(f1);
+    f0 = y0 / (1.f + __expf(-y0));
+    f1 = y1 / (1.f + __expf(-y1));
   } else if constexpr (EPI == EPI_ADD_RES) {
     f0 += bf16_lo(x);
     f1 += bf16_hi(x);

@@ -204,7 +204,7 @@ class Flux:
         if getattr(self, "_sigma_sampler", None) is None:   # keeps the round-robin cursor of custom timestep lists
             from ..training.schedule import FlowSigmaSampler
             self._sigma_sampler = FlowSigmaSampler(c, self.noise_schedule, dev)
-        sigmas, timesteps = self._sigma_sampler.sample(bsz, noise, state)
+        sigmas, timesteps = self._model_sigmas(*self._sigma_sampler.sample(bsz, noise, state), batch["latents"])
         batch["timesteps"] = timesteps
         batch["sigmas"] = sigmas.view(-1, 1, 1, 1)  # expand_sigmas, common.py:6825-6828
         # MixFlow (common.py:4962-4991): the model sees `sigmas`, the interpolation uses the slowed-down
@@ -246,6 +246,11 @@ class Flux:
         batch["conditioning_packed_latents"] = joint[:, S_scene:]
         batch["conditioning_ids"] = ids.to(dev, torch.bfloat16)[None].expand(bsz, -1, -1)   # the reference's dtype
         return batch
+
+    def _model_sigmas(self, sigmas: torch.Tensor, timesteps: torch.Tensor, latents: torch.Tensor):
+        """(sigmas, timesteps) the step trains at, from the sampler's draw: Flux trains at the drawn values (Chroma
+        remaps them)."""
+        return sigmas, timesteps
 
     def _kontext_conditions(self, batch: Dict[str, Any], state: Dict[str, Any]):
         """Flux.prepare_batch_conditions (flux/model.py:522-555) then the base class's list collapse (common.py:4668-4683).

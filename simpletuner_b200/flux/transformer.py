@@ -336,16 +336,21 @@ class FluxSingleTransformerBlock(nn.Module):
 
     def forward(self, h, silu_temb, cos, sin, lora_scaling, key_bias=None, segs=None):
         """segs (Flux Kontext): (text, scene, conditioning) token counts; silu_temb then holds those rows [3B, D]."""
-        mod = self.norm.linear(silu_temb)
-        st = {"H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "lora_drop": getattr(self, "_lora_drop", None), "key_bias": key_bias, "segs": segs}
-        a = self.attn
-        lora = _lora_list([a.to_q, a.to_k, a.to_v])
-        st["lokr_scales"] = _lokr_scales([a.to_q, a.to_k, a.to_v])
-        mlp = _lora_list([self.proj_mlp, self.proj_out])
-        if any(t is not None for t in mlp):
-            lora = lora + mlp
-        return SingleBlockFn.apply(h, mod, cos, sin, st, *lora)
+        return run_single_block(self, h, self.norm.linear(silu_temb), cos, sin, lora_scaling, key_bias, segs)
+
+
+def run_single_block(blk, h, mod, cos, sin, lora_scaling, key_bias, segs):
+    """SingleBlockFn over one single-stream block with its modulation rows `mod` [B, 3D] (shift | scale | gate); shared by
+    the Flux and Chroma single blocks."""
+    st = {"H": blk.heads, "hd": blk.head_dim, "plans": blk.plans(), "lora_scaling": lora_scaling,
+          "lora_drop": getattr(blk, "_lora_drop", None), "key_bias": key_bias, "segs": segs}
+    a = blk.attn
+    lora = _lora_list([a.to_q, a.to_k, a.to_v])
+    st["lokr_scales"] = _lokr_scales([a.to_q, a.to_k, a.to_v])
+    mlp = _lora_list([blk.proj_mlp, blk.proj_out])
+    if any(t is not None for t in mlp):
+        lora = lora + mlp
+    return SingleBlockFn.apply(h, mod, cos, sin, st, *lora)
 
 
 class _TimestepEmbedding(nn.Module):
@@ -655,6 +660,28 @@ class FluxTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, 
             self._rope_cache[key] = hit
         return hit
 
+    def _embed_image(self, x: torch.Tensor, out: torch.Tensor) -> None:
+        """out (the image rows of the joint buffer) = x_embedder(x), with its LoRA adapter when one is attached."""
+        xa, xb = self.x_embedder.lora_tensors()
+        if xa is None or not torch.is_grad_enabled():
+            ops.gemm([x.contiguous()], [self.x_embedder.weight], self.x_embedder.bias, out=out)
+            if xa is not None:          # inference with the adapter attached
+                out += F.linear(F.linear(x, xa), xb) * self._lora_scaling
+        else:
+            y = LoraLinearFn.apply(x.contiguous(), self.x_embedder.weight, self.x_embedder.bias,
+                                   self._lora_scaling, getattr(self.x_embedder, "_lora_drop", None), xa, xb)
+            out.copy_(y)                # autograd routes the image rows of dh to the adapter
+
+    def _tail(self, h, mod, S_txt: int, S_end: int, scaling: float) -> torch.Tensor:
+        """norm_out (mod [B, 2D] = scale | shift) and proj_out over the image rows [S_txt, S_end) of the joint buffer."""
+        if self._tail_plan is None:
+            self._tail_plan = {"w_proj": self.proj_out.weight.detach(), "b_proj": self.proj_out.bias.detach(),
+                               "w_proj_t": _wt(self.proj_out.weight.detach())}
+        pa, pb = self.proj_out.lora_tensors()
+        tail_lora = () if pa is None else (pa, pb)
+        return TailFn.apply(h, mod, {"S_txt": S_txt, "S_end": S_end, "lora_scaling": scaling,
+                                     "lora_drop": getattr(self.proj_out, "_lora_drop", None), **self._tail_plan}, *tail_lora)
+
     def _temb(self, timestep, guidance, pooled):
         tte = self.time_text_embed
         dt = pooled.dtype
@@ -700,15 +727,7 @@ class FluxTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, 
         h = torch.empty((B, S_txt + S_img, D), device=dev, dtype=dt)
         blocks = list(self.transformer_blocks) + list(self.single_transformer_blocks)
         self._begin_lora_dropout(blocks + [self.proj_out, self.x_embedder])      # one mask-stream slot each
-        xa, xb = self.x_embedder.lora_tensors()
-        if xa is None or not torch.is_grad_enabled():
-            ops.gemm([hidden_states.to(dt).contiguous()], [self.x_embedder.weight], self.x_embedder.bias, out=h[:, S_txt:])
-            if xa is not None:          # inference with the adapter attached
-                h[:, S_txt:] += F.linear(F.linear(hidden_states.to(dt), xa), xb) * self._lora_scaling
-        else:
-            y = LoraLinearFn.apply(hidden_states.to(dt).contiguous(), self.x_embedder.weight, self.x_embedder.bias,
-                                   self._lora_scaling, getattr(self.x_embedder, "_lora_drop", None), xa, xb)
-            h[:, S_txt:].copy_(y)       # autograd routes the image rows of dh to the adapter
+        self._embed_image(hidden_states.to(dt), h[:, S_txt:])
         ops.gemm([encoder_hidden_states.to(dt).contiguous()], [self.context_embedder.weight], self.context_embedder.bias,
                  out=h[:, :S_txt])
         # reference :1003-1007 — timestep / guidance arrive in [0,1] and are scaled by 1000 here
@@ -745,14 +764,8 @@ class FluxTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, 
             h = self._run_block(i, blk, h, silu_temb, cos, sin, S_txt, scaling, key_bias, img_segs)
         for i, blk in enumerate(self.single_transformer_blocks):
             h = self._run_block(i, blk, h, silu_temb, cos, sin, scaling, key_bias, single_segs)
-        if self._tail_plan is None:
-            self._tail_plan = {"w_proj": self.proj_out.weight.detach(), "b_proj": self.proj_out.bias.detach(),
-                               "w_proj_t": _wt(self.proj_out.weight.detach())}
         mod = self.norm_out.linear(silu_temb[B:2 * B] if S_c else silu_temb)     # norm_out uses temb_img: the scene rows
-        pa, pb = self.proj_out.lora_tensors()
-        tail_lora = () if pa is None else (pa, pb)
-        out = TailFn.apply(h, mod, {"S_txt": S_txt, "S_end": S_txt + S_scene, "lora_scaling": scaling, "lora_drop": getattr(self.proj_out, "_lora_drop", None),
-                                    **self._tail_plan}, *tail_lora)
+        out = self._tail(h, mod, S_txt, S_txt + S_scene, scaling)
         if not return_dict:
             return (out,)
         return SimpleNamespace(sample=out)

@@ -16,7 +16,7 @@ import torch
 from . import _lib
 from ._lib import QkPrep, AttnBwdArgs, AttnFwdArgs, GemmArgs, check
 
-EPI_STORE, EPI_GELU, EPI_GATE_RES, EPI_MUL_DGELU, EPI_ADD_RES, EPI_MUL, EPI_QUICK_GELU = 0, 1, 2, 3, 4, 5, 6
+EPI_STORE, EPI_GELU, EPI_GATE_RES, EPI_MUL_DGELU, EPI_ADD_RES, EPI_MUL, EPI_QUICK_GELU, EPI_SILU = 0, 1, 2, 3, 4, 5, 6, 7
 
 
 def _stream() -> int:
@@ -144,6 +144,38 @@ def _key_bias_stride(key_bias: torch.Tensor, B: int, Sk: int) -> int:
     return 0 if key_bias.shape[0] == 1 else key_bias.stride(0)
 
 
+def key_bias_live_list(key_bias: torch.Tensor) -> torch.Tensor:
+    """The live list of a per-key bias [B or 1, Sk] (stb_attn_fwd_args.kv_live): int32 [B or 1, 1 + 2 n_tiles], each row
+    {number of live 128-key tiles, their indices ascending (padded with the dead ones), a 0/1 live flag per tile}.  A tile
+    is dead when every key of it has bias -inf.  Device ops only: no host synchronisation, CUDA-graph capturable."""
+    Bb, Sk = key_bias.shape
+    n = (Sk + 127) // 128
+    dead_key = torch.isneginf(key_bias)
+    if n * 128 != Sk:
+        dead_key = torch.nn.functional.pad(dead_key, (0, n * 128 - Sk), value=True)
+    live = ~dead_key.view(Bb, n, 128).all(dim=2)
+    out = torch.empty((Bb, 1 + 2 * n), device=key_bias.device, dtype=torch.int32)
+    out[:, 0] = live.sum(dim=1)
+    out[:, 1:1 + n] = torch.argsort((~live).to(torch.uint8), dim=1, stable=True)
+    out[:, 1 + n:] = live
+    return out
+
+
+def _key_live(key_bias: torch.Tensor) -> torch.Tensor:
+    """key_bias_live_list(key_bias), built once per bias tensor and kept on it: every attention of a step that reads the
+    same bias (all blocks, forward and backward, and the re-runs of gradient checkpointing) shares one list."""
+    hit = getattr(key_bias, "_stb_kv_live", None)
+    if hit is None or hit[0] != key_bias._version:
+        hit = (key_bias._version, key_bias_live_list(key_bias))
+        key_bias._stb_kv_live = hit
+    return hit[1]
+
+
+def _set_live(a, live: Optional[torch.Tensor]) -> None:
+    if live is not None:
+        a.kv_live, a.kv_live_b = live.data_ptr(), (0 if live.shape[0] == 1 else live.stride(0))
+
+
 def attn_fwd(q, k, v, scale: Optional[float] = None, out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None,
              key_bias: Optional[torch.Tensor] = None):
     """q/k/v: [B, S, H, HD] views (HD contiguous).  Returns (o [B,Sq,H,HD] bf16, lse [B,H,Sq] fp32).
@@ -175,6 +207,7 @@ def attn_fwd(q, k, v, scale: Optional[float] = None, out: Optional[torch.Tensor]
         a.bias, a.bias_h, a.bias_q = bias.data_ptr(), (0 if bias.shape[0] == 1 else bias.stride(0)), bias.stride(1)
     if key_bias is not None:
         a.bias, a.bias_b, a.bias_h, a.bias_q = key_bias.data_ptr(), _key_bias_stride(key_bias, B, Sk), 0, 0
+        _set_live(a, _key_live(key_bias))
     check(_lib.lib().stb_attn_fwd(C.byref(a), _stream()))
     return out, lse
 
@@ -225,6 +258,7 @@ def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=No
         a.qk_prep = C.pointer(f)
     if key_bias is not None:
         a.bias, a.bias_b = key_bias.data_ptr(), _key_bias_stride(key_bias, B, Sk)
+        _set_live(a, _key_live(key_bias))
     check(_lib.lib().stb_attn_bwd(C.byref(a), _stream()))
     return dq, dk, dv
 

@@ -72,6 +72,16 @@ def _qwen_image_step():
     return QwenImage
 
 
+def _chroma():
+    from ..chroma.transformer import ChromaTransformer2DModel
+    return ChromaTransformer2DModel
+
+
+def _chroma_step():
+    from ..chroma.model import Chroma
+    return Chroma
+
+
 FAMILIES: Dict[str, FamilySpec] = {
     # registry keys: flux/model.py:1504, sd3/model.py:900, pixart/model.py:858 ("pixart_sigma"), qwen_image/model.py:1874
     "flux": FamilySpec("flux", "simpletuner.helpers.models.flux.model", "Flux", _flux, _flux_step,
@@ -87,13 +97,18 @@ FAMILIES: Dict[str, FamilySpec] = {
                                 "cross_attention_dim", "sample_size", "patch_size", "caption_channels", "interpolation_scale",
                                 "use_additional_conditions", "norm_eps")),
 }
-# Opt-in families: `install()` registers them only when named (`install(["qwen_image"])`), so an existing setup that calls
-# `install()` keeps exactly the families it had.
+# Opt-in families: `install()` registers them only when named (`install(["qwen_image"])`, `install(["chroma"])`), so an
+# existing setup that calls `install()` keeps exactly the families it had.  Registry key of Chroma: chroma/model.py:969.
 OPT_IN_FAMILIES: Dict[str, FamilySpec] = {
     "qwen_image": FamilySpec("qwen_image", "simpletuner.helpers.models.qwen_image.model", "QwenImage", _qwen_image,
                              _qwen_image_step,
                              ("patch_size", "in_channels", "out_channels", "num_layers", "attention_head_dim",
                               "num_attention_heads", "joint_attention_dim", "guidance_embeds", "axes_dims_rope")),
+    "chroma": FamilySpec("chroma", "simpletuner.helpers.models.chroma.model", "Chroma", _chroma, _chroma_step,
+                         ("patch_size", "in_channels", "out_channels", "num_layers", "num_single_layers",
+                          "attention_head_dim", "num_attention_heads", "joint_attention_dim", "axes_dims_rope",
+                          "approximator_num_channels", "approximator_hidden_dim", "approximator_layers",
+                          "enable_time_sign_embed", "musubi_blocks_to_swap", "deltatime_type")),
 }
 
 
