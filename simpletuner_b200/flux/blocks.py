@@ -7,10 +7,13 @@ Mirrors, for the training path, reference flux/transformer.py:
   * PEFT lora.Linear on the attention projections       (common.py:1094-1117, flux/model.py:1249-1262)
 
 Every arithmetic step is a libstb200 kernel (ops.*); torch only allocates, slices and carries the
-autograd graph between blocks.  Activations saved per block are the minimum the LoRA-only backward
-needs (block input, fused pre-norm QKV, attention output + LSE, post-attention stream, MLP
-pre-activation, the rank-r LoRA down-projections); LayerNorm-modulate, QK-RMSNorm/RoPE and GELU are
-recomputed inside the backward kernels instead of being stored.
+autograd graph between blocks.  Activations saved per block: block input, fused pre-norm QKV, the
+post-norm / post-RoPE q and k, attention output + LSE, post-attention stream, MLP pre-activation, the
+rank-r LoRA down-projections and, when a q/k/v adapter is present, the LayerNorm-modulated block input.
+Keeping q and k costs 2 B S D bytes per block (Flux.1-dev: 3.2 GB per 1024^2 sample over 57 blocks) and
+saves one HBM-bound RMSNorm + RoPE pass per block in backward; the modulated input (0.11 GB per block
+at B = 4, 1024^2) saves one LayerNorm-modulate pass.  GELU is recomputed inside the backward kernels.
+Gradient checkpointing with an interval is the way to trade this memory for compute.
 
 The hidden state travels as ONE joint buffer [B, S_txt + S_img, D] (text tokens first, as the
 reference concatenates them for attention, :166-168) so no torch.cat / split copies are needed.
@@ -29,15 +32,6 @@ import torch
 from .. import ops
 
 EPS = 1e-6
-# Keep the post-norm / post-RoPE q, k of every block for the backward instead of re-running the RMSNorm + RoPE pass there:
-# +2 B S D bytes per block (Flux.1-dev: +3.2 GB per sample over 57 blocks) for one HBM-bound kernel less per block in
-# backward.  STB_SAVE_QK=0 restores the recompute (larger batches / buckets).
-import os as _os
-SAVE_QK = _os.environ.get("STB_SAVE_QK", "1") != "0"
-# The LayerNorm-modulated block input (the A operand of the q|k|v projections and of their adapters' weight gradients) is kept
-# for backward instead of being recomputed: 0.11 GB per block at B = 4, 1024^2 (6.5 GB for Flux.1-dev) buys one LN-modulate
-# pass per block in backward.  STB_SAVE_NH=0 restores the recompute.
-SAVE_NH = _os.environ.get("STB_SAVE_NH", "1") != "0"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -70,21 +64,13 @@ def _t(w: torch.Tensor) -> torch.Tensor:
     return w.t().contiguous()
 
 
-# Dgrad operand policy.  A dgrad GEMM wants W^T in nn.Linear layout; it can get it as a real transposed copy (K-major B
-# operand, the fastest tile path: Flux LoRA step 362 ms of GEMM) or as a zero-copy view of the forward weight (ops.WT: the
-# kernel stages W as an MN-major B operand; +1.7 % GEMM time, but no second copy of the weights — 16 GB less for Flux.1-dev —
-# and, when the weights CHANGE every step, no per-step transposes at all).  STB_DGRAD_WKN = "auto" (default): the view for
-# weights that change per step (full fine-tune, LoKr), the copy for frozen weights; "1" / "0" force either.
-_WKN_MODE = _os.environ.get("STB_DGRAD_WKN", "auto")
-
-
-def use_wkn(dynamic: bool = False) -> bool:
-    return _WKN_MODE == "1" or (_WKN_MODE == "auto" and dynamic)
-
-
 def _wt(w: torch.Tensor, dynamic: bool = False):
-    """The dgrad operand of a base weight (see the policy above).  dynamic: the weight is rewritten every optimizer step."""
-    return ops.WT(w) if use_wkn(dynamic) else w.t().contiguous()
+    """The dgrad operand of a base weight.  A dgrad GEMM wants W^T in nn.Linear layout; it can get it as a real transposed
+    copy (K-major B operand, the fastest tile path: Flux LoRA step 362 ms of GEMM) or as a zero-copy view of the forward
+    weight (ops.WT: the kernel stages W as an MN-major B operand; +1.7 % GEMM time, but no second copy of the weights).
+    Frozen weights get the copy; weights rewritten every optimizer step (`dynamic`: full fine-tune, LoKr) get the view,
+    so no step spends a transpose on them."""
+    return ops.WT(w) if dynamic else _t(w)
 
 
 @dataclass
@@ -501,7 +487,7 @@ class DoubleBlockFn(torch.autograd.Function):
         packs = {}
         qkv = torch.empty((B, S, 3 * D), device=dev, dtype=torch.bfloat16)
         small = {}
-        keep_nh = SAVE_NH and any(x is not None for x in lora[0:6] + lora[8:14])     # only the adapters' weight gradients read it
+        keep_nh = any(x is not None for x in lora[0:6] + lora[8:14])     # only the adapters' weight gradients read it
         nh_joint = torch.empty_like(h) if keep_nh else None
         for name, sl, mod, base in streams:
             ap: AttnPlan = plans[name + "_attn"]
@@ -515,7 +501,7 @@ class DoubleBlockFn(torch.autograd.Function):
         q, k = _qk_fwd(qkv, D, H, hd, ia, ta, S_txt, cos, sin)
         v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
         o, lse = ops.attn_fwd(q, k, v, key_bias=st.get("key_bias"))
-        keep_qk = SAVE_QK and q.data_ptr() != qkv.data_ptr()      # (views of qkv when the model has neither norm nor RoPE)
+        keep_qk = q.data_ptr() != qkv.data_ptr()      # (views of qkv when the model has neither norm nor RoPE)
         if not keep_qk:
             del q, k
         o = o.view(B, S, D)
@@ -667,13 +653,11 @@ class DoubleBlockFn(torch.autograd.Function):
         for name, sl, mod, base, pre, t_qkv, t_out in streams:
             ap = plans[name + "_attn"]
             pk = packs[name + "_qkv"]
-            ish, isc = (1, 0) if name == "txt" and pre_only else (0, 1)
+            isc = 0 if name == "txt" and pre_only else 1         # chunk index of the scale
             d_nh, t_up = _linear_lora_dgrad(d_qkv[:, sl], ap.w_qkv_t, pk, dr(base))
             if pk is not None:
-                nh = nh_saved[:, sl] if nh_saved.numel() else _lnm_fwd(h[:, sl], segs[name], ish, isc)
-                for m, (da, db) in enumerate(_lora_grads(pk, nh, t_qkv, d_qkv[:, sl], t_up, dr(base))):
+                for m, (da, db) in enumerate(_lora_grads(pk, nh_saved[:, sl], t_qkv, d_qkv[:, sl], t_up, dr(base))):
                     grads[base + 2 * m], grads[base + 2 * m + 1] = da, db
-                del nh
             _lnm_bwd(d_nh, h[:, sl], segs[name], isc, add=dh1[:, sl], out=dh[:, sl])
             del d_nh
         if dual:
@@ -723,12 +707,10 @@ class SingleBlockFn(torch.autograd.Function):
         q, k = ops.qk_rmsnorm_rope_fwd(qkv, D, H, hd, ap.norm_q, ap.norm_k, None, None, 0, cos, sin, EPS)
         v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
         o, lse = ops.attn_fwd(q, k, v, key_bias=st.get("key_bias"))
-        if not SAVE_QK:
-            del q, k
         o = o.view(B, S, D)
         pre = torch.empty((B, S, 4 * D), device=dev, dtype=torch.bfloat16)
         act, t_mlp = _linear_lora_fwd(nh, mp.w1, mp.b1, pk_mlp, dr(3), epi=ops.EPI_GELU, aux=pre)
-        nh_keep = nh if (SAVE_NH and (pk is not None or pk_mlp is not None)) else None
+        nh_keep = nh if (pk is not None or pk_mlp is not None) else None
         del nh
         # proj_out(cat[attn, mlp]) as two K-segments of one GEMM; gate, residual, nan_to_num in the epilogue
         t_out = None
@@ -748,14 +730,12 @@ class SingleBlockFn(torch.autograd.Function):
         ctx.lora_present = [x is not None for x in lora]
         E = h.new_empty(0)
         keep = lambda t: t if t is not None else E
-        ctx.save_for_backward(h, mod, cos, sin, qkv, o, lse, pre, keep(t_qkv), q if SAVE_QK else E, k if SAVE_QK else E,
-                              keep(t_mlp), keep(t_out), keep(nh_keep))
+        ctx.save_for_backward(h, mod, cos, sin, qkv, o, lse, pre, keep(t_qkv), q, k, keep(t_mlp), keep(t_out), keep(nh_keep))
         return h_out
 
     @staticmethod
     def backward(ctx, dh_out):
-        h, mod, cos, sin, qkv, o, lse, pre, t_qkv, q_saved, k_saved, t_mlp, t_out, nh_saved = ctx.saved_tensors
-        qk_saved = (q_saved, k_saved) if q_saved.numel() else None
+        h, mod, cos, sin, qkv, o, lse, pre, t_qkv, q, k, t_mlp, t_out, nh = ctx.saved_tensors
         st = ctx.st
         pk, pk_mlp, pk_out = ctx.packs
         B, S, D = h.shape
@@ -787,8 +767,8 @@ class SingleBlockFn(torch.autograd.Function):
                 (grads[8], grads[9]), = _lora_grads(pk_out, torch.cat([o, act], 2), t_out, g, t_up, dr(4))
             del act, t_up
         del g
-        d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, ap, None, 0, cos, sin, qk=qk_saved, key_bias=st.get("key_bias"))
-        del d_o, qk_saved, q_saved, k_saved
+        d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, ap, None, 0, cos, sin, qk=(q, k), key_bias=st.get("key_bias"))
+        del d_o, q, k
         # d_nh = d_pre W_mlp + d_qkv W_qkv (+ LoRA branches as one more K-segment)
         t_ups, a_ts = [], []
         t_up_qkv = t_up_mlp = None
@@ -809,15 +789,12 @@ class SingleBlockFn(torch.autograd.Function):
             d_nh = ops.gemm([d_pre, d_qkv, t_ups[0]], [mp.w1_t, ap.w_qkv_t, a_ts[0]], None)
         else:                           # the GEMM takes three K-segments: both rank blocks travel as one
             d_nh = ops.gemm([d_pre, d_qkv, torch.cat(t_ups, 2)], [mp.w1_t, ap.w_qkv_t, torch.cat(a_ts, 1)], None)
-        if pk is not None or pk_mlp is not None:
-            nh = nh_saved if nh_saved.numel() else _lnm_fwd(h, segs, 0, 1)
-            if pk is not None:
-                for m, (da, db) in enumerate(_lora_grads(pk, nh, t_qkv, d_qkv, t_up_qkv, drop)):
-                    grads[2 * m], grads[2 * m + 1] = da, db
-            if pk_mlp is not None:
-                (grads[6], grads[7]), = _lora_grads(pk_mlp, nh, t_mlp, d_pre, t_up_mlp, dr(3))
-            del nh
-        del d_pre, d_qkv
+        if pk is not None:
+            for m, (da, db) in enumerate(_lora_grads(pk, nh, t_qkv, d_qkv, t_up_qkv, drop)):
+                grads[2 * m], grads[2 * m + 1] = da, db
+        if pk_mlp is not None:
+            (grads[6], grads[7]), = _lora_grads(pk_mlp, nh, t_mlp, d_pre, t_up_mlp, dr(3))
+        del nh, d_pre, d_qkv
         dh = _lnm_bwd(d_nh, h, segs, 1, add=dh_out)
         out = [grads[i] if ctx.lora_present[i] else None for i in range(ctx.n_lora_in)]
         return (dh, None, None, None, None, *out)

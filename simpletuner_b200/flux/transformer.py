@@ -31,7 +31,6 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
-from . import blocks as _blocks
 from .blocks import AttnPlan, DoubleBlockFn, LoraDrop, LoraLinearFn, MlpPlan, SingleBlockFn, TailFn, _t, _wt
 
 _ATTN = ["to_q", "to_k", "to_v", "add_q_proj", "add_k_proj", "add_v_proj", "to_out.0", "to_add_out"]
@@ -172,48 +171,49 @@ class _FeedForward(nn.Module):
     _lycoris_class_name = "FeedForward"
 
 
-def _fill_weight(lin: Linear, out: torch.Tensor, out_t: Optional[torch.Tensor]) -> None:
-    """Write `lin`'s effective weight and (unless the dgrad reads W itself, STB_DGRAD_WKN) its transpose into (slices of) a
-    plan's layouts; with a LoKr adapter both come out of one `stb_lokr_rebuild` pass over W."""
+def _fill_weight(lin: Linear, out: torch.Tensor) -> None:
+    """Write `lin`'s effective weight into (a slice of) a plan's layout; with a LoKr adapter it comes out of one
+    `stb_lokr_rebuild` pass over W."""
     if lin.lokr is None:
         out.copy_(lin.weight.detach())
-        if out_t is not None:
-            out_t.copy_(lin.weight.detach().t())
     else:
-        lin.lokr.rebuild_into(out, out_t)
+        lin.lokr.rebuild_into(out)
 
 
-def _weight_pair(lin: Linear):
+def _weight_pair(lin: Linear, dynamic: bool = False):
+    """(forward weight, dgrad operand) of one Linear.  dynamic: the weight is rewritten every optimizer step (full
+    fine-tune); a LoKr weight is rebuilt every step, so it is dynamic too."""
     if lin.lokr is None:
         w = lin.weight.detach()
-        return w, _wt(w)
+        return w, _wt(w, dynamic)
     w = torch.empty_like(lin.weight)
-    if _blocks.use_wkn(True):          # LoKr: the weight is rebuilt every step -> dgrad reads it in place
-        _fill_weight(lin, w, None)
-        return w, _wt(w, True)
-    w_t = torch.empty((lin.in_features, lin.out_features), device=w.device, dtype=w.dtype)
-    _fill_weight(lin, w, w_t)
-    return w, w_t
+    _fill_weight(lin, w)
+    return w, _wt(w, True)
 
 
-def _attn_plan(q: Linear, k: Linear, v: Linear, out: Optional[Linear], nq, nk) -> AttnPlan:
+def _attn_plan(q: Linear, k: Linear, v: Linear, out: Optional[Linear], nq, nk, dynamic: bool = False) -> AttnPlan:
+    """Fused q|k|v and output layouts of one attention stream; nq / nk None: no QK norm (SD3 without qk_norm)."""
     b_qkv = torch.cat([q.bias.detach(), k.bias.detach(), v.bias.detach()], 0).contiguous()
     if q.lokr is None and k.lokr is None and v.lokr is None:
         w_qkv = torch.cat([q.weight.detach(), k.weight.detach(), v.weight.detach()], 0).contiguous()
-        w_qkv_t = _wt(w_qkv)
+        w_qkv_t = _wt(w_qkv, dynamic)
     else:
-        n, kin = q.out_features, q.in_features
-        w_qkv = torch.empty((3 * n, kin), device=q.weight.device, dtype=q.weight.dtype)
-        w_qkv_t = None if _blocks.use_wkn(True) else torch.empty((kin, 3 * n), device=q.weight.device, dtype=q.weight.dtype)
+        n = q.out_features
+        w_qkv = torch.empty((3 * n, q.in_features), device=q.weight.device, dtype=q.weight.dtype)
         for m, lin in enumerate((q, k, v)):
-            _fill_weight(lin, w_qkv[m * n:(m + 1) * n], None if w_qkv_t is None else w_qkv_t[:, m * n:(m + 1) * n])
-        if w_qkv_t is None:
-            w_qkv_t = _wt(w_qkv, True)
-    p = AttnPlan(w_qkv, b_qkv, w_qkv_t, norm_q=nq.weight.detach(), norm_k=nk.weight.detach())
+            _fill_weight(lin, w_qkv[m * n:(m + 1) * n])
+        w_qkv_t = _wt(w_qkv, True)
+    p = AttnPlan(w_qkv, b_qkv, w_qkv_t, norm_q=None if nq is None else nq.weight.detach(),
+                 norm_k=None if nk is None else nk.weight.detach())
     if out is not None:
-        p.w_out, p.w_out_t = _weight_pair(out)
+        p.w_out, p.w_out_t = _weight_pair(out, dynamic)
         p.b_out = out.bias.detach()
     return p
+
+
+def _mlp_plan(fc1: Linear, fc2: Linear, dynamic: bool = False) -> MlpPlan:
+    (w1, w1_t), (w2, w2_t) = _weight_pair(fc1, dynamic), _weight_pair(fc2, dynamic)
+    return MlpPlan(w1, fc1.bias.detach(), w1_t, w2, fc2.bias.detach(), w2_t)
 
 
 def _lora_list(linears: Sequence[Linear]) -> List[Optional[torch.Tensor]]:
@@ -253,19 +253,14 @@ class FluxTransformerBlock(nn.Module):
             self._plans = {}
         pl = self._plans
         a = self.attn
-
-        def mk(ff):
-            (w1, w1_t), (w2, w2_t) = _weight_pair(ff.net[0].proj), _weight_pair(ff.net[2])
-            return MlpPlan(w1, ff.net[0].proj.bias.detach(), w1_t, w2, ff.net[2].bias.detach(), w2_t)
-
         if "img_attn" not in pl:
             pl["img_attn"] = _attn_plan(a.to_q, a.to_k, a.to_v, a.to_out[0], a.norm_q, a.norm_k)
         if "txt_attn" not in pl:
             pl["txt_attn"] = _attn_plan(a.add_q_proj, a.add_k_proj, a.add_v_proj, a.to_add_out, a.norm_added_q, a.norm_added_k)
         if "img_mlp" not in pl:
-            pl["img_mlp"] = mk(self.ff)
+            pl["img_mlp"] = _mlp_plan(self.ff.net[0].proj, self.ff.net[2])
         if "txt_mlp" not in pl:
-            pl["txt_mlp"] = mk(self.ff_context)
+            pl["txt_mlp"] = _mlp_plan(self.ff_context.net[0].proj, self.ff_context.net[2])
         return pl
 
     def drop_adapted_plans(self):
@@ -325,8 +320,7 @@ class FluxSingleTransformerBlock(nn.Module):
         if "attn" not in pl:
             pl["attn"] = _attn_plan(a.to_q, a.to_k, a.to_v, None, a.norm_q, a.norm_k)
         if "mlp" not in pl:
-            pl["mlp"] = MlpPlan(self.proj_mlp.weight.detach(), self.proj_mlp.bias.detach(), _wt(self.proj_mlp.weight.detach()),
-                                self.proj_out.weight.detach(), self.proj_out.bias.detach(), _wt(self.proj_out.weight.detach()))
+            pl["mlp"] = _mlp_plan(self.proj_mlp, self.proj_out)
         return pl
 
     def drop_adapted_plans(self):
@@ -495,14 +489,28 @@ class LoraDropoutAPI:
 
 
 class AdapterModelAPI:
-    """Gradient checkpointing and the PEFT adapter surface shared by the denoisers built on the Flux blocks.  A model sets
-    `_DEFAULT_LORA_TARGETS` and `_lora_adaptable(name)` (the Linears its block schedules can adapt)."""
+    """Gradient checkpointing, the PEFT adapter surface and the parameter lifecycle shared by every denoiser built on the
+    Flux blocks.  A model sets `_DEFAULT_LORA_TARGETS`, `_lora_adaptable(name)` (the Linears its block schedules can
+    adapt) and `invalidate_plans()` (drops what it derived from the parameters; run after `.to()` / `load_state_dict`)."""
 
     _DEFAULT_LORA_TARGETS: Sequence[str] = ()
 
     @staticmethod
     def _lora_adaptable(name: str) -> bool:
         raise NotImplementedError
+
+    def invalidate_plans(self):
+        raise NotImplementedError
+
+    def _apply(self, fn, *a, **k):
+        out = super()._apply(fn, *a, **k)
+        self.invalidate_plans()
+        return out
+
+    def load_state_dict(self, *a, **k):
+        out = super().load_state_dict(*a, **k)
+        self.invalidate_plans()
+        return out
 
     def enable_gradient_checkpointing(self):
         """common.py:3550-3636 / flux/transformer.py:1240-1287: blocks selected by `gradient_checkpointing_interval`
@@ -553,8 +561,8 @@ class AdapterModelAPI:
             if not isinstance(mod, Linear) or not _peft_match(name, targets):
                 continue
             if not self._lora_adaptable(name):
-                raise NotImplementedError(f"LoRA target {name} is not supported by the fused path (adaLN / embedder linears: "
-                                          "use the reference module, e.g. for flux_lora_target=ai-toolkit)")
+                raise NotImplementedError(f"LoRA target {name} is not supported by the fused path (use the reference "
+                                          "module, e.g. for the adaLN linears of flux_lora_target=ai-toolkit)")
             chosen.append(mod)
         for mod in chosen:
             mod.add_lora(rank, lora_alpha, adapter_name)
@@ -624,17 +632,7 @@ class FluxTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, 
         for blk in list(self.transformer_blocks) + list(self.single_transformer_blocks):
             blk._plans = None
         self._tail_plan = None
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self.invalidate_plans()
         self._rope_cache.clear()
-        return out
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self.invalidate_plans()
-        return out
 
     def after_optimizer_step(self):
         """TrainStep hook: with a LyCORIS LoKr network attached the projection layouts embed W + kron(w1, w2) and must follow

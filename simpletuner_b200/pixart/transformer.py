@@ -25,7 +25,7 @@ self-attention masks, full fine-tune.
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, List, Optional
 
 import torch
 import torch.nn as nn
@@ -33,7 +33,8 @@ import torch.nn.functional as F
 
 from .. import ops
 from ..flux.blocks import EPS, MlpPlan, TailFn, _linear_lora_dgrad, _linear_lora_fwd, _lora_grads, _t, _wt, pack_lora
-from ..flux.transformer import AttnProcessorAPI, LoraDropoutAPI, Linear, _FeedForward, _lora_list, _sinusoid, _TimestepEmbedding
+from ..flux.transformer import (AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, Linear, _FeedForward, _lora_list, _sinusoid,
+                                _TimestepEmbedding)
 
 PIXART_LORA_TARGETS = ["to_k", "to_q", "to_v", "to_out.0"]  # PixartSigma.DEFAULT_LORA_TARGET, reference pixart/model.py:59
 MASK_BIAS = -10000.0
@@ -303,8 +304,9 @@ def sincos_pos_embed_2d(dim: int, grid_h: int, grid_w: int, base_size: int, inte
     return torch.cat(parts, dim=1).float().to(device)
 
 
-class PixArtTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
+class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, nn.Module):
     _no_split_modules = ["BasicTransformerBlock", "PatchEmbed"]
+    _DEFAULT_LORA_TARGETS = PIXART_LORA_TARGETS
 
     def __init__(self, num_attention_heads: int = 16, attention_head_dim: int = 72, in_channels: int = 4,
                  out_channels: Optional[int] = 8, num_layers: int = 28, dropout: float = 0.0, norm_num_groups: int = 32,
@@ -351,18 +353,10 @@ class PixArtTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         self.gradient_checkpointing = False
 
     # ---- reference-facing utilities -------------------------------------------------------------
-    def enable_gradient_checkpointing(self):
-        """Re-run every transformer block in backward (torch.utils.checkpoint, as the reference does); off by default."""
-        self.gradient_checkpointing = True
-
-    def disable_gradient_checkpointing(self):
-        self.gradient_checkpointing = False
-
-    def _run_block(self, blk, *args):
-        if self.gradient_checkpointing and torch.is_grad_enabled():
-            from torch.utils.checkpoint import checkpoint
-            return checkpoint(blk, *args, use_reentrant=False)
-        return blk(*args)
+    @staticmethod
+    def _lora_adaptable(name: str) -> bool:
+        # the block schedule adapts the projections of both attentions only
+        return ".attn1." in name or ".attn2." in name
 
     def invalidate_plans(self):
         for blk in self.transformer_blocks:
@@ -370,61 +364,6 @@ class PixArtTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         self._tail_plan = {}
         self._pos_cache.clear()
         self._pad_index = None
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self.invalidate_plans()
-        return out
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self.invalidate_plans()
-        return out
-
-    def lora_linears(self) -> Dict[str, Linear]:
-        return {n: m for n, m in self.named_modules() if isinstance(m, Linear) and m.lora_A is not None}
-
-    def add_adapter(self, lora_config=None, adapter_name: str = "default", *, rank: Optional[int] = None,
-                    lora_alpha: Optional[float] = None, target_modules: Optional[Sequence[str]] = None,
-                    lora_dropout: float = 0.0):
-        if lora_config is not None:
-            rank = getattr(lora_config, "r", rank)
-            lora_alpha = getattr(lora_config, "lora_alpha", lora_alpha)
-            target_modules = getattr(lora_config, "target_modules", target_modules)
-            lora_dropout = getattr(lora_config, "lora_dropout", lora_dropout)
-        lora_dropout = self._check_dropout_p(lora_dropout)
-        if not 1 <= rank <= 128:
-            raise NotImplementedError("fused LoRA path supports rank 1..128 (one 128-wide rank block per adapted Linear)")
-        lora_alpha = float(lora_alpha) if lora_alpha is not None else float(rank)
-        targets = list(target_modules) if target_modules is not None else PIXART_LORA_TARGETS
-        n = 0
-        for name, mod in self.named_modules():
-            if not isinstance(mod, Linear):
-                continue
-            hit = [t for t in targets if name.endswith("." + t)]  # PEFT suffix matching
-            if not hit:
-                continue
-            if ".attn1." not in name and ".attn2." not in name:
-                raise NotImplementedError(f"LoRA target {name} is outside the attention projections the fused path adapts")
-            mod.add_lora(rank, lora_alpha, adapter_name)
-            n += 1
-        if n == 0:
-            raise ValueError(f"no module matched LoRA targets {targets}")
-        self._lora_scaling = lora_alpha / rank
-        self._lora_dropout_p = lora_dropout
-        self.peft_config[adapter_name] = SimpleNamespace(r=rank, lora_alpha=lora_alpha, target_modules=targets, lora_dropout=lora_dropout)
-        return n
-
-    def disable_lora(self):
-        for m in self.lora_linears().values():
-            m.lora_enabled = False
-
-    def enable_lora(self):
-        for m in self.lora_linears().values():
-            m.lora_enabled = True
-
-    def trainable_parameters(self):
-        return [p for p in self.parameters() if p.requires_grad]
 
     # ---- forward --------------------------------------------------------------------------------
     def _pos(self, hp: int, wp: int, dtype, device) -> torch.Tensor:
@@ -498,8 +437,8 @@ class PixArtTransformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         if self._pad_index is None and hdp != hd:
             self._pad_index = (torch.arange(H, device=dev)[:, None] * hdp + torch.arange(hd, device=dev)[None, :]).reshape(-1)
         self._begin_lora_dropout(list(self.transformer_blocks))
-        for blk in self.transformer_blocks:
-            h = self._run_block(blk, h, ctx, kbias, t6, self._lora_scaling, self._pad_index)
+        for i, blk in enumerate(self.transformer_blocks):
+            h = self._run_block(i, blk, h, ctx, kbias, t6, self._lora_scaling, self._pad_index)
         # 3. output: LN -> (scale_shift_table + embedded) modulate -> proj_out  (reference :749-760)
         mod = (self.scale_shift_table[None] + embedded[:, None].to(self.scale_shift_table.dtype)).to(dt)  # [B, 2, D] (shift | scale)
         mod = torch.cat([mod[:, 1], mod[:, 0]], dim=1).contiguous()                                         # TailFn wants (scale | shift)

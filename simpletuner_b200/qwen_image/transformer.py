@@ -242,16 +242,12 @@ class QwenImageTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropout
     def _lora_adaptable(name: str) -> bool:
         return name.endswith(_ADAPTABLE_SUFFIXES)
 
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)          # the attention modules re-fuse q|k|v in their own _apply
+    def invalidate_plans(self):
+        """The plans are built per forward; what is kept is the RoPE tables and the fused q|k|v storage, which
+        load_state_dict(assign=True) splits by replacing the q / k / v parameters."""
         self._rope_cache.clear()
-        return out
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        for blk in self.transformer_blocks:        # assign=True replaces the q / k / v parameters
+        for blk in self.transformer_blocks:
             blk.attn.fused_qkv()
-        return out
 
     def _rope(self, h: int, w: int, S_txt: int, device):
         key = (h, w, S_txt, str(device))

@@ -18,17 +18,19 @@ through sd3/fullft.py after `enable_full_finetune()`.
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import Any, Dict, Optional, Sequence, Tuple
+from typing import Any, Dict, Optional, Tuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
-from ..flux.blocks import AttnPlan, DoubleBlockFn, MlpPlan, TailFn, _t, _wt
-from ..flux.transformer import AttnProcessorAPI, LoraDropoutAPI, Linear, RMSNormWeight, _AdaNorm, _FeedForward, _TimestepEmbedding, _attn_plan, _lora_list, _sinusoid
+from ..flux.blocks import DoubleBlockFn, TailFn, _wt
+from ..flux.transformer import (_ATTN, AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, Linear, RMSNormWeight, _AdaNorm,
+                                _FeedForward, _TimestepEmbedding, _attn_plan, _lora_list, _mlp_plan, _sinusoid)
 
 SD3_LORA_TARGETS = ["to_k", "to_q", "to_v", "to_out.0"]  # SD3.DEFAULT_LORA_TARGET, reference sd3/model.py:122
+_ADAPTABLE_SUFFIXES = tuple("." + t for t in _ATTN)
 
 
 class _JointAttention(nn.Module):
@@ -50,20 +52,6 @@ class _JointAttention(nn.Module):
             if qk_norm:
                 self.norm_added_q = RMSNormWeight(head_dim, dtype)
                 self.norm_added_k = RMSNormWeight(head_dim, dtype)
-
-
-class _NoNorm:
-    weight = None
-
-
-def _plan(q, k, v, out, nq, nk, dyn: bool = False) -> AttnPlan:
-    w_qkv = torch.cat([q.weight.detach(), k.weight.detach(), v.weight.detach()], 0).contiguous()
-    b_qkv = torch.cat([q.bias.detach(), k.bias.detach(), v.bias.detach()], 0).contiguous()
-    p = AttnPlan(w_qkv, b_qkv, _wt(w_qkv, dyn), norm_q=None if nq is None else nq.weight.detach(),
-                 norm_k=None if nk is None else nk.weight.detach())
-    if out is not None:
-        p.w_out, p.b_out, p.w_out_t = out.weight.detach(), out.bias.detach(), _wt(out.weight.detach(), dyn)
-    return p
 
 
 class JointTransformerBlock(nn.Module):
@@ -88,18 +76,17 @@ class JointTransformerBlock(nn.Module):
             a = self.attn
             g = lambda m, n: getattr(m, n, None)
             dyn = bool(getattr(self, "_full_ft", False))      # full fine-tune: the weights change every step
-            mk = lambda ff: MlpPlan(ff.net[0].proj.weight.detach(), ff.net[0].proj.bias.detach(), _wt(ff.net[0].proj.weight.detach(), dyn),
-                                    ff.net[2].weight.detach(), ff.net[2].bias.detach(), _wt(ff.net[2].weight.detach(), dyn))
             pl = {
-                "img_attn": _plan(a.to_q, a.to_k, a.to_v, a.to_out[0], g(a, "norm_q"), g(a, "norm_k"), dyn),
-                "txt_attn": _plan(a.add_q_proj, a.add_k_proj, a.add_v_proj, g(a, "to_add_out"), g(a, "norm_added_q"), g(a, "norm_added_k"), dyn),
-                "img_mlp": mk(self.ff),
+                "img_attn": _attn_plan(a.to_q, a.to_k, a.to_v, a.to_out[0], g(a, "norm_q"), g(a, "norm_k"), dyn),
+                "txt_attn": _attn_plan(a.add_q_proj, a.add_k_proj, a.add_v_proj, g(a, "to_add_out"), g(a, "norm_added_q"),
+                                       g(a, "norm_added_k"), dyn),
+                "img_mlp": _mlp_plan(self.ff.net[0].proj, self.ff.net[2], dyn),
             }
             if not self.context_pre_only:
-                pl["txt_mlp"] = mk(self.ff_context)
+                pl["txt_mlp"] = _mlp_plan(self.ff_context.net[0].proj, self.ff_context.net[2], dyn)
             if self.use_dual_attention:
                 b = self.attn2
-                pl["img_attn2"] = _plan(b.to_q, b.to_k, b.to_v, b.to_out[0], g(b, "norm_q"), g(b, "norm_k"), dyn)
+                pl["img_attn2"] = _attn_plan(b.to_q, b.to_k, b.to_v, b.to_out[0], g(b, "norm_q"), g(b, "norm_k"), dyn)
             self._plans = pl
         return self._plans
 
@@ -158,8 +145,9 @@ class _TimeTextEmbed(nn.Module):
         self.text_embedder = _TimestepEmbedding(pooled_dim, dim, dtype)
 
 
-class SD3Transformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
+class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, nn.Module):
     _no_split_modules = ["JointTransformerBlock"]
+    _DEFAULT_LORA_TARGETS = SD3_LORA_TARGETS
 
     def __init__(self, sample_size: int = 128, patch_size: int = 2, in_channels: int = 16, num_layers: int = 18,
                  attention_head_dim: int = 64, num_attention_heads: int = 18, joint_attention_dim: int = 4096,
@@ -196,18 +184,10 @@ class SD3Transformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         self.gradient_checkpointing = False
 
     # ---- reference-facing utilities -------------------------------------------------------------
-    def enable_gradient_checkpointing(self):
-        """Re-run every joint block in backward (torch.utils.checkpoint, as the reference does); off by default."""
-        self.gradient_checkpointing = True
-
-    def disable_gradient_checkpointing(self):
-        self.gradient_checkpointing = False
-
-    def _run_block(self, blk, *args):
-        if self.gradient_checkpointing and torch.is_grad_enabled():
-            from torch.utils.checkpoint import checkpoint
-            return checkpoint(blk, *args, use_reentrant=False)
-        return blk(*args)
+    @staticmethod
+    def _lora_adaptable(name: str) -> bool:
+        # the attention projections of `attn` / `attn2`; the FeedForward and adaLN linears are not in the LoRA schedule
+        return (".attn." in name or ".attn2." in name) and name.endswith(_ADAPTABLE_SUFFIXES)
 
     def invalidate_plans(self):
         for blk in self.transformer_blocks:
@@ -238,62 +218,6 @@ class SD3Transformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         step (they depend on weights the optimizer changes between replays)."""
         if getattr(self, "_full_ft", False):
             self.invalidate_plans()
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self.invalidate_plans()
-        return out
-
-    def load_state_dict(self, *a, **k):
-        out = super().load_state_dict(*a, **k)
-        self.invalidate_plans()
-        return out
-
-    def lora_linears(self) -> Dict[str, Linear]:
-        return {n: m for n, m in self.named_modules() if isinstance(m, Linear) and m.lora_A is not None}
-
-    def add_adapter(self, lora_config=None, adapter_name: str = "default", *, rank: Optional[int] = None,
-                    lora_alpha: Optional[float] = None, target_modules: Optional[Sequence[str]] = None,
-                    lora_dropout: float = 0.0):
-        if lora_config is not None:
-            rank = getattr(lora_config, "r", rank)
-            lora_alpha = getattr(lora_config, "lora_alpha", lora_alpha)
-            target_modules = getattr(lora_config, "target_modules", target_modules)
-            lora_dropout = getattr(lora_config, "lora_dropout", lora_dropout)
-        lora_dropout = self._check_dropout_p(lora_dropout)
-        if not 1 <= rank <= 128:
-            raise NotImplementedError("fused LoRA path supports rank 1..128 (one 128-wide rank block per adapted Linear)")
-        lora_alpha = float(lora_alpha) if lora_alpha is not None else float(rank)
-        targets = list(target_modules) if target_modules is not None else SD3_LORA_TARGETS
-        supported = {"to_q", "to_k", "to_v", "to_out.0", "add_q_proj", "add_k_proj", "add_v_proj", "to_add_out"}
-        n = 0
-        for name, mod in self.named_modules():
-            if not isinstance(mod, Linear) or ".attn" not in name:
-                continue
-            hit = [t for t in targets if name.endswith("." + t)]  # PEFT suffix matching
-            if not hit:
-                continue
-            if hit[0] not in supported:
-                raise NotImplementedError(f"LoRA target {hit[0]} is not supported by the fused path")
-            mod.add_lora(rank, lora_alpha, adapter_name)
-            n += 1
-        if n == 0:
-            raise ValueError(f"no module matched LoRA targets {targets}")
-        self._lora_scaling = lora_alpha / rank
-        self._lora_dropout_p = lora_dropout
-        self.peft_config[adapter_name] = SimpleNamespace(r=rank, lora_alpha=lora_alpha, target_modules=targets, lora_dropout=lora_dropout)
-        return n
-
-    def disable_lora(self):
-        for m in self.lora_linears().values():
-            m.lora_enabled = False
-
-    def enable_lora(self):
-        for m in self.lora_linears().values():
-            m.lora_enabled = True
-
-    def trainable_parameters(self):
-        return [p for p in self.parameters() if p.requires_grad]
 
     # ---- forward --------------------------------------------------------------------------------
     def _cropped_pos(self, h: int, w: int, dtype) -> torch.Tensor:
@@ -351,8 +275,8 @@ class SD3Transformer2DModel(AttnProcessorAPI, LoraDropoutAPI, nn.Module):
         temb = tte.timestep_embedder(_sinusoid(timestep.to(dev).float()).to(dt)) + tte.text_embedder(pooled_projections.to(dt).contiguous())
         silu_temb = F.silu(temb).contiguous()
         self._begin_lora_dropout(list(self.transformer_blocks))
-        for blk in self.transformer_blocks:
-            h = self._run_block(blk, h, silu_temb, S_txt, self._lora_scaling)
+        for i, blk in enumerate(self.transformer_blocks):
+            h = self._run_block(i, blk, h, silu_temb, S_txt, self._lora_scaling)
         if self._tail_plan is None:
             self._tail_plan = {"w_proj": self.proj_out.weight.detach(), "b_proj": self.proj_out.bias.detach(),
                                "w_proj_t": _wt(self.proj_out.weight.detach(), bool(getattr(self, "_full_ft", False)))}
