@@ -25,7 +25,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..flux.transformer import (FluxAttention, FluxSingleTransformerBlock, FluxTransformer2DModel, FluxTransformerBlock,
-                                Linear, RMSNormWeight, _ATTN, _FFS, _FeedForward, run_double_block, run_single_block)
+                                Linear, RMSNormWeight, _FeedForward, run_double_block, run_single_block)
 
 _ALL = ["to_k", "to_q", "to_v", "to_qkv", "add_qkv_proj", "add_k_proj", "add_q_proj", "add_v_proj", "to_out.0", "to_add_out"]
 _CTX = ["add_k_proj", "add_q_proj", "add_v_proj", "add_qkv_proj", "to_add_out"]
@@ -45,13 +45,6 @@ CHROMA_LORA_TARGETS = {
     "tiny": _TINY,
     "tiny+embedder": ["x_embedder"] + _TINY,
 }
-ABSENT_TARGETS = ("to_qkv", "add_qkv_proj", "norm.linear", "norm1.linear", "norm1_context.linear")
-_ADAPTABLE_SUFFIXES = tuple("." + t for t in (_ATTN + _FFS))
-
-
-def chroma_target_supported(target: str) -> bool:
-    """Whether a LoRA target name adapts only Linears the Chroma block schedules can train (or matches nothing)."""
-    return target in ABSENT_TARGETS or target == "x_embedder" or ("." + target).endswith(_ADAPTABLE_SUFFIXES)
 
 
 def _timestep_embedding(t: torch.Tensor, dim: int, max_period: int = 10000) -> torch.Tensor:

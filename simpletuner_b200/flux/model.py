@@ -5,13 +5,10 @@
   * `model_predict(prepared_batch)` reference helpers/models/flux/model.py:630-864 (`_model_predict_single`)
   * `loss(prepared_batch, model_output)` / `loss_with_logs(...)`  common.py:6217-6430, xm_mixin.py:476-485
 
-Batch dict keys are the collate contract of the reference (training/collate.py:1316-1349):
-`latent_batch`, `prompt_embeds`, `add_text_embeds`; `prepare_batch` adds `latents`, `noise`,
-`input_noise`, `sigmas` ([B,1,1,1] after expand_sigmas), `timesteps`, `noisy_latents`,
-`encoder_hidden_states`, `added_cond_kwargs`.  Random draws use torch's default generators in the
-reference order (randn_like(latents) then randn((bsz,)), SURVEY.md §8d) so a seeded run samples
-the same noise / sigmas.  All tensor arithmetic is libstb200 (flow_prep_pack / flow_mse_loss / the
-transformer); the patchify / unpatchify index math is folded into those two kernels.
+The flow-matching batch draw, the packed prediction and the loss are the shared StepWrapper's (family.py); what is Flux's
+own is the guidance input, Kontext, attention-masked training, LyCORIS LoKr and the `flux_lora_target` lists.  All tensor
+arithmetic is libstb200 (flow_prep_pack / flow_mse_loss / the transformer); the patchify / unpatchify index math is folded
+into those two kernels.
 """
 from __future__ import annotations
 
@@ -21,9 +18,8 @@ from typing import Any, Dict, Optional
 import torch
 
 from .. import ops
-from ..training.schedule import sample_flow_sigmas
-from .blocks import FlowLossFn
-from .transformer import FluxTransformer2DModel
+from ..family import CONDITIONING_INPUTS, StepWrapper, lora_type
+from .transformer import FLUX_LORA_TARGETS, FluxTransformer2DModel
 
 
 def default_config(**over) -> SimpleNamespace:
@@ -41,41 +37,25 @@ def default_config(**over) -> SimpleNamespace:
     return SimpleNamespace(**cfg)
 
 
-class Flux:
-    """Drop-in for the reference `Flux(ImageModelFoundation)` step methods.  `self.model` is the
-    denoiser (optionally DDP-wrapped), `self.accelerator.device` the rank's CUDA device."""
+class Flux(StepWrapper):
+    """Drop-in for the reference `Flux(ImageModelFoundation)` step methods."""
 
     NAME = "Flux.1"
-    PREDICTION_TYPE = "flow_matching"
+    DENOISER = FluxTransformer2DModel
+    DEFAULT_CONFIG = staticmethod(default_config)
+    LORA_TYPES = ("standard", "lycoris")        # LyCORIS: LoKr only (validate_config)
+    REFUSED_BATCH_KEYS = CONDITIONING_INPUTS    # outside model_flavour='kontext'
 
     def __init__(self, config: Optional[SimpleNamespace] = None, transformer: Optional[FluxTransformer2DModel] = None,
                  device: Optional[torch.device] = None, **transformer_kwargs):
-        self.config = config or default_config()
-        dev = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
-        self.accelerator = SimpleNamespace(device=dev)
-        self.noise_schedule = SimpleNamespace(config=SimpleNamespace(num_train_timesteps=1000, patch_size=2,
-                                                                       base_image_seq_len=256, max_image_seq_len=4096,
-                                                                       base_shift=0.5, max_shift=1.15))
-        self.model = transformer if transformer is not None else FluxTransformer2DModel(**transformer_kwargs)
+        super().__init__(config, transformer, device, **transformer_kwargs)
         # set_attn_processor refuses the flash processors (key-padding semantics) while the additive mask is in use
         self._denoiser().attention_masked_training = bool(getattr(self.config, "flux_attention_masked_training", False))
 
-    # ------------------------------------------------------------------------------------------
-    def get_trained_component(self):
-        return self.model
-
-    def _denoiser(self) -> FluxTransformer2DModel:
-        m = self.model
-        return m.module if hasattr(m, "module") else m
-
-    def add_lora_adapter(self):
-        """common.py:1049-1117 for the Flux targets (flux/model.py:1235-1383)."""
-        c = self.config
-        alpha = c.lora_alpha if c.lora_alpha is not None else c.lora_rank
-        from .transformer import FLUX_LORA_TARGETS
-        return self._denoiser().add_adapter(rank=c.lora_rank, lora_alpha=alpha,
-                                            target_modules=FLUX_LORA_TARGETS[c.flux_lora_target],
-                                            lora_dropout=getattr(c, "lora_dropout", 0.0))
+    @classmethod
+    def _default_lora_targets(cls, c) -> list:
+        """The `flux_lora_target` list (flux/model.py:1235-1383)."""
+        return list(FLUX_LORA_TARGETS[getattr(c, "flux_lora_target", None) or "all"])
 
     def add_lycoris_adapter(self, lycoris_config):
         """trainer.py:3390-3505 (`lora_type = "lycoris"`): LycorisNetwork.apply_preset + create_lycoris + apply_to.  Takes the
@@ -100,15 +80,15 @@ class Flux:
     # ------------------------------------------------------------------------------------------
     @classmethod
     def validate_config(cls, c) -> None:
-        """Load-time counterpart of the per-batch guards: options of the reference this path does not implement raise
-        NotImplementedError so that the shim (shim/foundation.py) keeps the reference module for such a run."""
+        """StepWrapper.validate_config plus Flux's own options: the `flux_lora_target` list, the LyCORIS algorithm,
+        attention-masked training and Kontext's loss."""
         g = lambda k, d=None: getattr(c, k, d)
-        if g("controlnet", False):
-            raise NotImplementedError("controlnet training is not supported by the libstb200 path")
-        if str(g("model_type", "lora")) not in ("lora",):
-            raise NotImplementedError(f"model_type={g('model_type')!r}: only LoRA training runs on the libstb200 path")
-        lt = str(g("lora_type", "standard") or "standard").lower()
-        if lt == "lycoris":
+        tgt = g("flux_lora_target", "all") or "all"
+        if tgt not in FLUX_LORA_TARGETS:       # "ai-toolkit" (adaLN linears) / "controlnet" stay on the reference module
+            raise NotImplementedError(f"flux_lora_target={tgt!r} is not supported by the libstb200 path "
+                                      f"(supported: {sorted(FLUX_LORA_TARGETS)})")
+        super().validate_config(c)
+        if lora_type(c) == "lycoris":
             cfg = g("lycoris_config", None)
             if isinstance(cfg, str):
                 import json
@@ -117,15 +97,6 @@ class Flux:
             if isinstance(cfg, dict):       # only LoKr (the reference's documented default) runs here
                 from ..lycoris import validate_lycoris_config
                 validate_lycoris_config(cfg)
-        elif lt != "standard":
-            raise NotImplementedError(f"lora_type={g('lora_type')!r} is not supported by the libstb200 path")
-        if g("use_dora", False):
-            raise NotImplementedError("DoRA is not supported by the libstb200 path")
-        from .transformer import FLUX_LORA_TARGETS
-        tgt = g("flux_lora_target", "all") or "all"
-        if tgt not in FLUX_LORA_TARGETS:       # "ai-toolkit" (adaLN linears) / "controlnet" stay on the reference module
-            raise NotImplementedError(f"flux_lora_target={tgt!r} is not supported by the libstb200 path "
-                                      f"(supported: {sorted(FLUX_LORA_TARGETS)})")
         check_masked_training(c)
         if is_kontext(c):
             lt = str(g("loss_type", "l2"))
@@ -133,106 +104,33 @@ class Flux:
                 # the reference feeds Kontext's 2-D timesteps [B, S_scene + S_c] to compute_scheduled_huber_c
                 raise NotImplementedError(f"Kontext with loss_type={lt!r} and huber_schedule={g('huber_schedule')!r} is not "
                                           "supported by the libstb200 path (l2 or a constant huber_c run)")
-        if g("tread_config", None):
-            raise NotImplementedError("TREAD routing is not supported by the libstb200 path")
-        if g("flow_cubic_schedule", None) or g("flow_cubic_schedule_weights", None):
-            raise NotImplementedError("the cubic-spline flow schedule is not part of the libstb200 step")
-        for flag in ("twinflow_enabled", "crepa_enabled", "layersync_enabled", "scheduled_sampling_max_step_offset",
-                     "diff2flow_enabled"):
-            if g(flag, None):
-                raise NotImplementedError(f"{flag} is not supported by the libstb200 path")
-        if g("distillation_method", None) not in (None, "", "None"):
-            raise NotImplementedError("distillation is not supported by the libstb200 path")
-
-    def adopt_noise_schedule(self, sched) -> None:
-        """Use the reference family's scheduler object (its `.config` feeds the flow shift / timestep count)."""
-        self.noise_schedule = sched
 
     def _check_supported(self, batch: Dict[str, Any]) -> None:
-        """Options of the reference wrapper this path does not implement must RAISE, never be ignored, so that a shim can
-        route such a config to the reference class (INTEGRATION.md 2): masked training outside `check_masked_training`'s
-        rule or without the batch's `encoder_attention_mask` (flux/model.py:813-822), conditioning latents outside the
-        Kontext flavour, and pre-packed Kontext inputs that `prepare_batch` did not build (flux/model.py:757-786)."""
+        """Masked training outside `check_masked_training`'s rule or without the batch's `encoder_attention_mask`
+        (flux/model.py:813-822), conditioning latents outside the Kontext flavour, and pre-packed Kontext inputs that
+        `prepare_batch` did not build (flux/model.py:757-786) raise."""
         if check_masked_training(self.config) and batch.get("encoder_attention_mask") is None:
             raise NotImplementedError("flux_attention_masked_training: the batch has no encoder_attention_mask (the text-embed "
                                       "cache must carry attention_masks)")
-        kontext = is_kontext(self.config)
-        for k in ("conditioning_packed_latents", "conditioning_ids", "conditioning_latents"):
-            if batch.get(k) is None or (kontext and k == "conditioning_latents"):
-                continue
-            if kontext:
+        if not is_kontext(self.config):
+            return super()._check_supported(batch)
+        for k in ("conditioning_packed_latents", "conditioning_ids"):
+            if batch.get(k) is not None:
                 raise NotImplementedError(f"Kontext input `{k}` without `conditioning_latents`: the libstb200 Flux path "
                                           "packs the reference latents itself")
-            raise NotImplementedError(f"Kontext / conditioning input `{k}` is not supported by the libstb200 Flux path "
-                                      "outside model_flavour='kontext'")
 
-    def _check_loss_supported(self, prepared_batch: Dict[str, Any], apply_conditioning_mask: bool) -> None:
-        """common.py:6400-6424: with `apply_conditioning_mask` the reference multiplies the loss by the conditioning mask
-        when the dataset's `conditioning_type` is 'mask' or 'segmentation'.  Not implemented here -> raise."""
-        if not apply_conditioning_mask:
-            return
-        lm = prepared_batch.get("loss_mask_type") or prepared_batch.get("conditioning_type")   # legacy fallback, :6403-6408
-        if lm in ("mask", "segmentation"):
-            raise NotImplementedError("masked / segmentation-weighted loss is not supported by the libstb200 loss kernels")
-
-    def prepare_batch(self, batch: Dict[str, Any], state: Dict[str, Any]) -> Dict[str, Any]:
-        if not batch:
-            return batch
-        c = self.config
-        self._check_supported(batch)
-        dev = self.accelerator.device
-        kw = {"device": dev, "dtype": c.weight_dtype}
-        if batch.get("prompt_embeds") is not None:
-            batch["encoder_hidden_states"] = batch["prompt_embeds"].to(**kw, non_blocking=True)
-        pooled = batch.get("add_text_embeds")
-        batch["added_cond_kwargs"] = {}
-        if pooled is not None:
-            batch["added_cond_kwargs"]["text_embeds"] = pooled.to(**kw, non_blocking=True)
-        latents = batch.get("latent_batch")
-        if not hasattr(latents, "to"):
-            raise ValueError("Received invalid value for latents.")
-        batch["latents"] = latents.to(**kw, non_blocking=True).contiguous()
-        mask = batch.get("encoder_attention_mask")
-        if mask is not None and hasattr(mask, "to"):   # common.py:5911-5913
-            batch["encoder_attention_mask"] = mask.to(**kw, non_blocking=True)
-        # noise, then sigma draw — same order and generators as common.py:5938, 5068
-        from ..training.noise import sample_noise
-        noise, input_noise = sample_noise(c, batch["latents"], state, flow_matching=True)
-        bsz = batch["latents"].shape[0]
-        batch["noise"] = noise
-        batch["input_noise"] = input_noise.to(batch["latents"].dtype).contiguous()
-        if getattr(self, "_sigma_sampler", None) is None:   # keeps the round-robin cursor of custom timestep lists
-            from ..training.schedule import FlowSigmaSampler
-            self._sigma_sampler = FlowSigmaSampler(c, self.noise_schedule, dev)
-        sigmas, timesteps = self._model_sigmas(*self._sigma_sampler.sample(bsz, noise, state), batch["latents"])
-        batch["timesteps"] = timesteps
-        batch["sigmas"] = sigmas.view(-1, 1, 1, 1)  # expand_sigmas, common.py:6825-6828
-        # MixFlow (common.py:4962-4991): the model sees `sigmas`, the interpolation uses the slowed-down
-        # sigma + U * gamma * (1 - sigma); the extra rand_like draw happens here, after the sigma draw, as in the reference
-        interp = sigmas
-        if getattr(c, "mixflow_enabled", False) is True:
-            gamma = float(getattr(c, "mixflow_gamma", 0.8))
-            if not 0.0 <= gamma <= 1.0:
-                raise ValueError("mixflow_gamma must be between 0.0 and 1.0.")
-            slow = torch.rand_like(sigmas) if gamma > 0.0 else torch.zeros_like(sigmas)
-            interp = sigmas if gamma == 0.0 else sigmas + slow * gamma * (1.0 - sigmas)
-            batch["mixflow_slowdown_factors"] = slow
-            batch["mixflow_interpolation_sigmas"] = interp
-        cond = self._kontext_conditions(batch, state) if is_kontext(c) else None
+    def _prep_pack(self, batch: Dict[str, Any], state: Dict[str, Any], interp: torch.Tensor) -> Dict[str, Any]:
+        cond = self._kontext_conditions(batch, state) if is_kontext(self.config) else None
         if cond is None:
-            # fused: noisy = (1 - s) x + s eps  AND  2x2 patchify  (common.py:4975-4992, flux/__init__.py:25-30)
-            noisy, packed = ops.flow_prep_pack(batch["latents"], batch["input_noise"], interp.float().contiguous(),
-                                               want_unpacked=True)
-            batch["noisy_latents"] = noisy
-            batch["_packed_noisy_latents"] = packed
-            return batch
+            return super()._prep_pack(batch, state, interp)
         # Kontext: the x_embedder input [B, S_scene + S_c, 64] is filled in place, the noisy scene tokens first and then each
         # reference image's packed tokens (flux/model.py:767-779 concatenates them), with no cat / permute copies
         conds, ids = cond
-        Hh, Ww = batch["latents"].shape[2:]
+        dev = self.accelerator.device
+        bsz, C, Hh, Ww = batch["latents"].shape
         S_scene = (Hh // 2) * (Ww // 2)
         S_c = ids.shape[0]
-        joint = torch.empty((bsz, S_scene + S_c, 4 * batch["latents"].shape[1]), device=dev, dtype=torch.bfloat16)
+        joint = torch.empty((bsz, S_scene + S_c, 4 * C), device=dev, dtype=torch.bfloat16)
         noisy, _ = ops.flow_prep_pack(batch["latents"], batch["input_noise"], interp.float().contiguous(), want_unpacked=True,
                                       out=joint[:, :S_scene])
         off = S_scene
@@ -246,11 +144,6 @@ class Flux:
         batch["conditioning_packed_latents"] = joint[:, S_scene:]
         batch["conditioning_ids"] = ids.to(dev, torch.bfloat16)[None].expand(bsz, -1, -1)   # the reference's dtype
         return batch
-
-    def _model_sigmas(self, sigmas: torch.Tensor, timesteps: torch.Tensor, latents: torch.Tensor):
-        """(sigmas, timesteps) the step trains at, from the sampler's draw: Flux trains at the drawn values (Chroma
-        remaps them)."""
-        return sigmas, timesteps
 
     def _kontext_conditions(self, batch: Dict[str, Any], state: Dict[str, Any]):
         """Flux.prepare_batch_conditions (flux/model.py:522-555) then the base class's list collapse (common.py:4668-4683).
@@ -301,17 +194,14 @@ class Flux:
         raise ValueError(f"Unsupported Flux guidance mode: {c.flux_guidance_mode!r}.")
 
     def model_predict(self, prepared_batch: Dict[str, Any]) -> Dict[str, Any]:
-        """flux/model.py:707-864.  Returns the reference's dict (flux/model.py:855-864): `model_prediction` is the
-        un-packed [B, C, H, W] tensor (seam B9).  The packed token layout the loss kernel consumes rides along under the
-        private key `_packed_prediction`; `loss()` uses it when the caller has not replaced `model_prediction`."""
+        """flux/model.py:707-864."""
         pb = prepared_batch
         lat = pb["latents"]
         B, Cc, Hh, Ww = lat.shape
         dev = self.accelerator.device
         packed = pb.get("_packed_noisy_latents")
         if packed is None:
-            from .functional import pack_latents
-            packed = pack_latents(pb["noisy_latents"], B, Cc, Hh, Ww)
+            packed = self._pack(pb["noisy_latents"])
         img_ids = prepare_latent_image_ids(Hh, Ww)
         txt_ids = torch.zeros(pb["encoder_hidden_states"].shape[1], 3)
         # side effect kept from the reference: timesteps are overwritten with t / 1000 (flux/model.py:739-745)
@@ -340,71 +230,6 @@ class Flux:
             **({"conditioning_tokens": S_c} if S_c else {}),
         )[0]
         return self._prediction_dict(out, (B, Cc, Hh, Ww))
-
-    PACKED_LAYOUT = "packed"
-
-    def _prediction_dict(self, out_packed: torch.Tensor, latent_shape) -> Dict[str, Any]:
-        unpacked = self._unpack(out_packed, latent_shape)
-        return {"model_prediction": unpacked, "_packed_prediction": out_packed, "_unpacked_ref": unpacked,
-                "model_prediction_layout": self.PACKED_LAYOUT, "latent_shape": tuple(latent_shape),
-                "crepa_hidden_states": None, "hidden_states_buffer": None}
-
-    @staticmethod
-    def _unpack(out_packed: torch.Tensor, latent_shape) -> torch.Tensor:
-        from .functional import unpack_latents
-        B, Cc, Hh, Ww = latent_shape
-        return unpack_latents(out_packed, Hh * 8, Ww * 8, 16)   # flux/model.py:856-861
-
-    @staticmethod
-    def _pack(pred: torch.Tensor) -> torch.Tensor:
-        from .functional import pack_latents
-        B, Cc, Hh, Ww = pred.shape
-        return pack_latents(pred, B, Cc, Hh, Ww)
-
-    @staticmethod
-    def unpacked_prediction(model_output: Dict[str, Any]) -> torch.Tensor:
-        return model_output["model_prediction"]
-
-    def _packed_for_loss(self, model_output: Dict[str, Any]) -> torch.Tensor:
-        """The packed prediction the loss kernels read.  A caller that REPLACED `model_prediction` (e.g. the x-prediction
-        fix-up of trainer.py:6099-6105) is honoured: the private packed tensor is only used while it still describes the
-        same object; a bare `{"model_prediction": packed_tensor}` (3-D) is accepted as already packed."""
-        pred = model_output["model_prediction"]
-        packed = model_output.get("_packed_prediction")
-        if packed is not None and model_output.get("_unpacked_ref") is pred:
-            return packed
-        if pred.dim() == 3:
-            return pred
-        return self._pack(pred).contiguous()
-
-    # ------------------------------------------------------------------------------------------
-    def loss(self, prepared_batch: Dict[str, Any], model_output: Dict[str, Any], apply_conditioning_mask: bool = True):
-        """common.py:6217-6430, flow-matching / l2 branch: target = noise - latents (common.py:4610-4611),
-        mse in fp32, mean over (C,H,W) then over the batch."""
-        self._check_loss_supported(prepared_batch, apply_conditioning_mask)
-        return FlowLossFn.apply(self._packed_for_loss(model_output), prepared_batch["latents"], prepared_batch["noise"],
-                                self.LOSS_LAYOUT, *self._loss_kind(prepared_batch))
-
-    LOSS_LAYOUT = 0   # packed prediction feature order: 0 = (c, dy, dx) Flux, 1 = (dy, dx, c) SD3 / PixArt
-
-    def _loss_kind(self, prepared_batch):
-        """loss_type / per-sample huber_c (common.py:6230-6284).  For flow matching the reference ignores snr_gamma."""
-        c = self.config
-        lt = getattr(c, "loss_type", "l2")
-        if lt == "l2":
-            return "l2", None
-        if lt not in ("huber", "smooth_l1"):
-            raise NotImplementedError(f"Unsupported Loss Type {lt}")
-        from ..training.noise import compute_scheduled_huber_c
-        # NB: Flux.model_predict has overwritten `timesteps` with t / 1000 (flux/model.py:739-745) before loss() runs; the
-        # reference feeds those scaled values to compute_scheduled_huber_c as they are, and so does this mirror.
-        t = prepared_batch["timesteps"]
-        if t.dim() == 2:        # Kontext [B, S_scene + S_c]: validate_config allows only the constant c here
-            t = t[:, 0]
-        return lt, compute_scheduled_huber_c(c, self.noise_schedule, t.to(self.accelerator.device), self.PREDICTION_TYPE)
-
-    def loss_with_logs(self, prepared_batch, model_output, apply_conditioning_mask: bool = True):
-        return self.loss(prepared_batch, model_output, apply_conditioning_mask), None
 
 
 def is_kontext(c) -> bool:

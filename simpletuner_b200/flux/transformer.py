@@ -555,25 +555,30 @@ class AdapterModelAPI:
             raise NotImplementedError("fused LoRA path supports rank 1..128 (one 128-wide rank block per adapted Linear)")
         lora_alpha = float(lora_alpha) if lora_alpha is not None else float(rank)  # common.py:1090-1093
         targets = list(target_modules) if target_modules is not None else list(self._DEFAULT_LORA_TARGETS)
-        n = 0
-        chosen = []
+        chosen = self.lora_target_linears(targets)
+        if not chosen:
+            raise ValueError(f"no module matched LoRA targets {targets}")
+        for mod in chosen.values():
+            mod.add_lora(rank, lora_alpha, adapter_name)
+        self._lora_scaling = lora_alpha / rank
+        self._lora_dropout_p = lora_dropout
+        self.peft_config[adapter_name] = SimpleNamespace(r=rank, lora_alpha=lora_alpha, target_modules=targets,
+                                                         lora_dropout=lora_dropout)
+        return len(chosen)
+
+    def lora_target_linears(self, targets: Sequence[str]) -> Dict[str, Linear]:
+        """The Linears PEFT's suffix rule selects for `targets` (a qualified name equal to a target or ending with
+        ".<target>").  Raises NotImplementedError naming the first one the block schedules cannot adapt; the shim calls
+        this at load time so that such a run keeps the reference module."""
+        chosen = {}
         for name, mod in self.named_modules():
             if not isinstance(mod, Linear) or not _peft_match(name, targets):
                 continue
             if not self._lora_adaptable(name):
                 raise NotImplementedError(f"LoRA target {name} is not supported by the fused path (use the reference "
                                           "module, e.g. for the adaLN linears of flux_lora_target=ai-toolkit)")
-            chosen.append(mod)
-        for mod in chosen:
-            mod.add_lora(rank, lora_alpha, adapter_name)
-            n += 1
-        if n == 0:
-            raise ValueError(f"no module matched LoRA targets {targets}")
-        self._lora_scaling = lora_alpha / rank
-        self._lora_dropout_p = lora_dropout
-        self.peft_config[adapter_name] = SimpleNamespace(r=rank, lora_alpha=lora_alpha, target_modules=targets,
-                                                         lora_dropout=lora_dropout)
-        return n
+            chosen[name] = mod
+        return chosen
 
     def disable_lora(self):
         for m in self.lora_linears().values():

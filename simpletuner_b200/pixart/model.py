@@ -17,15 +17,16 @@ the loss, the tail GEMM only computes the 16 kept features.
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import Any, Dict, Optional
+from typing import Any, Dict
 
 import torch
 
 from .. import ops
-from ..flux.model import Flux, default_config as _flux_defaults
+from ..family import LOSS_LAYOUT, StepWrapper
+from ..flux.model import default_config as _flux_defaults
 from ..training.noise import make_ddpm_schedule, min_snr_loss_weights
 from ..training.schedule import generate_timestep_weights, segmented_timestep_selection
-from .transformer import PIXART_LORA_TARGETS, PixArtTransformer2DModel
+from .transformer import PixArtTransformer2DModel
 
 
 def default_config(**over) -> SimpleNamespace:
@@ -53,43 +54,18 @@ class _TargetLossFn(torch.autograd.Function):
         return (dpred.float() * g.float()).to(dpred.dtype), None, None, None, None, None, None   # fp32 scale, see FlowLossFn
 
 
-class PixartSigma(Flux):
+class PixartSigma(StepWrapper):
     NAME = "PixArt Sigma"
     PREDICTION_TYPE = "epsilon"
+    PREDICTION_TYPES = ("epsilon", "v_prediction")
     LATENT_CHANNEL_COUNT = 4
-    DEFAULT_LORA_TARGET = PIXART_LORA_TARGETS
-    LOSS_LAYOUT = 1
+    DENOISER = PixArtTransformer2DModel
+    DEFAULT_CONFIG = staticmethod(default_config)
+    PACKED_LAYOUT = "packed_dydxc"
 
-    def __init__(self, config: Optional[SimpleNamespace] = None, transformer: Optional[PixArtTransformer2DModel] = None,
-                 device: Optional[torch.device] = None, **transformer_kwargs):
-        self.config = config or default_config()
-        dev = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
-        self.accelerator = SimpleNamespace(device=dev)
+    def _noise_schedule(self):
         # PixArt-Sigma scheduler_config.json: DDPM, 1000 steps, linear betas 1e-4 .. 0.02, epsilon
-        self.noise_schedule = make_ddpm_schedule(1000, 0.0001, 0.02, "linear")
-        self.model = transformer if transformer is not None else PixArtTransformer2DModel(**transformer_kwargs)
-        self._sched_dev: Dict[Any, Any] = {}
-        pt = getattr(self.config, "prediction_type", None)      # pixart/model.py:698-700
-        if pt is not None:
-            if pt not in ("epsilon", "v_prediction"):
-                raise NotImplementedError(f"prediction_type {pt} is not implemented for the B200 PixArt step")
-            self.PREDICTION_TYPE = pt
-            self.noise_schedule.config.prediction_type = pt
-
-    def add_lora_adapter(self):
-        c = self.config
-        alpha = c.lora_alpha if c.lora_alpha is not None else c.lora_rank
-        return self._denoiser().add_adapter(rank=c.lora_rank, lora_alpha=alpha, target_modules=PIXART_LORA_TARGETS,
-                                            lora_dropout=getattr(c, "lora_dropout", 0.0))
-
-    def _coefs(self, timesteps: torch.Tensor, dev):
-        tab = self._sched_dev.get(dev)
-        if tab is None:
-            ac = self.noise_schedule.alphas_cumprod.to(dev)
-            tab = (ac ** 0.5, (1 - ac) ** 0.5)   # DDPMScheduler.add_noise: fp32 tables, gathered per sample
-            self._sched_dev[dev] = tab
-        t = timesteps.to(dev)
-        return tab[0][t].contiguous(), tab[1][t].contiguous()
+        return make_ddpm_schedule(1000, 0.0001, 0.02, "linear")
 
     def prepare_batch(self, batch: Dict[str, Any], state: Dict[str, Any]) -> Dict[str, Any]:
         if not batch:
@@ -118,7 +94,7 @@ class PixartSigma(Flux):
             batch["timesteps"] = segmented_timestep_selection(n_t, bsz, weights, c, use_refiner_range=False).to(dev)
         else:
             batch["timesteps"] = torch.multinomial(weights, bsz, replacement=True).long()
-        ca, cb = self._coefs(batch["timesteps"], dev)
+        ca, cb = self._ddpm_coefs(batch["timesteps"], dev)
         noisy, packed = ops.ddpm_prep_pack(batch["latents"], batch["input_noise"], ca, cb, want_unpacked=True, want_packed=True)
         batch["noisy_latents"] = noisy
         batch["_packed_noisy_latents"] = packed
@@ -156,12 +132,7 @@ class PixartSigma(Flux):
         if Cc != self.LATENT_CHANNEL_COUNT:
             raise ValueError(f"{self.NAME} requires a latent size of {self.LATENT_CHANNEL_COUNT} channels. "
                              "Ensure you are using the correct VAE cache path.")
-        dev = self.accelerator.device
-        timesteps = pb["timesteps"].to(dev)
-        if timesteps.ndim == 0 or (timesteps.ndim == 1 and timesteps.shape[0] == 1):
-            timesteps = timesteps.reshape(-1).expand(B)
-        elif timesteps.ndim != 1 or timesteps.shape[0] != B:
-            raise ValueError(f"PixArt expected 1 timestep or {B} per-batch timesteps, got {tuple(timesteps.shape)}.")
+        timesteps = self._batch_timesteps(pb["timesteps"].to(self.accelerator.device), B)
         mask = pb.get("encoder_attention_mask")
         out = self.model(
             pb["noisy_latents"], encoder_hidden_states=pb["encoder_hidden_states"], timestep=timesteps,
@@ -169,19 +140,6 @@ class PixartSigma(Flux):
             _packed_latents=pb.get("_packed_noisy_latents"), _packed_output="eps_half",
         )[0]
         return self._prediction_dict(out, (B, Cc, Hh, Ww))
-
-    PACKED_LAYOUT = "packed_dydxc"
-
-    @staticmethod
-    def _unpack(out_packed: torch.Tensor, latent_shape) -> torch.Tensor:
-        B, Cc, Hh, Ww = latent_shape
-        o = out_packed.reshape(B, Hh // 2, Ww // 2, 2, 2, Cc)
-        return torch.einsum("nhwpqc->nchpwq", o).reshape(B, Cc, Hh, Ww)
-
-    @staticmethod
-    def _pack(pred: torch.Tensor) -> torch.Tensor:
-        B, Cc, Hh, Ww = pred.shape
-        return pred.reshape(B, Cc, Hh // 2, 2, Ww // 2, 2).permute(0, 2, 4, 3, 5, 1).reshape(B, (Hh // 2) * (Ww // 2), 4 * Cc)
 
     def loss(self, prepared_batch, model_output, apply_conditioning_mask: bool = True):
         c = self.config
@@ -200,4 +158,5 @@ class PixartSigma(Flux):
                                   prepared_batch["timesteps"]).contiguous()
         else:
             target = prepared_batch["noise"]
-        return _TargetLossFn.apply(self._packed_for_loss(model_output), target, weights, snr_w, lt, hc)
+        return _TargetLossFn.apply(self._packed_for_loss(model_output), target, weights, snr_w, lt, hc,
+                                   LOSS_LAYOUT[self.PACKED_LAYOUT])

@@ -1,7 +1,7 @@
 """Qwen-Image training wrapper on libstb200: the step methods of reference `QwenImage` (qwen_image/model.py) for the
 text-to-image flavours v1.0 (Qwen/Qwen-Image) and v2.0 (Qwen/Qwen-Image-2512), LoRA only.
 
-  * `prepare_batch`   common.py:5862-6041 (flow-matching branch), as for Flux
+  * `prepare_batch`   common.py:5862-6041 (flow-matching branch), the shared StepWrapper draw
   * `model_predict`   qwen_image/model.py:1227-1345 (`_model_predict_standard`)
   * `loss` / `loss_with_logs`  common.py:6217-6430
 
@@ -13,16 +13,14 @@ B = 1 batch) runs the attention kernels without a bias.
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import Any, Dict, Optional
+from typing import Any, Dict
 
 import torch
 
 from .. import ops
+from ..family import LOSS_LAYOUT, StepWrapper
 from ..flux.blocks import FlowLossFn
-from ..flux.model import Flux
-from .transformer import QWEN_DEFAULT_LORA_TARGETS, QwenImageTransformer2DModel, _ADAPTABLE_SUFFIXES, mask_hides_keys
-
-FLAVOURS = ("v1.0", "v2.0")        # reference qwen_image/model.py:82-89; the edit flavours stay on the reference class
+from .transformer import QwenImageTransformer2DModel, mask_hides_keys
 
 
 def default_config(**over) -> SimpleNamespace:
@@ -37,81 +35,26 @@ def default_config(**over) -> SimpleNamespace:
     return SimpleNamespace(**cfg)
 
 
-def lora_targets(c) -> list:
-    """get_lora_target_layers (common.py:952-1007): `peft_lora_target_modules` when given, else the family default."""
-    t = getattr(c, "peft_lora_target_modules", None)
-    return list(t) if t else list(QWEN_DEFAULT_LORA_TARGETS)
-
-
-class QwenImage(Flux):
-    """Drop-in for the reference `QwenImage(ImageModelFoundation)` step methods.  Shares Flux's noise / sigma sampling,
-    prediction dict and loss plumbing; the denoiser and the batch conventions are Qwen's."""
+class QwenImage(StepWrapper):
+    """Drop-in for the reference `QwenImage(ImageModelFoundation)` step methods.  The flow-matching draw, prediction dict and
+    loss plumbing are the shared StepWrapper's; the denoiser, the 5-D latents and the prompt mask are Qwen's."""
 
     NAME = "Qwen-Image"
     # prepare_batch decides on the host whether the prompt mask hides a key, and the two answers take different kernels:
     # a replayed graph would keep the first batch's choice
     GRAPH_REPLAY = False
+    DENOISER = QwenImageTransformer2DModel
+    DEFAULT_CONFIG = staticmethod(default_config)
+    FLAVOURS = ("v1.0", "v2.0")        # reference qwen_image/model.py:82-89; the edit flavours stay on the reference class
+    # block swap is not implemented here, and flow-map and MixFlow training are not checked against the reference's Qwen step
+    REFUSED_OPTIONS = ("musubi_blocks_to_swap", "flowmap_enabled", "flow_map_enabled", "mixflow_enabled")
+    REFUSED_BATCH_KEYS = ("conditioning_latents", "conditioning_packed_latents", "control_latent_list",
+                          "conditioning_image_embeds")      # the edit flavours' inputs
 
-    def __init__(self, config: Optional[SimpleNamespace] = None, transformer: Optional[QwenImageTransformer2DModel] = None,
-                 device: Optional[torch.device] = None, **transformer_kwargs):
-        self.config = config or default_config()
-        dev = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
-        self.accelerator = SimpleNamespace(device=dev)
+    def _noise_schedule(self):
         # reference setup_training_noise_schedule (qwen_image/model.py:348-370)
-        self.noise_schedule = SimpleNamespace(config=SimpleNamespace(num_train_timesteps=1000, base_image_seq_len=256,
-                                                                       max_image_seq_len=8192, base_shift=0.5, max_shift=0.9))
-        self.model = transformer if transformer is not None else QwenImageTransformer2DModel(**transformer_kwargs)
-
-    def add_lora_adapter(self):
-        c = self.config
-        alpha = c.lora_alpha if c.lora_alpha is not None else c.lora_rank
-        return self._denoiser().add_adapter(rank=c.lora_rank, lora_alpha=alpha, target_modules=lora_targets(c),
-                                            lora_dropout=getattr(c, "lora_dropout", 0.0))
-
-    def add_lycoris_adapter(self, lycoris_config):
-        raise NotImplementedError("LyCORIS adapters on Qwen-Image are not supported by the libstb200 path")
-
-    @classmethod
-    def validate_config(cls, c) -> None:
-        """Every option of the reference this path does not run raises NotImplementedError, so that the shim keeps the
-        reference class for it."""
-        g = lambda k, d=None: getattr(c, k, d)
-        fl = g("model_flavour", None) or "v2.0"
-        if fl not in FLAVOURS:
-            raise NotImplementedError(f"Qwen-Image model_flavour={fl!r} (control latents / zero_cond_t) is not supported by "
-                                      f"the libstb200 path (supported: {FLAVOURS})")
-        if g("controlnet", False):
-            raise NotImplementedError("controlnet training is not supported by the libstb200 path")
-        if str(g("model_type", "lora")) != "lora":
-            raise NotImplementedError(f"model_type={g('model_type')!r}: only LoRA training runs on the libstb200 path")
-        lt = str(g("lora_type", "standard") or "standard").lower()
-        if lt != "standard":
-            raise NotImplementedError(f"lora_type={g('lora_type')!r} on Qwen-Image is not supported by the libstb200 path")
-        if g("use_dora", False):
-            raise NotImplementedError("DoRA is not supported by the libstb200 path")
-        if g("slider_lora_target", False):
-            raise NotImplementedError("slider LoRA targets are not supported by the libstb200 Qwen-Image path")
-        for t in lora_targets(c):
-            if not ("." + t).endswith(_ADAPTABLE_SUFFIXES):
-                raise NotImplementedError(f"LoRA target {t!r} is not supported by the libstb200 Qwen-Image path (adaLN, "
-                                          "embedder and output linears stay on the reference module)")
-        if g("tread_config", None):
-            raise NotImplementedError("TREAD routing is not supported by the libstb200 path")
-        if g("musubi_blocks_to_swap", 0):
-            raise NotImplementedError("musubi block swap is not supported by the libstb200 path")
-        if g("flow_cubic_schedule", None) or g("flow_cubic_schedule_weights", None):
-            raise NotImplementedError("the cubic-spline flow schedule is not part of the libstb200 step")
-        for flag in ("twinflow_enabled", "crepa_enabled", "layersync_enabled", "scheduled_sampling_max_step_offset",
-                     "diff2flow_enabled", "flowmap_enabled", "flow_map_enabled", "mixflow_enabled"):
-            if g(flag, None):
-                raise NotImplementedError(f"{flag} is not supported by the libstb200 path")
-        if g("distillation_method", None) not in (None, "", "None"):
-            raise NotImplementedError("distillation is not supported by the libstb200 path")
-
-    def _check_supported(self, batch: Dict[str, Any]) -> None:
-        for k in ("conditioning_latents", "conditioning_packed_latents", "control_latent_list", "conditioning_image_embeds"):
-            if batch.get(k) is not None:
-                raise NotImplementedError(f"Qwen-Image edit input `{k}` is not supported by the libstb200 path")
+        return SimpleNamespace(config=SimpleNamespace(num_train_timesteps=1000, base_image_seq_len=256, max_image_seq_len=8192,
+                                                      base_shift=0.5, max_shift=0.9))
 
     def prepare_batch(self, batch: Dict[str, Any], state: Dict[str, Any]) -> Dict[str, Any]:
         if not batch:
@@ -138,18 +81,10 @@ class QwenImage(Flux):
             # host decision before the upload: a mask that hides no key needs no bias (no device sync either way)
             batch["_qwen_masked_keys"] = True if mask.is_cuda else mask_hides_keys(mask)
             batch["encoder_attention_mask"] = mask.to(**kw, non_blocking=True)
-        from ..training.noise import sample_noise
-        noise, input_noise = sample_noise(c, lat4, state, flow_matching=True)
-        batch["noise"] = noise.view(lat.shape)
-        batch["input_noise"] = input_noise.to(lat.dtype).contiguous().view(lat.shape)
-        if getattr(self, "_sigma_sampler", None) is None:
-            from ..training.schedule import FlowSigmaSampler
-            self._sigma_sampler = FlowSigmaSampler(c, self.noise_schedule, dev)
-        sigmas, timesteps = self._sigma_sampler.sample(lat.shape[0], noise, state)
-        batch["timesteps"] = timesteps
-        batch["sigmas"] = sigmas.view(-1, 1, 1, 1)
-        noisy, packed = ops.flow_prep_pack(lat4, batch["input_noise"].view(lat4.shape), sigmas.float().contiguous(),
-                                           want_unpacked=True)
+        sigmas = self._flow_draw(batch, state, lat4)
+        noisy, packed = ops.flow_prep_pack(lat4, batch["input_noise"], sigmas.float().contiguous(), want_unpacked=True)
+        batch["noise"] = batch["noise"].view(lat.shape)
+        batch["input_noise"] = batch["input_noise"].view(lat.shape)
         batch["noisy_latents"] = noisy.view(lat.shape)
         batch["_packed_noisy_latents"] = packed
         return batch
@@ -167,13 +102,8 @@ class QwenImage(Flux):
         dev = self.accelerator.device
         packed = pb.get("_packed_noisy_latents")
         if packed is None:
-            noisy = pb["noisy_latents"]
-            packed = self._pack(noisy.squeeze(2) if noisy.dim() == 5 else noisy)
-        t = pb["timesteps"].to(device=dev, dtype=torch.float32)
-        if t.ndim == 0 or (t.ndim == 1 and t.shape[0] == 1):
-            t = t.reshape(1).expand(B)
-        if t.ndim != 1:
-            raise NotImplementedError("token-wise timesteps are not supported by the libstb200 Qwen-Image path")
+            packed = self._pack(pb["noisy_latents"])
+        t = self._batch_timesteps(pb["timesteps"].to(device=dev, dtype=torch.float32), B)
         mask = pb.get("encoder_attention_mask")
         if mask is not None and not pb.get("_qwen_masked_keys", True):
             mask = None
@@ -187,13 +117,19 @@ class QwenImage(Flux):
             res["model_prediction"] = res["_unpacked_ref"] = res["model_prediction"].unsqueeze(2)
         return res
 
-    @staticmethod
-    def _pack(pred: torch.Tensor) -> torch.Tensor:
-        return Flux._pack(pred.squeeze(2) if pred.dim() == 5 else pred)
+    @classmethod
+    def _pack(cls, pred: torch.Tensor) -> torch.Tensor:
+        return super()._pack(pred.squeeze(2) if pred.dim() == 5 else pred)
 
     def loss(self, prepared_batch: Dict[str, Any], model_output: Dict[str, Any], apply_conditioning_mask: bool = True):
         self._check_loss_supported(prepared_batch, apply_conditioning_mask)
         lat, noise = prepared_batch["latents"], prepared_batch["noise"]
         if lat.dim() == 5:
             lat, noise = lat.squeeze(2), noise.squeeze(2)
-        return FlowLossFn.apply(self._packed_for_loss(model_output), lat, noise, self.LOSS_LAYOUT, *self._loss_kind(prepared_batch))
+        return FlowLossFn.apply(self._packed_for_loss(model_output), lat, noise, LOSS_LAYOUT[self.PACKED_LAYOUT],
+                                *self._loss_kind(prepared_batch))
+
+
+def lora_targets(c) -> list:
+    """`QwenImage.lora_targets` as a module function."""
+    return QwenImage.lora_targets(c)

@@ -1,40 +1,25 @@
 """SD3 training wrapper on libstb200 — mirror of the step-level API of reference
 simpletuner/helpers/models/sd3/model.py (class SD3): `prepare_batch` (common.py:5862-6041, flow-matching
-branch — identical to Flux), `model_predict` (`_model_predict_single`, sd3/model.py:540-569) and `loss`
+branch — the shared StepWrapper's), `model_predict` (`_model_predict_single`, sd3/model.py:540-569) and `loss`
 (common.py:6217-6430, l2).  Differences from Flux that are reproduced here: latents go to the denoiser
 un-packed [B,16,H,W]; timesteps are passed RAW (0..1000) after a cast to the bf16 weight dtype (quirk Q8);
 no guidance input; pooled projections are 2048-wide; the prediction is un-patchified in (dy, dx, c) order.
 """
 from __future__ import annotations
 
-from types import SimpleNamespace
-from typing import Any, Dict, Optional
+from typing import Any, Dict
 
-import torch
-
-from ..flux.blocks import FlowLossFn
-from ..flux.model import Flux, default_config
-from .transformer import SD3_LORA_TARGETS, SD3Transformer2DModel
+from ..family import CONDITIONING_INPUTS, StepWrapper
+from ..flux.model import default_config
+from .transformer import SD3Transformer2DModel
 
 
-class SD3(Flux):
+class SD3(StepWrapper):
     NAME = "Stable Diffusion 3.x"
-
-    def __init__(self, config: Optional[SimpleNamespace] = None, transformer: Optional[SD3Transformer2DModel] = None,
-                 device: Optional[torch.device] = None, **transformer_kwargs):
-        self.config = config or default_config()
-        dev = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
-        self.accelerator = SimpleNamespace(device=dev)
-        self.noise_schedule = SimpleNamespace(config=SimpleNamespace(num_train_timesteps=1000, patch_size=2,
-                                                                       base_image_seq_len=256, max_image_seq_len=4096,
-                                                                       base_shift=0.5, max_shift=1.15))
-        self.model = transformer if transformer is not None else SD3Transformer2DModel(**transformer_kwargs)
-
-    def add_lora_adapter(self):
-        c = self.config
-        alpha = c.lora_alpha if c.lora_alpha is not None else c.lora_rank
-        return self._denoiser().add_adapter(rank=c.lora_rank, lora_alpha=alpha, target_modules=SD3_LORA_TARGETS,
-                                            lora_dropout=getattr(c, "lora_dropout", 0.0))
+    DENOISER = SD3Transformer2DModel
+    DEFAULT_CONFIG = staticmethod(default_config)
+    PACKED_LAYOUT = "packed_dydxc"
+    REFUSED_BATCH_KEYS = CONDITIONING_INPUTS
 
     def model_predict(self, prepared_batch: Dict[str, Any]) -> Dict[str, Any]:
         pb = prepared_batch
@@ -48,18 +33,3 @@ class SD3(Flux):
             _packed_latents=pb.get("_packed_noisy_latents"), _packed_output=True,
         )[0]
         return self._prediction_dict(out, (B, Cc, Hh, Ww))
-
-    PACKED_LAYOUT = "packed_dydxc"
-
-    @staticmethod
-    def _unpack(out_packed: torch.Tensor, latent_shape) -> torch.Tensor:
-        B, Cc, Hh, Ww = latent_shape
-        o = out_packed.reshape(B, Hh // 2, Ww // 2, 2, 2, Cc)
-        return torch.einsum("nhwpqc->nchpwq", o).reshape(B, Cc, Hh, Ww)
-
-    @staticmethod
-    def _pack(pred: torch.Tensor) -> torch.Tensor:
-        B, Cc, Hh, Ww = pred.shape
-        return pred.reshape(B, Cc, Hh // 2, 2, Ww // 2, 2).permute(0, 2, 4, 3, 5, 1).reshape(B, (Hh // 2) * (Ww // 2), 4 * Cc)
-
-    LOSS_LAYOUT = 1

@@ -18,7 +18,8 @@ from typing import Any, Dict, Optional
 import torch
 
 from .. import ops
-from ..pixart.model import PixartSigma, _TargetLossFn, default_config as _eps_defaults
+from ..family import CONDITIONING_INPUTS, StepWrapper
+from ..pixart.model import _TargetLossFn, default_config as _eps_defaults
 from ..training.noise import (gather_conditional_sdxl_size_features, make_ddpm_schedule, min_snr_loss_weights)
 from ..training.schedule import generate_timestep_weights, segmented_timestep_selection
 
@@ -30,26 +31,19 @@ def default_config(**over) -> SimpleNamespace:
     return SimpleNamespace(**cfg)
 
 
-class SDXL(PixartSigma):
+class SDXL(StepWrapper):
     NAME = "Stable Diffusion XL"
     PREDICTION_TYPE = "epsilon"
-    LATENT_CHANNEL_COUNT = 4
-    LOSS_LAYOUT = 2            # the UNet returns [B, C, H, W]
+    PREDICTION_TYPES = ("epsilon", "v_prediction")
+    DEFAULT_CONFIG = staticmethod(default_config)
+    REFUSED_BATCH_KEYS = CONDITIONING_INPUTS
 
     def __init__(self, config: Optional[SimpleNamespace] = None, unet=None, device: Optional[torch.device] = None):
-        self.config = config or default_config()
-        dev = device or torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
-        self.accelerator = SimpleNamespace(device=dev)
+        super().__init__(config, transformer=unet, device=device)
+
+    def _noise_schedule(self):
         # SDXL scheduler_config.json: DDPM, 1000 steps, scaled_linear betas 0.00085 .. 0.012, epsilon (v for some finetunes)
-        self.noise_schedule = make_ddpm_schedule(1000, 0.00085, 0.012, "scaled_linear")
-        self.model = unet
-        self._sched_dev: Dict[Any, Any] = {}
-        pt = getattr(self.config, "prediction_type", None)
-        if pt is not None:
-            if pt not in ("epsilon", "v_prediction"):
-                raise NotImplementedError(f"prediction_type {pt} is not implemented for the B200 SDXL step")
-            self.PREDICTION_TYPE = pt
-            self.noise_schedule.config.prediction_type = pt
+        return make_ddpm_schedule(1000, 0.00085, 0.012, "scaled_linear")
 
     def add_lora_adapter(self):
         raise NotImplementedError("SDXL LoRA attaches to the reference UNet (PEFT); the libstb200 step only wraps the UNet call")
@@ -89,7 +83,7 @@ class SDXL(PixartSigma):
             batch["timesteps"] = segmented_timestep_selection(n_t, bsz, weights, c, use_refiner_range=False).to(dev)
         else:
             batch["timesteps"] = torch.multinomial(weights, bsz, replacement=True).long()
-        ca, cb = self._coefs(batch["timesteps"], dev)
+        ca, cb = self._ddpm_coefs(batch["timesteps"], dev)
         noisy, _ = ops.ddpm_prep_pack(batch["latents"], batch["input_noise"], ca, cb, want_unpacked=True, want_packed=False)
         batch["noisy_latents"] = noisy
         return batch

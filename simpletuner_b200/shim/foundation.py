@@ -153,6 +153,8 @@ class B200FoundationMixin:
     def _b200_install(self):
         import torch
 
+        from ..family import lora_type
+
         spec = family_spec(self.B200_FAMILY)
         ref = self.model
         if ref is None:
@@ -164,13 +166,13 @@ class B200FoundationMixin:
             raise NotImplementedError(f"libstb200 computes in bf16; weight_dtype={dtype}")
         step_cls = spec.step()
         step_cls.validate_config(self.config)                      # raises NotImplementedError on unsupported options
-        if str(getattr(self.config, "lora_type", "standard") or "standard").lower() == "lycoris":
+        if lora_type(self.config) == "lycoris" and not _LYCORIS_ROUTED:
             # trainer.py:3391 calls the third-party `lycoris.create_lycoris` on the trained component; that wrapper only knows
             # torch.nn modules.  Only with `install_lycoris()` (which routes B200 denoisers to simpletuner_b200.lycoris) may
-            # the swap happen for a LyCORIS run — and only for the families whose block schedules carry LoKr.
-            if not _LYCORIS_ROUTED or self.B200_FAMILY != "flux":
-                raise NotImplementedError("LyCORIS run: call simpletuner_b200.shim.install_lycoris() first (Flux LoKr only)")
+            # the swap happen for a LyCORIS run (validate_config admits it only where the block schedules carry LoKr).
+            raise NotImplementedError("LyCORIS run: call simpletuner_b200.shim.install_lycoris() first (Flux LoKr only)")
         den = spec.denoiser()(**kwargs)
+        den.lora_target_linears(step_cls.lora_targets(self.config))     # a target the fused path cannot adapt raises here
         missing, unexpected = den.load_state_dict(ref.state_dict(), strict=False)
         missing = [k for k in missing if "lora_" not in k]
         unexpected = [k for k in unexpected if "lora_" not in k]

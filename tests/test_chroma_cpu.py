@@ -168,9 +168,12 @@ def test_target_lists_differ_from_flux_where_the_reference_does():
     (dict(model_flavour="kontext"), "model_flavour"), (dict(peft_lora_target_modules=["linear_1"]), "linear_1"),
     (dict(peft_lora_target_modules=["context_embedder"]), "context_embedder"),
 ])
-def test_validate_config_refusals(over, what):
+def test_unsupported_options_are_refused_at_load(over, what):
+    """What the shim refuses at load: validate_config, then the denoiser's rule for the resolved LoRA targets."""
+    c = default_config(**over)
     with pytest.raises(NotImplementedError, match=what):
-        Chroma.validate_config(default_config(**over))
+        Chroma.validate_config(c)
+        ChromaTransformer2DModel(**TINY).lora_target_linears(Chroma.lora_targets(c))
 
 
 def test_model_and_batch_refusals():

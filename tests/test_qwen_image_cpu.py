@@ -117,9 +117,12 @@ def test_qkv_parameters_share_one_fused_tensor():
     (dict(musubi_blocks_to_swap=10), "musubi"),
     (dict(controlnet=True), "controlnet"),
 ])
-def test_unsupported_options_raise(over, needle):
+def test_unsupported_options_are_refused_at_load(over, needle):
+    """What the shim refuses at load: validate_config, then the denoiser's rule for the resolved LoRA targets."""
+    c = default_config(**over)
     with pytest.raises(NotImplementedError, match=needle):
-        QwenImage.validate_config(default_config(**over))
+        QwenImage.validate_config(c)
+        QwenImageTransformer2DModel(**TINY).lora_target_linears(QwenImage.lora_targets(c))
 
 
 def test_supported_flavours_validate():
