@@ -337,7 +337,7 @@ int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm
  *                      stride 1: padding 1;  stride 2: F.pad(x,(0,1,0,1)) then stride-2 (Downsample2D)
  *   stb_conv_in_3ch  : conv_in on the NCHW pixel tensor [B,3,H,W] (w OIHW [C,3,3,3]) -> NHWC [B,H,W,C]
  *   stb_groupnorm_nhwc : GroupNorm(G, eps, affine) (+ SiLU) over NHWC; stats = fp32 scratch [B*G*2]
- *   stb_softmax_rows : in-place softmax(scale * s) over rows of the mid-block attention scores
+ *   stb_softmax_rows : in-place softmax(scale * s) over rows of the mid-block attention scores (scale > 0)
  *   stb_gaussian_sample_scale : z = (mean + exp(.5 clamp(logvar,-30,20)) * eps - shift) * scale, NHWC moments
  *                      [B,h*w,2L] + NCHW eps [B,L,h,w] -> NCHW latents [B,L,h,w]
  * ------------------------------------------------------------------------------------------- */

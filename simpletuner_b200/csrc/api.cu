@@ -1086,7 +1086,10 @@ int stb_conv_in_3ch(const void* pixels, const void* w, const void* bias, void* o
 int stb_groupnorm_nhwc(const void* x, const void* gamma, const void* beta, void* out, float* stats, int B, int HW,
                        int C, int G, float eps, int silu, void* stream) {
   if (int r = check_device()) return r;
+  if (!x || !gamma || !beta || !out || !stats || B < 1 || HW < 1 || C < 8 || G < 1) return fail(STB_ERR_ARG, "groupnorm_nhwc: bad arguments");
   if (C % 8 || C > 512 || G > 64 || C % G || (8 % (C / G) && (C / G) % 8)) return fail(STB_ERR_ARG, "groupnorm_nhwc: unsupported C=%d G=%d", C, G);
+  if (!aligned16(x) || !aligned16(out) || !aligned16(gamma) || !aligned16(beta))
+    return fail(STB_ERR_ARG, "groupnorm_nhwc: x, out, gamma and beta must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   STB_CUDA(cudaMemsetAsync(stats, 0, sizeof(float) * 2 * B * G, st));
   const int chunks = std::max(1, std::min((HW + 255) / 256, (num_sms() * 4 + B - 1) / B));
@@ -1104,6 +1107,8 @@ int stb_groupnorm_nhwc(const void* x, const void* gamma, const void* beta, void*
 
 int stb_softmax_rows(void* s, long long row_stride, int rows, int cols, float scale, void* stream) {
   if (int r = check_device()) return r;
+  // the kernel takes the row max of the unscaled logits, which is the max of the scaled ones only for scale > 0
+  if (!s || rows < 1 || cols < 8 || !(scale > 0.f)) return fail(STB_ERR_ARG, "softmax_rows: bad arguments (rows >= 1, cols >= 8, scale > 0)");
   if (cols % 8 || (row_stride & 7) || !aligned16(s)) return fail(STB_ERR_ARG, "softmax_rows alignment");
   stb::softmax_rows_kernel<<<rows, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<__nv_bfloat16*>(s), row_stride, cols, scale);
   STB_LAUNCH_CHECK("softmax_rows");
@@ -1113,6 +1118,7 @@ int stb_softmax_rows(void* s, long long row_stride, int rows, int cols, float sc
 int stb_gaussian_sample_scale(const void* moments, const void* eps, void* out, int B, int L, int hw, float shift,
                               float scale, int has_shift, void* stream) {
   if (int r = check_device()) return r;
+  if (!moments || !eps || !out || B < 1 || L < 1 || hw < 1) return fail(STB_ERR_ARG, "gaussian_sample_scale: bad arguments");
   const long long total = (long long)B * L * hw;
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 8);
   stb::gaussian_sample_scale_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(

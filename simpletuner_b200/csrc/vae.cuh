@@ -2,7 +2,7 @@
 // Activations are NHWC bf16 so that every 3x3 / 1x1 conv is a wgmma GEMM over pixels
 // (gemm.cuh, CONV mode: 9 shifted K-segments whose halo TMA zero-fills).  Here: the HBM-bound pieces.
 //   conv_in_3ch_kernel     : 3 -> C conv3x3 on the NCHW pixel tensor (K = 27: CUDA cores), writes NHWC
-//   groupnorm_stats_kernel : per (image, group) sum / sum-of-squares over H*W*(C/G)   (fp32 atomics)
+//   groupnorm_stats_kernel : per (image, group) sum / sum-of-squares of x - pivot over H*W*(C/G)   (fp32 atomics)
 //   groupnorm_apply_kernel : (x - mean) * rstd * gamma + beta, optional SiLU, bf16 NHWC
 //   softmax_rows_kernel    : in-place row softmax of the mid-block attention scores (fp32 math)
 //   gaussian_sample_scale  : z = (mean + exp(0.5 clamp(logvar)) * eps - shift) * scale -> NCHW latents
@@ -158,6 +158,15 @@ conv_in_3ch_mma_kernel(const __nv_bfloat16* __restrict__ px, const __nv_bfloat16
 
 // x: NHWC [B, HW, C]; stats: fp32 [B, G, 2] (zeroed by the caller).  grid = (chunks, B); each CTA reduces a
 // contiguous chunk of pixels for all channels; C <= 512, channels-per-group cpg = C / G in {1, 2, 4} or a multiple of 8.
+// The sums are taken around a pivot p per (image, group), the group's first channel at pixel 0: stats hold sum (x - p)
+// and sum (x - p)^2.  A single-pass E[x^2] - mean^2 loses about log2(1 + (mean / sigma)^2) bits of the variance to
+// cancellation (12 of fp32's 24 at mean / sigma = 64); around p the factor is 1 + (mean - p)^2 / sigma^2, a few units
+// for any group whose first element is a typical member.  groupnorm_apply_kernel reads the same pivot to form the mean.
+__device__ __forceinline__ void groupnorm_pivots(const __nv_bfloat16* __restrict__ xb, int v, int cpg, float (&pv)[8]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) pv[j] = __bfloat162float(xb[((v * 8 + j) / cpg) * cpg]);
+}
+
 __global__ void __launch_bounds__(256)
 groupnorm_stats_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ stats, int HW, int C, int G,
                        int pix_per_cta) {
@@ -175,13 +184,19 @@ groupnorm_stats_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
   const int r0 = threadIdx.x / vec_per_pix;
   if (r0 < rows_par) {
     const int v = threadIdx.x % vec_per_pix;
-    float f[8], a[8], q[8];
+    float f[8], a[8], q[8], pv[8];
+    groupnorm_pivots(xb, v, cpg, pv);
 #pragma unroll
     for (int j = 0; j < 8; ++j) a[j] = 0.f, q[j] = 0.f;
+    // unrolled so that several independent 16-byte loads are in flight; each lane still adds its pixels in order
+#pragma unroll 4
     for (long long pix = p0 + r0; pix < p1; pix += rows_par) {
       unpack8(*reinterpret_cast<const uint4*>(xb + pix * C + v * 8), f);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) a[j] += f[j], q[j] += f[j] * f[j];
+      for (int j = 0; j < 8; ++j) {
+        const float t = f[j] - pv[j];
+        a[j] += t, q[j] += t * t;
+      }
     }
     if (cpg >= 8) {  // the whole 8-vector belongs to one group
       float sa = 0.f, sq = 0.f;
@@ -205,8 +220,8 @@ groupnorm_stats_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ 
 }
 
 // grid = (chunks, B): like the stats kernel, a thread owns one fixed 8-channel vector column, so the per-channel
-// affine (a = rstd * gamma, b = beta - mean * a) is computed once per thread and the streaming loop is two loads-free
-// FMAs + SiLU per element — no integer division or rsqrt in the inner loop (the first version spent 4x the HBM time there).
+// affine (a = rstd * gamma, b = beta - mean * a, mean = p + (mean - p)) is computed once per thread and the streaming loop
+// is one FMA + SiLU per element — no integer division or rsqrt in the inner loop (the first version spent 4x the HBM time there).
 __global__ void __launch_bounds__(256)
 groupnorm_apply_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ stats,
                        const __nv_bfloat16* __restrict__ gamma, const __nv_bfloat16* __restrict__ beta,
@@ -220,7 +235,8 @@ groupnorm_apply_kernel(const __nv_bfloat16* __restrict__ x, const float* __restr
   if (r0 >= rows_par) return;
   const int v = threadIdx.x - r0 * vec_per_pix;
   const float inv_n = 1.f / (float(HW) * float(cpg));
-  float sc[8], sh[8], gm[8], bt[8];
+  float sc[8], sh[8], gm[8], bt[8], pv[8];   // pv: the stats kernel's pivots
+  groupnorm_pivots(x + (long long)b * HW * C, v, cpg, pv);
   unpack8(__ldg(reinterpret_cast<const uint4*>(gamma + v * 8)), gm);
   unpack8(__ldg(reinterpret_cast<const uint4*>(beta + v * 8)), bt);
 #pragma unroll
@@ -228,11 +244,11 @@ groupnorm_apply_kernel(const __nv_bfloat16* __restrict__ x, const float* __restr
     const int g = (v * 8 + j) / cpg;
     const float s1 = stats[((long long)b * G + g) * 2 + 0];
     const float q1 = stats[((long long)b * G + g) * 2 + 1];
-    const float mean = s1 * inv_n;
-    const float var = fmaxf(q1 * inv_n - mean * mean, 0.f);
+    const float dm = s1 * inv_n;                       // mean - p
+    const float var = fmaxf(q1 * inv_n - dm * dm, 0.f);
     const float rstd = rsqrtf(var + eps);
     sc[j] = rstd * gm[j];
-    sh[j] = bt[j] - mean * sc[j];
+    sh[j] = bt[j] - (pv[j] + dm) * sc[j];
   }
   const long long p0 = (long long)blockIdx.x * pix_per_cta;
   const long long p1 = min((long long)HW, p0 + pix_per_cta);

@@ -628,13 +628,18 @@ def conv_in_3ch(pixels, w, bias):
 
 
 def groupnorm_nhwc(x, gamma, beta, groups: int = 32, eps: float = 1e-6, silu: bool = True, out=None):
-    """x [B, ..., C] NHWC contiguous."""
-    _chk(x, "x")
+    """x [B, ..., C] NHWC contiguous; out, when given, contiguous with the shape of x."""
+    _chk(x, "x"); _chk(gamma, "gamma"); _chk(beta, "beta")
     assert x.is_contiguous()
     B, C = x.shape[0], x.shape[-1]
+    assert gamma.shape == (C,) and beta.shape == (C,)
     HW = x.numel() // (B * C)
     if out is None:
         out = torch.empty_like(x)
+    else:
+        _chk(out, "out")
+        if not out.is_contiguous() or out.shape != x.shape:
+            raise ValueError(f"out must be contiguous with the shape of x {tuple(x.shape)}, got {tuple(out.shape)}")
     stats = torch.empty((B * groups * 2,), device=x.device, dtype=torch.float32)
     check(_lib.lib().stb_groupnorm_nhwc(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), out.data_ptr(), stats.data_ptr(),
                                         B, HW, C, groups, eps, int(silu), _stream()))
@@ -642,7 +647,7 @@ def groupnorm_nhwc(x, gamma, beta, groups: int = 32, eps: float = 1e-6, silu: bo
 
 
 def softmax_rows_(s, scale: float):
-    """in-place softmax(scale * s) over the last dim of a contiguous [..., cols] bf16 tensor."""
+    """in-place softmax(scale * s) over the last dim of a contiguous [..., cols] bf16 tensor; scale > 0."""
     _chk(s, "s")
     assert s.is_contiguous()
     cols = s.shape[-1]
@@ -652,6 +657,7 @@ def softmax_rows_(s, scale: float):
 
 def gaussian_sample_scale(moments_nhwc, eps_nchw, shift, scale):
     """moments [B, h, w, 2L] NHWC; eps [B, L, h, w]; returns scaled latents [B, L, h, w]."""
+    _chk(moments_nhwc, "moments"); _chk(eps_nchw, "eps")
     B, h, w, L2 = moments_nhwc.shape
     L = L2 // 2
     assert moments_nhwc.is_contiguous() and eps_nchw.is_contiguous() and eps_nchw.shape == (B, L, h, w)

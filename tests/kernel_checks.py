@@ -1325,43 +1325,458 @@ def check_conv_in(B=2, H=20, W=36, C=128, exact=False):
     return _combine(name, [_bits("out", out, want)], exact_bound=exact_bound_ok([x], [w], mag))
 
 
-def check_groupnorm(B=2, H=16, W=24, C=128, G=32, silu=True, mean=0.0):
+# --------------------------------------------------------------------------------------------- VAE-encode reference model
+# GroupNorm, the mid-block row softmax and the latent sampling are compared with fp64 references on the kernels' own bf16
+# inputs, element by element, with every bound derived below.  u = 2^-24 (half an fp32 ulp, relative).
+#
+# GroupNorm (stb_groupnorm_nhwc): interval replay.  The stats kernel sums t = x - p and t^2 around a pivot p per (image,
+# group), the group's first channel at pixel 0 (gn_pivot).  Every term passes through at most L fp32 additions
+# (gn_chains: the thread's own pixels, the 8-lane vector sum when cpg >= 8, the CTA's shared atomics, the image's global
+# atomics, from the chunking of api.cu), so with d = mean - p, E2 = mean t^2 = var + d^2 and A1 = mean |t|:
+#     |d32 - d| <= e_d = (L + 1) u A1 + 2 u |d|                   (+1: t itself rounds when x and p are far apart)
+#     |var32 - var| <= e_v = (L + 7) u E2 + 2 |d| e_d + e_d^2     (t^2, / n, d d, the subtraction)
+# rstd = rsqrtf(var32 + eps) (2 ulp = 4 u, + u for the sum) lies in [rsqrt(var + eps + e_v), rsqrt(var - e_v + eps)]
+# widened by 5 u: rel_r; a = rstd gamma adds u.  mean32 = p + d32 is within e_d + u |mean|, and the output
+# y = x a + (beta - mean32 a) is one FMA after one rounding of b, so
+#     |y32 - y| <= |x - mean| |a| rel_a + (e_d + u |mean|) |a| (1 + rel_a) + u (|beta| + |mean a|) + u |y|
+# and bf16(y32) lies in [bf16(y - err), bf16(y + err)] (_bf16_range): one value almost everywhere.  The bound has no
+# (mean / sigma)^2 term: E2 holds (mean - p)^2, a few sigma^2 for a group whose first element is a typical member.
+# Without SiLU that range is the check.  With SiLU the kernel rounds y to bf16 (the GroupNorm module's output) and
+# evaluates __fdividef(v, 1 + __expf(-v)): the output must be a bf16 neighbour of fp64 silu(v) for v one of the two
+# ends of the range.  One deliberate absolute floor: once 1 + __expf(-v) passes 2^126 (v < about -87) __fdividef
+# returns 0, which is accepted only where |silu(v)| < 2^-120.  A constant group (sigma = 0) has t = 0 exactly, so
+# var = 0 and rstd = 1 / sqrt(eps); its output is beta up to the u |mean a| of the FMA form.  tol_use: the worst |got - y| / (err + half a bf16 ulp of y).
+#
+# Row softmax (stb_softmax_rows): out_i = __expf((s_i - m) scale) / sum.  z = (s - m) scale rounds twice (2 u |z|
+# absolute in the exponent), and __expf is within 2 + floor(1.173 |z|) fp32 ulps (CUDA programming guide), so every term
+# is within delta_i = 2^-23 (2 + 2.173 |z_i|) relative; the sum adds L u (8 terms per 2048-column sweep, 5 shuffle levels,
+# 7 adds over the warps) plus the terms' own errors, weighted; 1 / sum and the product add 2 u.  The output must lie in
+# the bf16 range of p_i (1 +- rel_i).  ex2.approx.ftz flushes terms below 2^-126, so where p_i < 2^-126 any output in
+# [0, 2^-126] is accepted.  A uniform row must give bf16(fp32(1 / cols)) bit for bit.
+#
+# Latent sampling (stb_gaussian_sample_scale): std = bf16(__expf(0.5 clamp(logvar, -30, 20))) lies in the bf16 range of
+# exp(x) (1 +- (2 + floor(1.173 |x|)) 2^-23): one value almost everywhere, two near a rounding midpoint.  The eager
+# bf16 chain of diffusers' DiagonalGaussianDistribution.sample and the latent scaling, bf16(mean + bf16(std eps)) then
+# bf16(bf16(z - shift) scale) (no shift: bf16(z scale)), is replayed on each candidate; the output must equal one.
+U24 = 2.0 ** -24
+
+
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count if DEV == "cuda" else 132
+
+
+def gn_chains(B, HW, C, G, sms=132):
+    """Longest chain of fp32 additions a term of one group's sums passes through in stb_groupnorm_nhwc's stats kernel,
+    from the chunking of api.cu: the thread's pixels, the 8-lane vector sum (cpg >= 8), the CTA's shared-memory atomics
+    into the group and the global atomics of the image's CTAs."""
+    chunks = max(1, min((HW + 255) // 256, (sms * 4 + B - 1) // B))
+    ppc = -(-HW // chunks)
+    ctas = -(-HW // ppc)
+    rows_par = 256 // (C // 8)
+    cpg = C // G
+    shared = rows_par * (cpg if cpg < 8 else cpg // 8)
+    return -(-ppc // rows_par) + (7 if cpg >= 8 else 0) + shared + ctas
+
+
+def gn_pivot(x, G):
+    """The kernel's pivot per (image, group) of x [B, HW, C]: the group's first channel at pixel 0; [B, G] fp64."""
+    return x[:, 0, ::x.shape[-1] // G].double()
+
+
+def gn_reference(x, gamma, beta, G, eps, L=None, pivot=None):
+    """(y, err) [B, HW, C] fp64: the GroupNorm value and the bound on the kernel's fp32 error (see above) for x
+    [B, HW, C] bf16.  L: the addition chain length (gn_chains); pivot: [B, G] (gn_pivot)."""
+    B, HW, C = x.shape
+    cpg = C // G
+    u = U24
+    if L is None:
+        L = gn_chains(B, HW, C, G, _sms())
+    x64 = x.double().view(B, HW, G, cpg)
+    p = (gn_pivot(x, G) if pivot is None else pivot.double())[:, None, :, None]
+    t = x64 - p
+    d = t.mean((1, 3), keepdim=True)
+    E2 = t.pow(2).mean((1, 3), keepdim=True)
+    A1 = t.abs().mean((1, 3), keepdim=True)
+    xc = t - d                                            # x - mean
+    var = xc.pow(2).mean((1, 3), keepdim=True)            # two-pass
+    e_d = (L + 1) * u * A1 + 2 * u * d.abs()
+    e_v = (L + 7) * u * E2 + 2 * d.abs() * e_d + e_d * e_d
+    e32 = _f32(eps)
+    r = (var + e32).rsqrt()
+    r_lo = (var + e32 + e_v).rsqrt() * (1 - 5 * u)
+    r_hi = ((var - e_v).clamp_min(0) + e32).rsqrt() * (1 + 5 * u)
+    rel_a = torch.maximum(1 - r_lo / r, r_hi / r - 1) + u
+    a = r * gamma.double().view(1, 1, G, cpg)
+    b64 = beta.double().view(1, 1, G, cpg)
+    y = xc * a + b64
+    mean = (p + d).abs()
+    err = (xc.abs() * a.abs() * rel_a + (e_d + u * mean) * a.abs() * (1 + rel_a) + u * (b64.abs() + (mean * a).abs())
+           + u * y.abs())
+    return y.view(B, HW, C), err.view(B, HW, C)
+
+
+def _half_ulp(y):
+    """Half a bf16 ulp at |y| (fp64)."""
+    e = torch.frexp(y.abs())[1]
+    return torch.where(y == 0, torch.zeros_like(y), torch.ldexp(torch.ones_like(y), e - 9))
+
+
+def _range_use(got, y, err, where=None):
+    """The largest share of the fp32 error bound err an element needs: (|got - y| - half a bf16 ulp of y)+ / err; above
+    1 the element lies outside its range (up to the ulp at a power of two)."""
+    use = ((got.double() - y).abs() - _half_ulp(y)).clamp_min(0) / (err + 1e-300)
+    if where is not None:
+        use = use[where]
+    return round(float(use.max().item()), 4) if use.numel() else 0.0
+
+
+def silu64(v):
+    return v * torch.sigmoid(v)
+
+
+SILU_ARGMIN = -1.2784645427610738      # silu is decreasing below, increasing above
+
+
+def silu_check(name, got, lo, hi):
+    """got (bf16) is a bf16 neighbour of fp64 silu(v) for some v in [lo, hi] (the GroupNorm output's range; near 0 it
+    holds several bf16 values): its two neighbours bracket a point of silu([lo, hi]).  Or 0 where |silu(v)| < 2^-120
+    (the __fdividef floor)."""
+    dn, up = _bf16_steps(got)
+    sl, sh = silu64(lo.double()), silu64(hi.double())
+    smin = torch.where((lo.double() <= SILU_ARGMIN) & (SILU_ARGMIN <= hi.double()),
+                       torch.full_like(sl, silu64(torch.tensor(SILU_ARGMIN, dtype=torch.float64)).item()), torch.minimum(sl, sh))
+    smax = torch.maximum(sl, sh)
+    ok = (dn <= smax) & (up >= smin)
+    ok |= (got == 0) & (torch.minimum(sl.abs(), sh.abs()) < 2.0 ** -120)
+    bad = ~(ok & torch.isfinite(got))
+    n = int(bad.sum().item())
+    out = {"name": name, "ok": n == 0, "n_bad": n, "numel": got.numel()}
+    if n:
+        _first(bad, got.float(), silu64(lo.double()), out)
+    return out
+
+
+def _gn_input(B, HW, C, G, ratio, const=False, seed=1):
+    """x [B, HW, C] bf16.  Group (b, g), k = b G + g, is N(mu, s^2) with its own s = 2^(k % 5 - 2) and
+    mu = (-1)^k ratio s (1 + (7 k % 16) / 64): mean / sigma between ratio and 1.23 ratio, different for every group
+    and image, so a wrong group index or image offset moves the statistics.  const: every third group is the constant
+    0.3 (1 + k / 8), sigma = 0."""
+    cpg = C // G
+    gen = torch.Generator().manual_seed(seed)
+    k = torch.arange(B * G, dtype=torch.float64).view(B, G)
+    s = torch.pow(2.0, (k % 5) - 2)
+    mu = torch.where(k % 2 == 0, 1.0, -1.0) * ratio * s * (1 + ((7 * k) % 16) / 64)
+    x = torch.randn(B, HW, G, cpg, generator=gen, dtype=torch.float32) * s[:, None, :, None].float() + \
+        mu[:, None, :, None].float()
+    if const:
+        cm = (k % 3 == 0)[:, None, :, None].expand_as(x)
+        x = torch.where(cm, (0.3 * (1 + k / 8))[:, None, :, None].float().expand_as(x), x)
+    return x.reshape(B, HW, C).to(torch.bfloat16).to(DEV)
+
+
+def check_groupnorm(B=2, H=16, W=24, C=128, G=32, silu=True, ratio=0.0, const=False, beta0=False, control=False):
+    """stb_groupnorm_nhwc by interval replay (above).  ratio: mean / sigma of the groups (_gn_input); const: every
+    third group constant; beta0: beta = 0.
+    control: also run torch's F.group_norm on the same bf16 input on the device and report its tol_use under the same
+    bound (information: torch is not held to this kernel's bound)."""
     import torch.nn.functional as F
-    x = (_rand(B, H, W, C, seed=1).float() + mean).bfloat16()
+    HW = H * W
+    x = _gn_input(B, HW, C, G, ratio, const).view(B, H, W, C)
     gm = (1.0 + 0.1 * _rand(C, seed=2).float()).bfloat16()
-    bt = _rand(C, scale=0.1, seed=3)
+    bt = torch.zeros(C, dtype=torch.bfloat16, device=DEV) if beta0 else _rand(C, scale=0.1, seed=3)
     out = ops.groupnorm_nhwc(x, gm, bt, G, 1e-6, silu)
     torch.cuda.synchronize()
-    ref = F.group_norm(x.float().permute(0, 3, 1, 2), G, gm.float(), bt.float(), 1e-6)
+    x3 = x.view(B, HW, C)
+    y, err = gn_reference(x3, gm, bt, G, 1e-6)
+    lo, hi = _bf16_range(y, err)
+    got = out.view(B, HW, C)
+    extra = {"gn_frac_exact": round(float((lo == hi).double().mean().item()), 4), "chain_L": gn_chains(B, HW, C, G, _sms())}
     if silu:
-        ref = F.silu(ref)
-    return _report(f"groupnorm_C{C}_silu{int(silu)}_mean{mean}", out, ref.permute(0, 2, 3, 1), atol=2e-2, rtol=1e-2)
+        parts = [silu_check("out", got, lo, hi)]
+    else:
+        parts = [_in_range("out", got, lo, hi)]
+        parts[0]["tol_use"] = _range_use(got, y, err)
+    if control:
+        ref = F.group_norm(x.permute(0, 3, 1, 2), G, gm, bt, 1e-6).permute(0, 2, 3, 1).reshape(B, HW, C)
+        extra["torch_tol_use"] = _range_use(ref, y, err)
+        if not silu:
+            extra["kernel_tol_use"] = parts[0]["tol_use"]
+    name = f"groupnorm_B{B}_HW{HW}_C{C}_G{G}_silu{int(silu)}_r{ratio:g}" + ("_const" if const else "") + \
+        ("_beta0" if beta0 else "")
+    return _combine(name, parts, **extra)
 
 
-def check_softmax_rows(rows=300, cols=1024, scale=0.0442):
-    s = _rand(rows, cols, scale=20.0, seed=1)
-    ref = torch.softmax(s.float() * scale, dim=-1)
+def softmax_range(s, scale):
+    """(lo, hi) bf16 range of softmax(f32(scale) s) per element of s [rows, cols] (bf16) under the kernel's error bound,
+    with the flush-to-zero floor: where p < 2^-126, lo = 0 and hi >= 2^-126."""
+    rows, cols = s.shape
+    s64 = s.double()
+    z = (s64 - s64.amax(-1, keepdim=True)) * _f32(scale)
+    e = z.exp()
+    p = e / e.sum(-1, keepdim=True)
+    delta = 2.0 ** -23 * (2 + 2.173 * z.abs())
+    L = 8 * -(-cols // 2048) + 5 + 7
+    rel = delta + L * U24 + (e * delta).sum(-1, keepdim=True) / e.sum(-1, keepdim=True) + 3 * U24
+    lo, hi = _bf16_range(p, rel * p)
+    tiny = p < 2.0 ** -126
+    lo = torch.where(tiny, torch.zeros_like(lo), lo)
+    hi = torch.where(tiny, torch.maximum(hi, torch.full_like(hi, 2.0 ** -126)), hi)
+    return lo, hi, p, rel * p
+
+
+def _softmax_rows_input(rows, cols, scale, sigma, seed=1):
+    """bf16 scores [rows, cols] (unscaled).  Row 0 uniform (3.0), row 1 peaked (one logit, at column 2 cols / 3, 40
+    above N(0, 1) scaled logits), row 2 wide (N(0, 25^2) scaled logits, some flushed to zero), row 3 a ramp of scaled
+    logits from -120 up to 0 at the last column (the row max lies far from the first columns); the rest N(0, sigma^2)."""
+    gen = torch.Generator().manual_seed(seed)
+    s = torch.randn(rows, cols, generator=gen) * sigma
+    if rows >= 4:
+        s[0] = 3.0
+        s[1] = torch.randn(cols, generator=gen) / scale
+        s[1, (2 * cols) // 3] = (float(s[1].max()) * scale + 40.0) / scale
+        s[2] = torch.randn(cols, generator=gen) * 25.0 / scale
+        s[3] = torch.linspace(-120.0, 0.0, cols) / scale
+    return s.to(torch.bfloat16).to(DEV)
+
+
+def check_softmax_rows(rows=300, cols=1024, scale=0.0442, sigma=20.0):
+    """In-place row softmax against fp64 softmax(f32(scale) s) by the bound above; row 0 (uniform) bit for bit."""
+    s = _softmax_rows_input(rows, cols, scale, sigma)
+    s0 = s.clone()
     ops.softmax_rows_(s, scale)
     torch.cuda.synchronize()
-    return _report("softmax_rows", s, ref, atol=2e-3, rtol=1e-2)
+    lo, hi, p, err = softmax_range(s0, scale)
+    parts = [_in_range("out", s, lo, hi)]
+    parts[0]["tol_use"] = _range_use(s, p, err, where=p >= 2.0 ** -126)
+    if rows >= 4:
+        parts.append(_bits("uniform_row", s[0], torch.full_like(s[0], 1.0 / cols, dtype=torch.float32).bfloat16()))
+    return _combine(f"softmax_rows_{rows}x{cols}_scale{scale:g}", parts, flushed=int((p < 2.0 ** -126).sum().item()))
 
 
-def check_gaussian_sample(B=2, L=16, h=12, w=20, shift=0.1159):
-    m = _rand(B, h, w, 2 * L, seed=1)
-    eps = _rand(B, L, h, w, seed=2)
-    out = ops.gaussian_sample_scale(m, eps, shift, 0.3611)
+LOGVAR_EDGES = (-40.0, -30.0, -29.875, 19.875, 20.0, 25.0)
+
+
+def gaussian_std_range(logvar):
+    """bf16 range of the kernel's std = bf16(__expf(0.5 clamp(logvar, -30, 20))) (logvar bf16)."""
+    x = 0.5 * logvar.double().clamp(-30.0, 20.0)
+    e = x.exp()
+    return _bf16_range(e, e * 2.0 ** -23 * (2 + torch.floor(1.173 * x.abs())))
+
+
+def gaussian_replay(mean, std, eps, shift, scale):
+    """The eager bf16 chain on a bf16 std: bf16(mean + bf16(std eps)), then bf16(bf16(z - shift) scale) (no shift:
+    bf16(z scale)), fp32 arithmetic rounded after every op as torch's bf16 tensor ops do."""
+    z = (mean.float() + (std.float() * eps.float()).bfloat16().float()).bfloat16()
+    if shift is None:
+        return (z.float() * _f32(scale)).bfloat16()
+    return ((z.float() - _f32(shift)).bfloat16().float() * _f32(scale)).bfloat16()
+
+
+def _gaussian_input(B, L, h, w, seed=1):
+    """moments NHWC [B, h, w, 2L], eps NCHW [B, L, h, w]: logvar N(0, 1) with LOGVAR_EDGES at (pixel + channel) % 8 < 6,
+    so the clamp is reached from both sides and at its ends."""
+    m = _rand(B, h, w, 2 * L, seed=seed)
+    pix = torch.arange(h * w, device=DEV).view(h, w, 1)
+    sel = (pix + torch.arange(L, device=DEV).view(1, 1, L)) % 8
+    lv = m[..., L:]
+    for i, v in enumerate(LOGVAR_EDGES):
+        lv[:, sel == i] = v
+    return m, _rand(B, L, h, w, seed=seed + 1)
+
+
+def check_gaussian_sample(B=2, L=16, h=12, w=20, shift=0.1159, scale=0.3611):
+    """Interval replay of the latent sample (above); shift None: no shift (SDXL, sample())."""
+    m, eps = _gaussian_input(B, L, h, w)
+    out = ops.gaussian_sample_scale(m, eps, shift, scale)
     torch.cuda.synchronize()
     mn = m.permute(0, 3, 1, 2)
     mean, logvar = mn[:, :L], mn[:, L:]
-    z = mean + torch.exp(0.5 * torch.clamp(logvar, -30.0, 20.0)) * eps          # bf16 tensor ops, like diffusers
-    ref = (z - shift) * 0.3611 if shift is not None else z * 0.3611
-    r = _report("gaussian_sample_scale", out, ref, atol=0.0, rtol=0.0)
-    if not r["ok"]:  # exp() ulp differences may move a bf16 rounding; never more than 1 bf16 ulp
-        r2 = _report("gaussian_sample_scale", out, ref, atol=1e-3, rtol=2 ** -7)
-        r2["bit_exact"] = False
-        return r2
-    r["bit_exact"] = True
-    return r
+    s_lo, s_hi = gaussian_std_range(logvar)
+    r_lo, r_hi = gaussian_replay(mean, s_lo, eps, shift, scale), gaussian_replay(mean, s_hi, eps, shift, scale)
+    iv = torch.int16
+    hit = (out.view(iv) == r_lo.view(iv)) | (out.view(iv) == r_hi.view(iv))
+    n = int((~hit).sum().item())
+    part = {"name": "out", "ok": n == 0, "n_bad": n, "numel": out.numel()}
+    if n:
+        _first(~hit, out.float(), r_lo.float(), part)
+    return _combine(f"gaussian_sample_B{B}_L{L}_{h}x{w}_shift{shift}_scale{scale:g}", [part],
+                    n_two_std=int((s_lo != s_hi).sum().item()), n_two_out=int((r_lo != r_hi).sum().item()))
+
+
+# --------------------------------------------------------------------------------------------- LoKr and LoRA dropout reference model
+# LoKr rebuild: out = bf16(fmaf(f32(scale w1[i, k']), w2[j, l], W)).  f32(scale w1) has 24 significant bits and w2 8,
+# so the product is exact in fp64; adding the bf16 W rounds at most once in fp64, and lokr_single_rounding asserts from
+# the drawn values that the fp32 rounding of that sum is the exact sum's (the fp64 sum is exact, or it is not an fp32
+# rounding midpoint): fp64 -> fp32 -> bf16 then reproduces the kernel's single fp32 rounding and the bf16 store bit for
+# bit.  out_t must be out transposed, bit for bit.  n_vs_eager counts the elements
+# where this differs from lycoris's own fp32 chain bf16(W + kron(w1, w2) scale) (information).
+# LoKr factor gradients: d w1 = scale sum_{j,l} dW w2 (K = b d terms) and d w2 = scale sum_{i,k'} dW w1 (K = a c terms)
+# against fp64 with tol = 2^-23 |ref| + LOKR_C 2^-24 sqrt(K) M_ij, M the magnitude sum.  d w2 is one sequential fp32
+# FMA chain per element, whose error is typically about 0.5 u M; d w1 a tree of 8-term FMA chains, shuffles and atomics.
+# LOKR_C = 1: on an H100 80GB HBM3 (700 W limit) the largest c_half was 0.91 (d w1 at the Flux ff shape, K = 2.4M) and
+# the largest tol_use 0.47.  Exact inputs (dW integers in [-2, 2], w1 / w2 integers in [-6, 6] x 2^-4, a power-of-two scale): every
+# partial sum is a multiple of 2^-8 below 2^19, so both outputs match fp64 bit for bit in any atomic order.
+# LoRA dropout: the mask is replayed in numpy uint32 (dropout_keep_np: mix32 / dropout_keep of elementwise.cuh and the
+# llround(p 2^24) threshold of api.cu); expand must be bf16(x f32(1 / (1 - p))) where kept, 0 elsewhere, bit for bit;
+# accum is replayed in member order in fp32, each kept term added with an FMA or rounded twice: either is accepted per
+# element and counted.
+LOKR_C = 1.0
+
+
+def lokr_single_rounding(prod, W):
+    """fp64 prod + W, rounded to fp32, is the exact sum rounded once: the fp64 sum is exact (its TwoSum error is 0) or
+    it is not an fp32 rounding midpoint (only there could rounding twice differ)."""
+    s = prod + W
+    bb = s - prod
+    err = (prod - (s - bb)) + (W - bb)
+    f = s.float()
+    g = torch.nextafter(f, torch.where(s > f.double(), torch.full_like(f, math.inf), torch.full_like(f, -math.inf)))
+    mid = (f.double() + g.double()) * 0.5 == s
+    return bool(((err == 0) | ~mid).all().item())
+
+
+def lokr_rebuild_replay(W, w1, w2, scale):
+    """(bf16 out, single): the kernel's fmaf(f32(scale w1), w2, W) rounded to fp32 then bf16, from the fp64 sum."""
+    s1 = (w1.float() * _f32(scale)).double()
+    prod = torch.kron(s1, w2.double())
+    return (prod + W.double()).float().bfloat16(), lokr_single_rounding(prod, W.double())
+
+
+def lokr_eager(W, w1, w2, scale):
+    """lycoris.py's host chain: bf16(W + kron(w1, w2) scale) in fp32."""
+    return (W.float() + torch.kron(w1.float(), w2.float()) * scale).bfloat16()
+
+
+def check_lokr_rebuild(a=8, b=48, c=4, d=40, scale=0.5, fused=True, pad=0):
+    """stb_lokr_rebuild bit for bit (above).  fused: out / out_t are the middle slices of [3 N, K] / [K, 3 N] buffers
+    whose other slices must stay zero.  pad: W, out and out_t rows are padded by `pad` elements (row strides that are
+    not multiples of 8 take the scalar paths); the padding must stay zero."""
+    N, K = a * b, c * d
+    W = (_rand(N, K + pad, seed=61) * 0.05)[:, :K]
+    w1, w2 = _rand(a, c, seed=62), _rand(b, d, seed=63) * 0.05
+    big = torch.zeros(3 * N if fused else N, K + pad, device=DEV, dtype=torch.bfloat16)
+    big_t = torch.zeros(K, 3 * N + pad if fused else N + pad, device=DEV, dtype=torch.bfloat16)
+    n0 = N if fused else 0
+    out, out_t = big[n0:n0 + N, :K], big_t[:, n0:n0 + N]
+    ops.lokr_rebuild(W, w1, w2, scale, out, out_t)
+    torch.cuda.synchronize()
+    want, fits = lokr_rebuild_replay(W, w1, w2, scale)
+    parts = [_bits("out", out, want), _bits("out_t", out_t, want.t())]
+    mask, mask_t = torch.ones_like(big, dtype=torch.bool), torch.ones_like(big_t, dtype=torch.bool)
+    mask[n0:n0 + N, :K] = False
+    mask_t[:, n0:n0 + N] = False
+    clean = bool((big[mask] == 0).all().item()) and bool((big_t[mask_t] == 0).all().item())
+    n_eager = int((want.view(torch.int16) != lokr_eager(W, w1, w2, scale).view(torch.int16)).sum().item())
+    return _combine(f"lokr_rebuild_{a}x{b}_{c}x{d}_s{scale:.4g}" + (f"_pad{pad}" if pad else ""), parts, single_rounding=fits,
+                    halo_clean=clean, n_vs_eager=n_eager)
+
+
+def check_lokr_factor_grads(a=8, b=48, c=4, d=40, scale=0.5, strided=True, exact=False):
+    """stb_lokr_factor_grads against fp64 (tolerance above) or, exact, bit for bit; d w2 (no atomics) must be
+    bit-identical on a second run.  strided: dW is a window of a wider buffer."""
+    N, K = a * b, c * d
+    ea, ew = ("int", "frac") if exact else (None, None)
+    w1, w2 = _gen(a, c, seed=64, exact=ew), _gen(b, d, seed=65, exact=ew)
+    g_full = _gen(N + 8, K + 16, seed=66, exact=ea)
+    dW = g_full[4:4 + N, 8:8 + K] if strided else g_full[:N, :K].contiguous()
+    g4 = dW.double().reshape(a, b, c, d)
+    r1, m1 = torch.einsum("ajcl,jl->ac", g4, w2.double()), torch.einsum("ajcl,jl->ac", g4.abs(), w2.double().abs())
+    r2, m2 = torch.einsum("ajcl,ac->jl", g4, w1.double()), torch.einsum("ajcl,ac->jl", g4.abs(), w1.double().abs())
+    d1, d2 = ops.lokr_factor_grads(dW, w1, w2, scale)
+    d2_again = ops.lokr_factor_grads(dW, w1, w2, scale)[1]
+    torch.cuda.synchronize()
+    s = _f32(scale)
+    extra = {"dw2_repeatable": bool(torch.equal(d2, d2_again))}
+    if exact:
+        assert _is_pow2(s)
+        extra["exact_bound"] = exact_bound_ok([dW], [w1, w2], torch.cat([m1.flatten(), m2.flatten()]))
+        parts = [_bits("dw1", d1, (s * r1).float()), _bits("dw2", d2, (s * r2).float())]
+    else:
+        parts = [_report_acc("dw1", d1, s * r1, abs(s) * m1, b * d, GEMM_RTOL_F32, c=LOKR_C),
+                 _report_acc("dw2", d2, s * r2, abs(s) * m2, a * c, GEMM_RTOL_F32, c=LOKR_C)]
+    return _combine(f"lokr_factor_grads_{a}x{b}_{c}x{d}_s{scale:g}" + ("_strided" if strided else "") +
+                    ("_exact" if exact else ""), parts, **extra)
+
+
+def mix32_np(h):
+    """elementwise.cuh mix32 (murmur3 finaliser) on a numpy uint32 array."""
+    import numpy as np
+    h = h ^ (h >> np.uint32(16))
+    h = h * np.uint32(0x85EBCA6B)
+    h = h ^ (h >> np.uint32(13))
+    h = h * np.uint32(0xC2B2AE35)
+    return h ^ (h >> np.uint32(16))
+
+
+def dropout_thresh(p):
+    """api.cu's llround(double(float(p)) * 2^24)."""
+    return int(math.floor(_f32(p) * 16777216.0 + 0.5))
+
+
+def dropout_keep_np(seed, stream, idx, p):
+    """dropout_keep(seed, stream, idx, thresh) for a numpy uint64 array of logical element indices."""
+    import numpy as np
+    lo, hi = (idx & np.uint64(0xFFFFFFFF)).astype(np.uint32), (idx >> np.uint64(32)).astype(np.uint32)
+    inner = mix32_np(hi + np.uint32((stream * 0x85EBCA77 + seed) & 0xFFFFFFFF))
+    h = mix32_np(lo * np.uint32(0x9E3779B1) + inner)
+    return (h >> np.uint32(8)) >= np.uint32(dropout_thresh(p))
+
+
+def dropout_masks(members, B, S, K, p, seed, stream0):
+    """Bool [members, B, S, K] on DEV: the keep mask of member m is stream stream0 + m over the logical [B, S, K] index."""
+    import numpy as np
+    idx = np.arange(B * S * K, dtype=np.uint64)
+    return torch.from_numpy(np.stack([dropout_keep_np(seed, (stream0 + m) & 0xFFFFFFFF, idx, p)
+                                      for m in range(members)])).view(members, B, S, K).to(DEV)
+
+
+def dropout_inv_keep(p):
+    """api.cu's 1.f / (1.f - p) in fp32."""
+    one = torch.tensor(1.0, dtype=torch.float32)
+    return one / (one - torch.tensor(p, dtype=torch.float32))
+
+
+def dropout_accum_replay(dx0, d, keep, inv):
+    """(fma, twice): dx0 + sum_m keep_m d_m inv in member order in fp32, each kept term added by one FMA (the bf16 x fp32
+    product is exact in fp64) or rounded twice; bf16."""
+    fma, twice = dx0.float(), dx0.float()
+    inv64 = inv.double().to(d.device)
+    for m in range(d.shape[0]):
+        fma = torch.where(keep[m], (d[m].double() * inv64 + fma.double()).float(), fma)
+        twice = torch.where(keep[m], twice + d[m].float() * inv.to(d.device), twice)
+    return fma.bfloat16(), twice.bfloat16()
+
+
+def check_dropout(members=3, B=2, S=77, K=200, p=0.1, window=False, seed=1234, stream0=7):
+    """dropout_expand and dropout_accum_ bit for bit against the numpy mask (above).  window: x and dx are row / column
+    windows of wider buffers whose halo must stay unchanged."""
+    if window:
+        xfull = _rand(B, S + 3, K + 16, seed=81)
+        x = xfull[:, 1:S + 1, 8:8 + K]
+        dxfull = _rand(B, S + 3, K + 16, seed=82)
+        dx = dxfull[:, 2:S + 2, 8:8 + K]
+        halo0 = dxfull.clone()
+    else:
+        x, dx = _rand(B, S, K, seed=81), _rand(B, S, K, seed=82)
+    dx0 = dx.clone()
+    d = _rand(members, B, S, K, seed=83)
+    xm = ops.dropout_expand(x, members, p, seed, stream0)
+    ops.dropout_accum_(dx, d, p, seed, stream0)
+    torch.cuda.synchronize()
+    keep = dropout_masks(members, B, S, K, p, seed, stream0)
+    inv = dropout_inv_keep(p)
+    want = torch.where(keep, (x.float() * inv.to(DEV)).bfloat16(), torch.zeros_like(x))
+    parts = [_bits("expand", xm, want)]
+    fma, twice = dropout_accum_replay(dx0, d, keep, inv)
+    iv = torch.int16
+    hit_f, hit_t = dx.view(iv) == fma.view(iv), dx.view(iv) == twice.view(iv)
+    extra = {"accum_fma_or_two_roundings": bool((hit_f | hit_t).all().item()), "n_fma": int((hit_f & ~hit_t).sum().item()),
+             "n_twice": int((hit_t & ~hit_f).sum().item()), "keep_rate": round(float(keep.float().mean().item()), 4)}
+    if window:
+        m = torch.ones_like(dxfull, dtype=torch.bool)
+        m[:, 2:S + 2, 8:8 + K] = False
+        extra["halo_clean"] = bool(torch.equal(dxfull[m], halo0[m]))
+    return _combine(f"dropout_m{members}_B{B}_S{S}_K{K}_p{p:g}" + ("_window" if window else ""), parts, **extra)
 
 
 CHECKS.update({
@@ -1375,7 +1790,7 @@ CHECKS.update({
     "conv_in_3ch": lambda: check_conv_in(),
     "groupnorm_silu": lambda: check_groupnorm(),
     "groupnorm_plain_512": lambda: check_groupnorm(C=512, silu=False),
-    "groupnorm_256_offset": lambda: check_groupnorm(C=256, mean=3.0),
+    "groupnorm_256_offset": lambda: check_groupnorm(C=256, ratio=4.0),
     "groupnorm_c64": lambda: check_groupnorm(C=64),
     "softmax_rows": lambda: check_softmax_rows(),
     "gaussian_sample": lambda: check_gaussian_sample(),
@@ -1598,41 +2013,6 @@ CHECKS.update({
 
 
 # --------------------------------------------------------------------------------------------- LyCORIS LoKr + stand-alone GELU
-def check_lokr_rebuild(a=8, b=48, c=4, d=40, scale=0.5, fused=True):
-    """out = bf16(W + kron(w1, w2) * scale) and its transpose, written into slices of larger (fused q|k|v style) buffers."""
-    N, K = a * b, c * d
-    W, w1, w2 = _rand(N, K, seed=61) * 0.05, _rand(a, c, seed=62), _rand(b, d, seed=63) * 0.05
-    ref = (W.float() + torch.kron(w1.float(), w2.float()) * scale).bfloat16()
-    if fused:
-        big, big_t = torch.zeros(3 * N, K, device="cuda", dtype=torch.bfloat16), torch.zeros(K, 3 * N, device="cuda", dtype=torch.bfloat16)
-        out, out_t = big[N:2 * N], big_t[:, N:2 * N]
-    else:
-        out, out_t = torch.empty(N, K, device="cuda", dtype=torch.bfloat16), None
-    ops.lokr_rebuild(W, w1, w2, scale, out, out_t)
-    torch.cuda.synchronize()
-    # fp32 association differs (scale * w1 first), so a rare bf16 rounding tie may land on the neighbouring value
-    close = lambda x, y: float((x != y).float().mean()) < 2e-3 and bool(torch.allclose(x.float(), y.float(), rtol=2 ** -7, atol=1e-6))
-    ok = close(out, ref)
-    if fused:
-        ok = ok and bool(torch.equal(out_t, out.t())) and float(big[:N].abs().sum() + big[2 * N:].abs().sum() + big_t[:, :N].abs().sum()) == 0.0
-    return {"name": f"lokr_rebuild_{a}x{b}_{c}x{d}", "ok": ok, "max_err": float((out.float() - ref.float()).abs().max())}
-
-
-def check_lokr_factor_grads(a=8, b=48, c=4, d=40, scale=0.5, strided=True):
-    N, K = a * b, c * d
-    w1, w2 = _rand(a, c, seed=64), _rand(b, d, seed=65)
-    g_full = _rand(N + 8, K + 16, seed=66)
-    dW = g_full[4:4 + N, 8:8 + K] if strided else g_full[:N, :K].contiguous()
-    g4 = dW.float().view(a, b, c, d) if not strided else dW.float().reshape(a, b, c, d)
-    r1 = torch.einsum("ajcl,jl->ac", g4, w2.float()) * scale
-    r2 = torch.einsum("ajcl,ac->jl", g4, w1.float()) * scale
-    d1, d2 = ops.lokr_factor_grads(dW, w1, w2, scale)
-    torch.cuda.synchronize()
-    x1 = _report("lokr_dw1", d1, r1, atol=float(r1.abs().max()) * 1e-4, rtol=1e-4)
-    x2 = _report("lokr_dw2", d2, r2, atol=float(r2.abs().max()) * 1e-4, rtol=1e-4)
-    return {"name": f"lokr_factor_grads_{a}x{b}_{c}x{d}", "ok": x1["ok"] and x2["ok"], "max_err": max(x1["max_err"], x2["max_err"])}
-
-
 def check_gelu_tanh(B=2, S=77, D=640, scale=1.0):
     """gelu_tanh(pre) is a bf16 neighbour of fp64 gelu_tanh(pre), and mul_dgelu_tanh(g, pre) one of g gelu'(pre) with the
     fp32 formulas' cancellation allowance (_gelu_atol), as the GEMM's exact-mode EPI_GELU / EPI_MUL_DGELU; in place equals
@@ -1973,3 +2353,71 @@ for _lt in ("l2", "huber", "smooth_l1"):
 for _lt in ("huber", "smooth_l1"):
     CHECKS[f"flow_loss_full_size_{_lt}"] = _case(check_loss_full_size, "flow", loss_type=_lt)
     CHECKS[f"target_loss_full_size_{_lt}"] = _case(check_loss_full_size, "target", loss_type=_lt)
+
+
+# --------------------------------------------------------------------------------------------- VAE encode, LoKr, LoRA dropout
+# GroupNorm: cpg 4 / 8 / 16 at G = 32, cpg 1 / 2 at G = 64, C = 384 at G = 48 (16 idle threads per CTA), C = 8; HW 1,
+# 7, 1000;
+# B = 3; the Flux VAE stage sizes; offset groups at mean / sigma 0, 4, 16, 64 and 256 with torch's GroupNorm as a control;
+# constant groups with beta = 0 and beta != 0 at a pixel count that is not a power of two.
+for _c, _g in ((128, 32), (256, 32), (512, 32), (64, 64), (128, 64), (384, 48), (8, 8), (8, 4)):
+    for _silu in (True, False):
+        CHECKS[f"groupnorm_c{_c}_g{_g}_silu{int(_silu)}"] = _case(check_groupnorm, B=2, H=20, W=36, C=_c, G=_g, silu=_silu)
+for _h, _w in ((1, 1), (1, 7), (25, 40)):
+    for _c, _g in ((128, 32), (64, 64), (512, 32)):
+        CHECKS[f"groupnorm_hw{_h * _w}_c{_c}_g{_g}"] = _case(check_groupnorm, B=2, H=_h, W=_w, C=_c, G=_g, silu=_h == 1)
+CHECKS["groupnorm_b3"] = _case(check_groupnorm, B=3, H=33, W=17, C=256, G=32, ratio=4.0)
+CHECKS["groupnorm_flux_512px_c128"] = _case(check_groupnorm, B=1, H=512, W=512, C=128, G=32)
+CHECKS["groupnorm_flux_128px_c512"] = _case(check_groupnorm, B=1, H=128, W=128, C=512, G=32)
+CHECKS["groupnorm_flux_1024px_c128"] = _case(check_groupnorm, B=1, H=1024, W=1024, C=128, G=32)
+for _r in (0, 4, 16, 64, 256):
+    for _c, _g in ((128, 32), (512, 32), (128, 64)):
+        CHECKS[f"groupnorm_offset_r{_r}_c{_c}_g{_g}"] = _case(check_groupnorm, B=2, H=32, W=48, C=_c, G=_g, silu=False,
+                                                             ratio=float(_r), control=True)
+    CHECKS[f"groupnorm_offset_r{_r}_silu"] = _case(check_groupnorm, B=2, H=32, W=48, C=256, G=32, ratio=float(_r))
+for _silu in (True, False):
+    for _b0 in (True, False):
+        CHECKS[f"groupnorm_const_silu{int(_silu)}_beta{'0' if _b0 else 'x'}"] = _case(
+            check_groupnorm, B=2, H=7, W=11, C=128, G=32, silu=_silu, const=True, beta0=_b0)
+
+# row softmax: short rows, a partial second 2048-column sweep, the mid-block S at 512 px and 1024 px, scale 512^-0.5
+for _cols in (8, 24, 1024, 2056, 4096, 16384):
+    CHECKS[f"softmax_rows_c{_cols}"] = _case(check_softmax_rows, rows=64 if _cols >= 4096 else 300, cols=_cols)
+CHECKS["softmax_rows_c4096_midblock_scale"] = _case(check_softmax_rows, rows=128, cols=4096, scale=512 ** -0.5, sigma=30.0)
+
+# latent sampling: the Flux, SD3, SDXL and sample() scalings, L = 4 / 16, odd h x w, B = 3
+for _nm, _sh, _sc in (("flux", 0.1159, 0.3611), ("sd3", 0.0609, 1.5305), ("sdxl", None, 0.13025), ("sample", None, 1.0)):
+    for _l in (4, 16):
+        CHECKS[f"gaussian_sample_{_nm}_l{_l}"] = _case(check_gaussian_sample, B=2, L=_l, h=13, w=21, shift=_sh, scale=_sc)
+CHECKS["gaussian_sample_b3_flux_64px"] = _case(check_gaussian_sample, B=3, L=16, h=64, w=64, shift=0.1159, scale=0.3611)
+
+# LoKr rebuild: N and K not multiples of 8 (both scalar paths and the scalar transpose), row strides that are not
+# multiples of 8, scale 0.75 and 1/3, and lycoris.factorization of Flux's 3072 / 12288 widths at factor -1 and 16
+CHECKS["lokr_rebuild_ragged_transposed"] = _case(check_lokr_rebuild, a=3, b=37, c=5, d=13, scale=0.75, fused=False)
+CHECKS["lokr_rebuild_odd_strides"] = _case(check_lokr_rebuild, a=4, b=40, c=6, d=32, scale=1 / 3, pad=3)
+CHECKS["lokr_rebuild_ragged_odd_strides"] = _case(check_lokr_rebuild, a=3, b=37, c=5, d=13, scale=1 / 3, fused=False, pad=5)
+_FLUX_LOKR = {(3072, -1): (48, 64), (3072, 16): (16, 192), (12288, -1): (96, 128), (12288, 16): (16, 768)}
+for _n, _k in ((3072, 3072), (12288, 3072), (3072, 12288)):
+    for _f in (-1, 16):
+        (_a, _b), (_cc, _d) = _FLUX_LOKR[(_n, _f)], _FLUX_LOKR[(_k, _f)]
+        CHECKS[f"lokr_rebuild_flux_{_n}x{_k}_f{_f}"] = _case(check_lokr_rebuild, a=_a, b=_b, c=_cc, d=_d, scale=0.75,
+                                                             fused=_n == _k)
+        CHECKS[f"lokr_factor_grads_flux_{_n}x{_k}_f{_f}"] = _case(check_lokr_factor_grads, a=_a, b=_b, c=_cc, d=_d,
+                                                                  scale=0.75, strided=False)
+# factor gradients: b d not a multiple of 2048 (dead threads in the last CTA), b d < 2048, a c near the 12288 limit of
+# the partial-sum buffer, a strided dW; each also with exact inputs (bit for bit)
+for _nm, _kw in (("bd4800", dict(a=6, b=300, c=3, d=16)), ("bd1920", dict(a=8, b=48, c=4, d=40)),
+                 ("ac12192", dict(a=96, b=16, c=127, d=8)), ("tiny", dict(a=2, b=3, c=2, d=8))):
+    for _x in (False, True):
+        CHECKS[f"lokr_factor_grads_{_nm}_strided" + ("_exact" if _x else "")] = _case(
+            check_lokr_factor_grads, **_kw, scale=0.5, strided=True, exact=_x)
+CHECKS["lokr_factor_grads_flux_3072x3072_f-1_exact"] = _case(check_lokr_factor_grads, a=48, b=64, c=48, d=64, scale=0.25,
+                                                             strided=False, exact=True)
+
+# LoRA dropout: 1 / 3 / 8 members, p 0 / 0.1 / 0.5, K 8 / 200, row and column windows of x and dx
+for _m in (1, 3, 8):
+    for _p in (0.0, 0.1, 0.5):
+        CHECKS[f"dropout_m{_m}_p{_p:g}"] = _case(check_dropout, members=_m, B=2, S=77, K=200 if _m != 8 else 8, p=_p,
+                                                 window=_p == 0.1)
+CHECKS["dropout_m3_k8_window"] = _case(check_dropout, members=3, B=3, S=33, K=8, p=0.5, window=True, seed=99, stream0=0xFFFFFFFE)
+CHECKS["dropout_m3_flux_3072"] = _case(check_dropout, members=3, B=1, S=4608, K=3072, p=0.1, seed=5, stream0=3)
