@@ -119,21 +119,6 @@ typedef struct {
 } stb_attn_fwd_args;
 int stb_attn_fwd(const stb_attn_fwd_args* args, void* stream);
 
-/* Optional: fuse the backward of the q / k pre-processing (per-head RMSNorm -> RoPE, stb_qk_rmsnorm_rope_fwd; reference
- * attn.norm_q/k + _apply_rotary_emb_anyshape, flux/transformer.py:73-98,138-141,189-190) into the attention backward
- * epilogues.  dq / dk then receive the gradient w.r.t. the PROJECTION outputs (pre-norm), i.e. what
- * stb_qk_rmsnorm_rope_bwd would have produced from the post-RoPE dq / dk.  Self-attention only (Sq == Sk; the token
- * index is the row index).  src: pre-norm projection output [B, S, C] with q at column 0 and k at column k_off. */
-typedef struct {
-  const void* src;
-  long long src_b, src_s;
-  int k_off;
-  const void *wq, *wk, *wq_added, *wk_added;   /* RMSNorm weights [HD] (image stream | tokens s < s_split); NULL = none */
-  int s_split;
-  const float *cos_t, *sin_t;                  /* [S, HD] fp32 or NULL */
-  float eps;
-} stb_qk_prep;
-
 typedef struct {
   int B, H, Sq, Sk, HD;
   float scale;
@@ -141,10 +126,8 @@ typedef struct {
   long long q_b, q_s, q_h, k_b, k_s, k_h, v_b, v_s, v_h, o_b, o_s, o_h, do_b, do_s, do_h;
   const float* lse;  /* [B, H, Sq] from the forward */
   float* delta;      /* [B, H, Sq] fp32 scratch: rowsum(dO * O) */
-  float* dq_accum;   /* unused: neither read nor written (kept for ABI compatibility) */
   void *dq, *dk, *dv;
   long long dq_b, dq_s, dq_h, dk_b, dk_s, dk_h, dv_b, dv_s, dv_h;
-  const stb_qk_prep* qk_prep; /* NULL: dq / dk are the gradients of the q / k inputs */
   /* the forward's per-key bias (bias_q = bias_h = 0 form of stb_attn_fwd_args; reference flux/transformer.py:170-173,
    * 200-207): bf16 bias[b * bias_b + sk], bias_b = 0 shares one row across the batch; NULL = none.  Any other form
    * returns STB_ERR_UNSUPPORTED.  Keys whose bias is -inf get dk = dv = 0. */

@@ -91,14 +91,6 @@ class AttnFwdArgs(C.Structure):
     ]
 
 
-class QkPrep(C.Structure):
-    _fields_ = [
-        ("src", C.c_void_p), ("src_b", C.c_longlong), ("src_s", C.c_longlong), ("k_off", C.c_int),
-        ("wq", C.c_void_p), ("wk", C.c_void_p), ("wq_added", C.c_void_p), ("wk_added", C.c_void_p), ("s_split", C.c_int),
-        ("cos_t", C.c_void_p), ("sin_t", C.c_void_p), ("eps", C.c_float),
-    ]
-
-
 class AttnBwdArgs(C.Structure):
     _fields_ = [
         ("B", C.c_int), ("H", C.c_int), ("Sq", C.c_int), ("Sk", C.c_int), ("HD", C.c_int),
@@ -109,12 +101,11 @@ class AttnBwdArgs(C.Structure):
         ("v_b", C.c_longlong), ("v_s", C.c_longlong), ("v_h", C.c_longlong),
         ("o_b", C.c_longlong), ("o_s", C.c_longlong), ("o_h", C.c_longlong),
         ("do_b", C.c_longlong), ("do_s", C.c_longlong), ("do_h", C.c_longlong),
-        ("lse", C.c_void_p), ("delta", C.c_void_p), ("dq_accum", C.c_void_p),
+        ("lse", C.c_void_p), ("delta", C.c_void_p),
         ("dq", C.c_void_p), ("dk", C.c_void_p), ("dv", C.c_void_p),
         ("dq_b", C.c_longlong), ("dq_s", C.c_longlong), ("dq_h", C.c_longlong),
         ("dk_b", C.c_longlong), ("dk_s", C.c_longlong), ("dk_h", C.c_longlong),
         ("dv_b", C.c_longlong), ("dv_s", C.c_longlong), ("dv_h", C.c_longlong),
-        ("qk_prep", C.POINTER(QkPrep)),
         ("bias", C.c_void_p), ("bias_b", C.c_longlong),
         ("kv_live", C.c_void_p), ("kv_live_b", C.c_longlong),
     ]

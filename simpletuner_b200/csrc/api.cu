@@ -9,7 +9,6 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <initializer_list>
 #include <mutex>
@@ -482,25 +481,6 @@ int stb_attn_bwd(const stb_attn_bwd_args* a, void* stream) {
   p.dq_b = a->dq_b; p.dq_s = a->dq_s; p.dq_h = a->dq_h;
   p.dk_b = a->dk_b; p.dk_s = a->dk_s; p.dk_h = a->dk_h;
   p.dv_b = a->dv_b; p.dv_s = a->dv_s; p.dv_h = a->dv_h;
-  p.fuse_prep = 0;
-  if (const stb_qk_prep* f = a->qk_prep) {
-    if (a->Sq != a->Sk) return fail(STB_ERR_ARG, "qk_prep fusion needs self-attention (Sq == Sk)");
-    if (!f->src || !aligned16(f->src) || (f->src_b & 7) || (f->src_s & 7) || (f->k_off & 7))
-      return fail(STB_ERR_ARG, "qk_prep.src must be 16-byte aligned with strides / k_off multiple of 8 elements");
-    if ((f->cos_t == nullptr) != (f->sin_t == nullptr)) return fail(STB_ERR_ARG, "qk_prep: give both cos_t and sin_t or neither");
-    p.fuse_prep = 1;
-    p.src = static_cast<const __nv_bfloat16*>(f->src);
-    p.src_b = f->src_b; p.src_s = f->src_s; p.k_off = f->k_off;
-    p.wq0 = static_cast<const __nv_bfloat16*>(f->wq); p.wk0 = static_cast<const __nv_bfloat16*>(f->wk);
-    p.wq1 = static_cast<const __nv_bfloat16*>(f->wq_added); p.wk1 = static_cast<const __nv_bfloat16*>(f->wk_added);
-    p.s_split = f->s_split;
-    p.cosT = f->cos_t; p.sinT = f->sin_t;
-    p.eps = f->eps;
-  }
-  p.q = static_cast<const __nv_bfloat16*>(a->q);
-  p.d_o = static_cast<const __nv_bfloat16*>(a->d_o);
-  p.q_b = a->q_b; p.q_s = a->q_s; p.q_h = a->q_h;
-  p.do_b = a->do_b; p.do_s = a->do_s; p.do_h = a->do_h;
   p.bias = static_cast<const __nv_bfloat16*>(a->bias);
   p.bias_b = a->bias_b;
   p.kv_live = a->kv_live;
@@ -629,15 +609,14 @@ int stb_qk_rmsnorm_rope_bwd(const void* dq, const void* dk, long long d_b, long 
   using HD128 = std::integral_constant<int, 128>;
   using HD64 = std::integral_constant<int, 64>;
   if (HD == 128 && !dw) {
-    static const bool loop_kernel = [] { const char* e = std::getenv("STB_ROPE_BWD_LOOP"); return e && e[0] == '1'; }();
     const bool flat_ok = aligned16(dq) && aligned16(dk) && aligned16(src) && aligned16(dsrc) && !(d_b & 7) && !(d_s & 7) && !(src_s & 7) &&
                          !(src_b & 7) && !(k_off & 7) && !(ds_s & 7) && !(ds_b & 7) && (!cos_t || (aligned16(cos_t) && aligned16(sin_t))) &&
                          (!wq || aligned16(wq)) && (!wk || aligned16(wk)) && (!wq_added || aligned16(wq_added)) && (!wk_added || aligned16(wk_added));
-    if (flat_ok && !loop_kernel) {   // one 16-byte chunk per thread: 4.0 TB/s vs 2.7 for the warp-per-token loop
+    if (flat_ok) {   // one 16-byte chunk per thread: 4.0 TB/s vs 2.7 for the warp-per-token loop
       const long long threads = (long long)B * S * 2 * H * 16;
-      stb::qk_rmsnorm_rope_flat128_kernel<true><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
+      stb::qk_rmsnorm_rope_flat128_bwd_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
           cast(dq), cast(dk), d_b, d_s, cast(src), src_b, src_s, k_off, cast(wq), cast(wk), cast(wq_added), cast(wk_added), s_split,
-          cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), nullptr, ds_b, ds_s, B, S, H, eps);
+          cos_t, sin_t, static_cast<__nv_bfloat16*>(dsrc), ds_b, ds_s, B, S, H, eps);
     } else {
       launch(HD128{}, std::false_type{});
     }

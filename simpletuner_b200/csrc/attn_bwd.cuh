@@ -12,8 +12,8 @@
 //       from the same shared-memory bytes as MN-major operands).
 //   attn_bwd_dq_kernel   : one CTA per (b, h, 128-row query tile), warpgroups 1 and 2 own 64 rows each; streams 64-key
 //       tiles: S = Q K^T, dP = dO V^T, dS in registers, dQ += dS K.
-// The accumulators are staged through shared memory (fp32) for the store, so that one thread handles contiguous
-// columns of a row — the fused q / k pre-processing backward (qk_prep) needs whole-row sums.
+// The accumulators are staged through shared memory (fp32) for the store, so that each thread pair owns one whole row
+// and writes it with 16-byte stores (in the wgmma accumulator layout a thread's columns of a row come in pairs 8 apart).
 #pragma once
 #include "../../include/stb200.h"
 #include "attn_fwd.cuh"
@@ -29,19 +29,6 @@ struct AttnBwdParams {
   const float* delta;  // [B, H, Sq]
   __nv_bfloat16 *dq, *dk, *dv;
   long long dq_b, dq_s, dq_h, dk_b, dk_s, dk_h, dv_b, dv_s, dv_h;
-  // raw views of q / dO (the operands themselves go through the TMA maps)
-  const __nv_bfloat16 *q, *d_o;
-  long long q_b, q_s, q_h, do_b, do_s, do_h;
-  // optional fused backward of the q / k pre-processing (per-head RMSNorm -> RoPE, qk_rmsnorm_rope_fwd_kernel):
-  // dq / dk then receive the gradient w.r.t. the PROJECTION outputs (self-attention only: token index == row index)
-  int fuse_prep;
-  const __nv_bfloat16* src;          // pre-norm projection output [B, S, C]: q at column 0, k at column k_off
-  long long src_b, src_s;
-  int k_off;
-  const __nv_bfloat16 *wq0, *wk0, *wq1, *wk1;   // RMSNorm weights (image stream | tokens s < s_split), may be null
-  int s_split;
-  const float *cosT, *sinT;          // [S, HD] or null
-  float eps;
   // BIAS instantiations only: the forward's per-key logit bias, bias[b * bias_b + sk] (bf16, -inf = masked key)
   const __nv_bfloat16* bias;
   long long bias_b;
@@ -110,66 +97,18 @@ __device__ __forceinline__ void stage_acc(float* rows, const float (&acc)[HD / 2
 }
 
 // One staged row (fp32, already multiplied by the softmax scale) -> bf16 global row.  Two threads per row, HD / 2
-// columns each (thread pair = lanes 2k, 2k+1).  With `prep`, the row is the gradient w.r.t. the post-RoPE q or k and
-// is taken back through RoPE and the per-head RMSNorm (same math as qk_rmsnorm_rope_bwd_kernel):
-//   dy = R^T go;  g = dy * w;  dx = rstd * (g - xhat * mean(g * xhat)),  xhat = x * rstd
+// columns each (thread pair = lanes 2k, 2k+1).
 template <int HD>
-__device__ __forceinline__ void store_row_half(const float* row, int half, __nv_bfloat16* grow, bool row_ok, bool prep,
-                                               const __nv_bfloat16* xrow, const __nv_bfloat16* w, const float* cs,
-                                               const float* sn, float eps) {
+__device__ __forceinline__ void store_row_half(const float* row, int half, __nv_bfloat16* grow, bool row_ok) {
   constexpr int NC = HD / 2;
   const int c0 = half * NC;
-  if (!prep) {
-    if (row_ok) {
-#pragma unroll
-      for (int c = 0; c < NC; c += 8) {
-        float o[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = row[c0 + c + i];
-        *reinterpret_cast<uint4*>(grow + c0 + c) = pack8(o);
-      }
-    }
-    return;
-  }
-  float ss = 0.f, sgx = 0.f;
-  float g[NC];
+  if (!row_ok) return;
 #pragma unroll
   for (int c = 0; c < NC; c += 8) {
-    float x[8], wv[8];
-    unpack8(row_ok ? __ldg(reinterpret_cast<const uint4*>(xrow + c0 + c)) : make_uint4(0u, 0u, 0u, 0u), x);
-    if (w) unpack8(__ldg(reinterpret_cast<const uint4*>(w + c0 + c)), wv);
+    float o[8];
 #pragma unroll
-    for (int i = 0; i < 8; i += 2) {
-      const int j = c0 + c + i;
-      const float go0 = row[j], go1 = row[j + 1];
-      float dy0 = go0, dy1 = go1;
-      if (cs && row_ok) {
-        const float2 c2 = __ldg(reinterpret_cast<const float2*>(cs + j));
-        const float2 s2 = __ldg(reinterpret_cast<const float2*>(sn + j));
-        // o[i] = y[i] c[i] - y[i+1] s[i];  o[i+1] = y[i+1] c[i+1] + y[i] s[i+1]
-        dy0 = go0 * c2.x + go1 * s2.y;
-        dy1 = go1 * c2.y - go0 * s2.x;
-      }
-      const float g0 = w ? dy0 * wv[i] : dy0, g1 = w ? dy1 * wv[i + 1] : dy1;
-      ss += x[i] * x[i] + x[i + 1] * x[i + 1];
-      sgx += g0 * x[i] + g1 * x[i + 1];
-      g[c + i] = g0;
-      g[c + i + 1] = g1;
-    }
-  }
-  ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-  sgx += __shfl_xor_sync(0xffffffffu, sgx, 1);
-  const float rstd = rsqrtf(ss / HD + eps);
-  const float m = sgx * rstd / HD;
-  if (row_ok) {
-#pragma unroll
-    for (int c = 0; c < NC; c += 8) {
-      float x[8], o[8];
-      unpack8(__ldg(reinterpret_cast<const uint4*>(xrow + c0 + c)), x);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) o[i] = rstd * (g[c + i] - (x[i] * rstd) * m);
-      *reinterpret_cast<uint4*>(grow + c0 + c) = pack8(o);
-    }
+    for (int i = 0; i < 8; ++i) o[i] = row[c0 + c + i];
+    *reinterpret_cast<uint4*>(grow + c0 + c) = pack8(o);
   }
 }
 
@@ -407,19 +346,10 @@ attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdPara
     named_bar_sync(2 + cw, 128);
     if (cw == 0) {
       store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dv + (long long)b * p.dv_b + (long long)kv * p.dv_s + (long long)h * p.dv_h,
-                         row_ok, false, nullptr, nullptr, nullptr, nullptr, 0.f);
+                         row_ok);
     } else {
-      const __nv_bfloat16* xrow = nullptr;
-      const __nv_bfloat16* wk = nullptr;
-      const float *cs = nullptr, *sn = nullptr;
-      if (p.fuse_prep) {   // dK row -> gradient of the k projection output (token index == key index)
-        xrow = p.src + (long long)b * p.src_b + (long long)min(kv, p.Sk - 1) * p.src_s + p.k_off + h * HD;
-        wk = (kv < p.s_split) ? p.wk1 : p.wk0;
-        cs = p.cosT ? p.cosT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
-        sn = p.sinT ? p.sinT + (long long)min(kv, p.Sk - 1) * HD : nullptr;
-      }
       store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dk + (long long)b * p.dk_b + (long long)kv * p.dk_s + (long long)h * p.dk_h,
-                         row_ok, p.fuse_prep != 0, xrow, wk, cs, sn, p.eps);
+                         row_ok);
     }
   }
 }
@@ -583,18 +513,8 @@ attn_bwd_dq_kernel(const __grid_constant__ AttnBwdMaps maps, const AttnBwdParams
     const bool row_ok = qrow < p.Sq;
     stage_acc<HD>(stage_rows, dq_acc, p.scale);
     named_bar_sync(2 + cw, 128);
-    const __nv_bfloat16* xrow = nullptr;
-    const __nv_bfloat16* wqn = nullptr;
-    const float *cs = nullptr, *sn = nullptr;
-    if (p.fuse_prep) {   // dQ row -> gradient of the q projection output
-      const int qc = min(qrow, p.Sq - 1);
-      xrow = p.src + (long long)b * p.src_b + (long long)qc * p.src_s + h * HD;
-      wqn = (qrow < p.s_split) ? p.wq1 : p.wq0;
-      cs = p.cosT ? p.cosT + (long long)qc * HD : nullptr;
-      sn = p.sinT ? p.sinT + (long long)qc * HD : nullptr;
-    }
     store_row_half<HD>(stage_rows + r * (HD + 4), half, p.dq + (long long)b * p.dq_b + (long long)qrow * p.dq_s + (long long)h * p.dq_h,
-                       row_ok, p.fuse_prep != 0, xrow, wqn, cs, sn, p.eps);
+                       row_ok);
   }
 }
 

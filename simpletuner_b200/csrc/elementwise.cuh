@@ -426,26 +426,24 @@ qk_rmsnorm_rope_bwd_kernel(const __nv_bfloat16* __restrict__ dq, const __nv_bflo
 }
 
 // ------------------------------------------------------------------------------------------------
-// "Flat" variants of the two kernels above for HD = 128 with frozen norm weights (the LoRA / LoKr training path): one
+// "Flat" variant of the backward kernel above for HD = 128 with frozen norm weights (the LoRA / LoKr training path): one
 // thread = one 16-byte chunk (8 elements) of one head row, 16 lanes = one head row, no per-thread loop — the launch
-// exposes B*S*2H*16 independent threads at ~56 registers instead of one warp walking 48 head rows of a token, i.e. the
+// exposes B*S*2H*16 independent threads at 44 registers instead of one warp walking 48 head rows of a token, i.e. the
 // memory-level parallelism of the plain streaming kernels.  Measured at the Flux shape (B = 4, S = 4608, 24 x 128;
 // tools/one_kernel.py time_rope_bwd): backward 169 us = 4.0 TB/s against 254 us for the warp-per-token loop (and 196-586 us
-// for its occupancy / unroll variants) -> the backward uses this kernel; forward 137 us against 114 us -> the forward keeps
-// the loop kernel (its cos / sin registers are amortised over 48 head rows there).  The token's cos / sin row (1 KB) is
-// re-read per head row and hits L1 (16 head rows of a token share a block).
+// for its occupancy / unroll variants) -> the backward uses this kernel; the same scheme for the forward took 137 us
+// against 114 us -> the forward keeps the loop kernel (its cos / sin registers are amortised over 48 head rows there).
+// The token's cos / sin row (1 KB) is re-read per head row and hits L1 (16 head rows of a token share a block).
+// g_q / g_k: gradients w.r.t. the post-RoPE q, k;  dsrc: the fused d_qkv buffer (q at column 0, k at column k_off).
 // ------------------------------------------------------------------------------------------------
-template <bool BWD>
 __global__ void __launch_bounds__(256)
-qk_rmsnorm_rope_flat128_kernel(const __nv_bfloat16* __restrict__ g_q, const __nv_bfloat16* __restrict__ g_k, long long g_b,
-                               long long g_s, const __nv_bfloat16* __restrict__ src, long long src_b, long long src_s,
-                               int k_off, const __nv_bfloat16* __restrict__ wq0, const __nv_bfloat16* __restrict__ wk0,
-                               const __nv_bfloat16* __restrict__ wq1, const __nv_bfloat16* __restrict__ wk1, int s_split,
-                               const float* __restrict__ cosT, const float* __restrict__ sinT,
-                               __nv_bfloat16* __restrict__ out_q, __nv_bfloat16* __restrict__ out_k, long long o_b,
-                               long long o_s, int B, int S, int H, float eps) {
-  // FWD: src = pre-norm projection output, out_q / out_k = post-norm / RoPE q, k ([B, S, H, 128] via o_b / o_s); g_* unused.
-  // BWD: g_q / g_k = gradients w.r.t. the post-RoPE q, k; out_q = the fused d_qkv buffer (out_k unused, k at column k_off).
+qk_rmsnorm_rope_flat128_bwd_kernel(const __nv_bfloat16* __restrict__ g_q, const __nv_bfloat16* __restrict__ g_k,
+                                   long long g_b, long long g_s, const __nv_bfloat16* __restrict__ src, long long src_b,
+                                   long long src_s, int k_off, const __nv_bfloat16* __restrict__ wq0,
+                                   const __nv_bfloat16* __restrict__ wk0, const __nv_bfloat16* __restrict__ wq1,
+                                   const __nv_bfloat16* __restrict__ wk1, int s_split, const float* __restrict__ cosT,
+                                   const float* __restrict__ sinT, __nv_bfloat16* __restrict__ dsrc, long long ds_b,
+                                   long long ds_s, int B, int S, int H, float eps) {
   constexpr int HD = 128;
   const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 4;   // (token, which, head)
   const int sub = threadIdx.x & 15;                                                   // 8-element chunk of the head row
@@ -478,47 +476,29 @@ qk_rmsnorm_rope_flat128_kernel(const __nv_bfloat16* __restrict__ g_q, const __nv
   float ss = 0.f;
 #pragma unroll
   for (int i = 0; i < 8; ++i) ss = fmaf(x[i], x[i], ss);
-  if constexpr (!BWD) {
+  float go[8], g[8];
+  unpack8(*reinterpret_cast<const uint4*>((which ? g_k : g_q) + b * g_b + s * g_s + hh * HD + sub * 8), go);
+  float sgx = 0.f;
 #pragma unroll
-    for (int o = 8; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    const float rstd = rsqrtf(ss / HD + eps);
-    float y[8], o8[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float n = bf16r(x[i] * rstd);            // fp32 normalise, cast to the weight dtype ...
-      y[i] = w ? bf16r(n * wv[i]) : n;               // ... then * weight (bf16 tensor op)
-    }
-#pragma unroll
-    for (int i = 0; i < 8; i += 2) {
-      o8[i] = y[i] * cs[i] + (-y[i + 1]) * sn[i];
-      o8[i + 1] = y[i + 1] * cs[i + 1] + y[i] * sn[i + 1];
-    }
-    if (live) *reinterpret_cast<uint4*>((which ? out_k : out_q) + b * o_b + s * o_s + hh * HD + sub * 8) = pack8(o8);
-  } else {
-    float go[8], g[8];
-    unpack8(*reinterpret_cast<const uint4*>((which ? g_k : g_q) + b * g_b + s * g_s + hh * HD + sub * 8), go);
-    float sgx = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; i += 2) {
-      const float dy0 = go[i] * cs[i] + go[i + 1] * sn[i + 1];
-      const float dy1 = go[i + 1] * cs[i + 1] - go[i] * sn[i];
-      g[i] = dy0 * wv[i];
-      g[i + 1] = dy1 * wv[i + 1];
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) sgx = fmaf(g[i], x[i], sgx);
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) {
-      ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      sgx += __shfl_xor_sync(0xffffffffu, sgx, o);
-    }
-    const float rstd = rsqrtf(ss / HD + eps);
-    const float m = sgx * rstd / HD;
-    float o8[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) o8[i] = rstd * (g[i] - (x[i] * rstd) * m);
-    if (live) *reinterpret_cast<uint4*>(out_q + b * o_b + s * o_s + (which ? k_off : 0) + hh * HD + sub * 8) = pack8(o8);
+  for (int i = 0; i < 8; i += 2) {
+    const float dy0 = go[i] * cs[i] + go[i + 1] * sn[i + 1];
+    const float dy1 = go[i + 1] * cs[i + 1] - go[i] * sn[i];
+    g[i] = dy0 * wv[i];
+    g[i + 1] = dy1 * wv[i + 1];
   }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) sgx = fmaf(g[i], x[i], sgx);
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) {
+    ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    sgx += __shfl_xor_sync(0xffffffffu, sgx, o);
+  }
+  const float rstd = rsqrtf(ss / HD + eps);
+  const float m = sgx * rstd / HD;
+  float o8[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) o8[i] = rstd * (g[i] - (x[i] * rstd) * m);
+  if (live) *reinterpret_cast<uint4*>(dsrc + b * ds_b + s * ds_s + (which ? k_off : 0) + hh * HD + sub * 8) = pack8(o8);
 }
 
 // ------------------------------------------------------------------------------------------------

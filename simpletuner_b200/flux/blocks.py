@@ -420,9 +420,7 @@ def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, s
                      dq=d_qkv[:, :, 0:D].unflatten(-1, (H, hd)), dk=d_qkv[:, :, D:2 * D].unflatten(-1, (H, hd)), dv=dv,
                      key_bias=key_bias)
         return d_qkv
-    # The backward of RMSNorm + RoPE stays a separate HBM-bound pass.  libstb200 can also run it inside the
-    # attention-backward epilogues (ops.attn_bwd(qk_prep=...), tests: attn_bwd_fused_prep*); the step keeps the separate
-    # pass because the longer epilogue of the fused form is not overlapped by anything (not measured on H100).
+    # The backward of RMSNorm + RoPE is a separate HBM-bound pass over the post-RoPE dq / dk.
     dq = torch.empty_like(q)
     dk = torch.empty_like(k)
     ops.attn_bwd(q, k, v, o.view(B, S, H, hd), d_o.view(B, S, H, hd), lse, dq=dq, dk=dk, dv=dv, key_bias=key_bias)

@@ -14,7 +14,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from ._lib import QkPrep, AttnBwdArgs, AttnFwdArgs, GemmArgs, check
+from ._lib import AttnBwdArgs, AttnFwdArgs, GemmArgs, check
 
 EPI_STORE, EPI_GELU, EPI_GATE_RES, EPI_MUL_DGELU, EPI_ADD_RES, EPI_MUL, EPI_QUICK_GELU, EPI_SILU = 0, 1, 2, 3, 4, 5, 6, 7
 
@@ -212,13 +212,9 @@ def attn_fwd(q, k, v, scale: Optional[float] = None, out: Optional[torch.Tensor]
     return out, lse
 
 
-def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=None, dv=None, qk_prep: Optional[dict] = None,
+def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=None, dv=None,
              key_bias: Optional[torch.Tensor] = None):
-    """Backward of attn_fwd.  Returns (dq, dk, dv) shaped like q, k, v ([B, S, H, HD], bf16).  key_bias: the forward's.
-
-    qk_prep (self-attention only): dict(src=[B,S,C] pre-norm projection output, k_off, wq, wk, wq_added, wk_added,
-    s_split, cos, sin, eps) — fuses the backward of qk_rmsnorm_rope_fwd into the epilogues, so dq / dk receive the
-    gradient w.r.t. the projection outputs (what qk_rmsnorm_rope_bwd would write)."""
+    """Backward of attn_fwd.  Returns (dq, dk, dv) shaped like q, k, v ([B, S, H, HD], bf16).  key_bias: the forward's."""
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (o, "o"), (d_o, "d_o")):
         _chk(t, n)
     B, Sq, H, HD = q.shape
@@ -237,25 +233,11 @@ def attn_bwd(q, k, v, o, d_o, lse, scale: Optional[float] = None, dq=None, dk=No
     a.v_b, a.v_s, a.v_h = v.stride(0), v.stride(1), v.stride(2)
     a.o_b, a.o_s, a.o_h = o.stride(0), o.stride(1), o.stride(2)
     a.do_b, a.do_s, a.do_h = d_o.stride(0), d_o.stride(1), d_o.stride(2)
-    a.lse, a.delta, a.dq_accum = lse.data_ptr(), delta.data_ptr(), None
+    a.lse, a.delta = lse.data_ptr(), delta.data_ptr()
     a.dq, a.dk, a.dv = dq.data_ptr(), dk.data_ptr(), dv.data_ptr()
     a.dq_b, a.dq_s, a.dq_h = dq.stride(0), dq.stride(1), dq.stride(2)
     a.dk_b, a.dk_s, a.dk_h = dk.stride(0), dk.stride(1), dk.stride(2)
     a.dv_b, a.dv_s, a.dv_h = dv.stride(0), dv.stride(1), dv.stride(2)
-    if qk_prep is not None:
-        f = _lib.QkPrep()
-        src = qk_prep["src"]
-        _chk(src, "qk_prep.src")
-        f.src, f.src_b, f.src_s, f.k_off = src.data_ptr(), src.stride(0), src.stride(1), int(qk_prep["k_off"])
-        f.wq, f.wk = _ptr(qk_prep.get("wq")), _ptr(qk_prep.get("wk"))
-        f.wq_added, f.wk_added = _ptr(qk_prep.get("wq_added")), _ptr(qk_prep.get("wk_added"))
-        f.s_split = int(qk_prep.get("s_split", 0))
-        cos, sin = qk_prep.get("cos"), qk_prep.get("sin")
-        if cos is not None:
-            assert cos.dtype == torch.float32 and cos.is_contiguous() and cos.shape == (Sq, HD) and sin.shape == (Sq, HD)
-        f.cos_t, f.sin_t = _ptr(cos), _ptr(sin)
-        f.eps = float(qk_prep.get("eps", 1e-6))
-        a.qk_prep = C.pointer(f)
     if key_bias is not None:
         a.bias, a.bias_b = key_bias.data_ptr(), _key_bias_stride(key_bias, B, Sk)
         _set_live(a, _key_live(key_bias))

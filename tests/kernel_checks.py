@@ -1880,48 +1880,6 @@ CHECKS.update({
 })
 
 
-# --------------------------------------------------------------------------------------------- fused q/k-prep backward epilogue
-def check_attn_bwd_fused_prep(B=2, S=333, H=3, HD=128, s_split=77, rope=True, norm_w=True, key_bias=None):
-    """attn_bwd(qk_prep=...) == attn_bwd -> qk_rmsnorm_rope_bwd (the two-kernel path) on the same inputs; dv, which the
-    prep does not touch, bit for bit.  key_bias: None or a _key_bias kind."""
-    D = H * HD
-    qkv = _rand(B, S, 3 * D, seed=1)
-    d_o = _rand(B, S, H, HD, seed=2)
-    mk = lambda sd: (1.0 + 0.1 * _rand(HD, seed=sd).float()).bfloat16() if norm_w else None
-    wq, wk, wqa, wka = mk(3), mk(4), mk(5), mk(6)
-    cos, sin = _rope_tables(S, HD) if rope else (None, None)
-    kb = _key_bias(key_bias, B, S, seed=9) if key_bias else None
-    q, k = ops.qk_rmsnorm_rope_fwd(qkv, D, H, HD, wq, wk, wqa, wka, s_split, cos, sin, 1e-6)
-    v = qkv[:, :, 2 * D:].unflatten(-1, (H, HD))
-    o, lse = ops.attn_fwd(q, k, v, key_bias=kb)
-    # reference: two kernels
-    dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse, key_bias=kb)
-    ref = torch.zeros_like(qkv)
-    ops.qk_rmsnorm_rope_bwd(dq, dk, qkv, D, H, HD, wq, wk, wqa, wka, s_split, cos, sin, 1e-6, dsrc=ref)
-    ref[:, :, 2 * D:] = dv.reshape(B, S, D)
-    got = torch.zeros_like(qkv)
-    ops.attn_bwd(q, k, v, o, d_o, lse, dq=got[:, :, 0:D].unflatten(-1, (H, HD)), dk=got[:, :, D:2 * D].unflatten(-1, (H, HD)),
-                 dv=got[:, :, 2 * D:].unflatten(-1, (H, HD)), key_bias=kb,
-                 qk_prep=dict(src=qkv, k_off=D, wq=wq, wk=wk, wq_added=wqa, wk_added=wka, s_split=s_split, cos=cos, sin=sin, eps=1e-6))
-    torch.cuda.synchronize()
-    # Both sides are bf16 and the two-kernel path rounds dq / dk to bf16 before the norm backward, the fused one does not:
-    # the two results may land on neighbouring bf16 values, one ulp = up to 2^-7 |x| apart, hence rtol 2^-6.
-    rows = lambda t: t.unflatten(-1, (3 * H, HD))   # one row per token and head, as attn_compare scales its atol
-    r = _report(f"attn_bwd_fused_prep_S{S}_HD{HD}_rope{int(rope)}_w{int(norm_w)}" + (f"_kb_{key_bias}" if key_bias else ""),
-                rows(got), rows(ref), atol=2e-2 * _row_rms(rows(ref)), rtol=2 ** -6)
-    r["dv_exact"] = bool(torch.equal(got[:, :, 2 * D:], ref[:, :, 2 * D:]))
-    r["ok"] = r["ok"] and r["dv_exact"]
-    return r
-
-
-CHECKS.update({
-    "attn_bwd_fused_prep": lambda: check_attn_bwd_fused_prep(),
-    "attn_bwd_fused_prep_hd64_norope": lambda: check_attn_bwd_fused_prep(B=1, S=320, H=4, HD=64, s_split=0, rope=False),
-    "attn_bwd_fused_prep_now": lambda: check_attn_bwd_fused_prep(B=1, S=256, H=2, HD=128, s_split=0, rope=True, norm_w=False),
-    "attn_bwd_fused_prep_key_bias": lambda: check_attn_bwd_fused_prep(key_bias="dense"),
-})
-
-
 # --------------------------------------------------------------------------------------------- implicit-GEMM conv at VAE sizes
 # (many persistent tiles per CTA; output rows that are not a multiple of the 128-pixel tile).  "pair" in the names is
 # historical: these are the larger conv shapes, run by the same one-CTA wgmma kernel as the small ones.

@@ -8,7 +8,7 @@ import torch
 import torch.nn.functional as F
 
 from simpletuner_b200 import ops
-from tests.kernel_checks import _attn_ref, _key_bias, attn_compare, check_attn_bwd_fused_prep
+from tests.kernel_checks import _attn_ref, _key_bias, attn_compare
 
 pytestmark = pytest.mark.gpu
 
@@ -85,11 +85,6 @@ def test_all_ones_bias_equals_no_bias_in_the_backward_exponent():
     assert float((o1.float() - o0.float()).abs().max()) <= 1e-2 and torch.allclose(l1, l0 + 1.0, atol=1e-4)
     ref = _attn_ref(q, k, v, HD ** -0.5, d_o=d_o, o=o1)
     r = attn_compare("all_ones", dict(zip(("dq", "dk", "dv"), g1)), ref)
-    assert r["ok"], r
-
-
-def test_fused_qk_prep_with_key_bias_equals_the_separate_pass():
-    r = check_attn_bwd_fused_prep(B=2, S=333, H=3, HD=128, s_split=77, key_bias="01")
     assert r["ok"], r
 
 

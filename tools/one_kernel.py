@@ -111,7 +111,7 @@ elif which == "time_tail":
     res["adamw_bf16_multi"] = {"ms": t, "GBps": n_el * 18 / t / 1e6}
     print(json.dumps(res))
 elif which == "time_rope_bwd":
-    import json, os
+    import json
     B, S, H, HD, D = 4, 4608, 24, 128, 3072
     qkv = torch.randn(B, S, 3 * D, device="cuda").bfloat16()
     wq, wk = torch.ones(HD, device="cuda").bfloat16(), torch.ones(HD, device="cuda").bfloat16()
@@ -129,7 +129,7 @@ elif which == "time_rope_bwd":
     e1.record()
     torch.cuda.synchronize()
     t = e0.elapsed_time(e1) / 20
-    print(json.dumps({"variant": os.environ.get("STB_ROPE_BWD_VARIANT", "0"), "ms": t, "GBps": 6 * B * S * D * 2 / t / 1e6, "checksum": float(dqkv[:, :, :2 * D].float().abs().mean())}))
+    print(json.dumps({"kernel": "qk_rmsnorm_rope_bwd", "ms": t, "GBps": 6 * B * S * D * 2 / t / 1e6, "checksum": float(dqkv[:, :, :2 * D].float().abs().mean())}))
     fq = lambda: ops.qk_rmsnorm_rope_fwd(qkv, D, H, HD, wq, wk, None, None, 0, cos, sin, 1e-6)
     for _ in range(3):
         q_, k_ = fq()
@@ -140,6 +140,6 @@ elif which == "time_rope_bwd":
     e1.record()
     torch.cuda.synchronize()
     t = e0.elapsed_time(e1) / 20
-    print(json.dumps({"fwd_variant": os.environ.get("STB_ROPE_FWD_VARIANT", "0"), "ms": t, "GBps": 4 * B * S * D * 2 / t / 1e6, "checksum": float(q_.float().abs().mean() + k_.float().abs().mean())}))
+    print(json.dumps({"kernel": "qk_rmsnorm_rope_fwd", "ms": t, "GBps": 4 * B * S * D * 2 / t / 1e6, "checksum": float(q_.float().abs().mean() + k_.float().abs().mean())}))
 torch.cuda.synchronize()
 print("done", which)
