@@ -10,7 +10,9 @@ A family sets class attributes and writes only the steps that are its own:
     loss kernel's layout;
   * `FLAVOURS`, `LORA_TYPES`, `REFUSED_OPTIONS` and `REFUSED_BATCH_KEYS`: what `validate_config` and `_check_supported`
     refuse, so that the shim keeps the reference class for it (INTEGRATION.md §2);
-  * `PREDICTION_TYPES`: the `prediction_type` values a DDPM family's loss implements.
+  * `PREDICTION_TYPES`: the `prediction_type` values a DDPM family's loss implements;
+  * `FULL_FINETUNE`: whether `model_type="full"` runs on this path (the denoiser has `enable_full_finetune()`); such a run
+    is checked by `validate_full_finetune`.
 """
 from __future__ import annotations
 
@@ -53,6 +55,7 @@ class StepWrapper:
     REFUSED_OPTIONS: Sequence[str] = ()     # the family's refusals on top of _REFUSED_FLAGS
     REFUSED_BATCH_KEYS: Sequence[str] = ()
     PREDICTION_TYPES: Sequence[str] = ()
+    FULL_FINETUNE = False
 
     def __init__(self, config: Optional[SimpleNamespace] = None, transformer=None, device: Optional[torch.device] = None,
                  **transformer_kwargs):
@@ -131,9 +134,20 @@ class StepWrapper:
     # ------------------------------------------------------------------------------------------
     @classmethod
     def validate_config(cls, c) -> None:
-        """Load-time counterpart of the per-batch guards: options of the reference this path does not implement raise
-        NotImplementedError so that the shim (shim/foundation.py) keeps the reference module for such a run.  Whether the
-        resolved LoRA targets can be adapted is the denoiser's rule (`lora_target_linears`), which the shim applies."""
+        """Load-time counterpart of the per-batch guards for a LoRA run: options of the reference this path does not
+        implement raise NotImplementedError so that the shim (shim/foundation.py) keeps the reference module for such a run.
+        Whether the resolved LoRA targets can be adapted is the denoiser's rule (`lora_target_linears`), which the shim
+        applies.  A `model_type="full"` run is checked by `validate_full_finetune` instead."""
+        cls._validate(c, full=False)
+
+    @classmethod
+    def validate_full_finetune(cls, c) -> None:
+        """The load-time check of a `model_type="full"` run: admitted where the family sets `FULL_FINETUNE`, with the same
+        refusals as a LoRA run (so LyCORIS, DoRA and controlnet still keep the reference module)."""
+        cls._validate(c, full=True)
+
+    @classmethod
+    def _validate(cls, c, full: bool) -> None:
         g = lambda k, d=None: getattr(c, k, d)
         fl = g("model_flavour", None)
         if cls.FLAVOURS and fl and fl not in cls.FLAVOURS:
@@ -141,7 +155,8 @@ class StepWrapper:
                                       f"(supported: {cls.FLAVOURS})")
         if g("controlnet", False):
             raise NotImplementedError("ControlNet (controlnet) training is not supported by the libstb200 path")
-        if str(g("model_type", "lora")) != "lora":
+        model_type = str(g("model_type", "lora"))
+        if model_type != "lora" and not (full and model_type == "full" and cls.FULL_FINETUNE):
             raise NotImplementedError(f"model_type={g('model_type')!r}: only LoRA training runs on the libstb200 path")
         if lora_type(c) not in cls.LORA_TYPES:
             raise NotImplementedError(f"lora_type={g('lora_type')!r} on {cls.NAME} is not supported by the libstb200 path")

@@ -62,6 +62,7 @@ class PixartSigma(StepWrapper):
     DENOISER = PixArtTransformer2DModel
     DEFAULT_CONFIG = staticmethod(default_config)
     PACKED_LAYOUT = "packed_dydxc"
+    FULL_FINETUNE = True
 
     def _noise_schedule(self):
         # PixArt-Sigma scheduler_config.json: DDPM, 1000 steps, linear betas 1e-4 .. 0.02, epsilon

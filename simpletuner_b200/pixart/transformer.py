@@ -20,7 +20,7 @@ The additive -10000 key mask of cross attention (reference :562-564) rides in th
 q[..., 72] = 1 (a bias entry of the padded to_q), k[b, j, :, 72] = -10000 / scale for masked keys — masked keys get
 probability exactly 0 like the reference's fp32 softmax, with no mask operand in the kernel.
 Unsupported (raise): token-wise timesteps, TREAD routes, controlnet residuals, flow-map `r_timestep`, GLIGEN,
-self-attention masks, full fine-tune.
+self-attention masks.  Full fine-tune (model_type=full) runs through pixart/fullft.py after `enable_full_finetune()`.
 """
 from __future__ import annotations
 
@@ -35,6 +35,7 @@ from .. import ops
 from ..flux.blocks import EPS, MlpPlan, TailFn, _linear_lora_dgrad, _linear_lora_fwd, _lora_grads, _t, _wt, pack_lora
 from ..flux.transformer import (AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, Linear, _FeedForward, _lora_list, _sinusoid,
                                 _TimestepEmbedding)
+from ..pretrained import ModelConfig, PretrainedIOAPI
 
 PIXART_LORA_TARGETS = ["to_k", "to_q", "to_v", "to_out.0"]  # PixartSigma.DEFAULT_LORA_TARGET, reference pixart/model.py:59
 MASK_BIAS = -10000.0
@@ -212,6 +213,8 @@ class PixArtTransformerBlock(nn.Module):
     def plans(self):
         if self._plans is None:
             H, hd, hdp = self.heads, self.head_dim, self.hdp
+            dyn = bool(getattr(self, "_full_ft", False))      # full fine-tune: the weights change every step
+            wt = lambda w: _wt(w, dyn)
             pr = lambda lin: (_pad_rows(lin.weight.detach(), H, hd, hdp), _pad_rows(lin.bias.detach(), H, hd, hdp))
             a1, a2 = self.attn1, self.attn2
             (wq, bq), (wk, bk), (wv, bv) = pr(a1.to_q), pr(a1.to_k), pr(a1.to_v)
@@ -221,17 +224,18 @@ class PixArtTransformerBlock(nn.Module):
                 b_q2 = b_q2.clone()
                 b_q2.view(H, hdp)[:, hd] = 1.0           # the query side of the mask column
             (wk2, bk2), (wv2, bv2) = pr(a2.to_k), pr(a2.to_v)
+            w_kv2 = torch.cat([wk2, wv2], 0).contiguous()
             w_out1 = _pad_cols(a1.to_out[0].weight.detach(), H, hd, hdp)
             w_out2 = _pad_cols(a2.to_out[0].weight.detach(), H, hd, hdp)
             ff = self.ff
             self._plans = {
-                "w_qkv1": w_qkv1, "b_qkv1": torch.cat([bq, bk, bv], 0).contiguous(), "w_qkv1_t": _wt(w_qkv1),
-                "w_out1": w_out1, "b_out1": a1.to_out[0].bias.detach(), "w_out1_t": _wt(w_out1),
-                "w_q2": w_q2, "b_q2": b_q2, "w_q2_t": _wt(w_q2),
-                "w_kv2": torch.cat([wk2, wv2], 0).contiguous(), "b_kv2": torch.cat([bk2, bv2], 0).contiguous(),
-                "w_out2": w_out2, "b_out2": a2.to_out[0].bias.detach(), "w_out2_t": _wt(w_out2),
-                "mlp": MlpPlan(ff.net[0].proj.weight.detach(), ff.net[0].proj.bias.detach(), _wt(ff.net[0].proj.weight.detach()),
-                               ff.net[2].weight.detach(), ff.net[2].bias.detach(), _wt(ff.net[2].weight.detach())),
+                "w_qkv1": w_qkv1, "b_qkv1": torch.cat([bq, bk, bv], 0).contiguous(), "w_qkv1_t": wt(w_qkv1),
+                "w_out1": w_out1, "b_out1": a1.to_out[0].bias.detach(), "w_out1_t": wt(w_out1),
+                "w_q2": w_q2, "b_q2": b_q2, "w_q2_t": wt(w_q2),
+                "w_kv2": w_kv2, "b_kv2": torch.cat([bk2, bv2], 0).contiguous(), "w_kv2_t": wt(w_kv2) if dyn else None,
+                "w_out2": w_out2, "b_out2": a2.to_out[0].bias.detach(), "w_out2_t": wt(w_out2),
+                "mlp": MlpPlan(ff.net[0].proj.weight.detach(), ff.net[0].proj.bias.detach(), wt(ff.net[0].proj.weight.detach()),
+                               ff.net[2].weight.detach(), ff.net[2].bias.detach(), wt(ff.net[2].weight.detach())),
             }
         return self._plans
 
@@ -241,6 +245,10 @@ class PixArtTransformerBlock(nn.Module):
         mod = (self.scale_shift_table[None] + t6.reshape(B, 6, D)).reshape(B, 6 * D)
         st = {"H": self.heads, "hd": self.head_dim, "hdp": self.hdp, "plans": self.plans(), "lora_scaling": lora_scaling,
               "pad_index": pad_index, "lora_drop": getattr(self, "_lora_drop", None)}
+        if getattr(self, "_full_ft", False):
+            from .fullft import BLOCK_PARAMS, PixArtBlockFullFn
+            params = dict(self.named_parameters())
+            return PixArtBlockFullFn.apply(h, ctx, kbias, mod, st, *[params[n] for n in BLOCK_PARAMS])
         a1, a2 = self.attn1, self.attn2
         lora = _lora_list([a1.to_q, a1.to_k, a1.to_v, a1.to_out[0], a2.to_q, a2.to_k, a2.to_v, a2.to_out[0]])
         return PixArtBlockFn.apply(h, ctx, kbias, mod, st, *lora)
@@ -304,7 +312,7 @@ def sincos_pos_embed_2d(dim: int, grid_h: int, grid_w: int, base_size: int, inte
     return torch.cat(parts, dim=1).float().to(device)
 
 
-class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, nn.Module):
+class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, PretrainedIOAPI, nn.Module):
     _no_split_modules = ["BasicTransformerBlock", "PatchEmbed"]
     _DEFAULT_LORA_TARGETS = PIXART_LORA_TARGETS
 
@@ -329,12 +337,12 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         D = num_attention_heads * attention_head_dim
         if cross_attention_dim is None:
             cross_attention_dim = D
-        self.config = SimpleNamespace(num_attention_heads=num_attention_heads, attention_head_dim=attention_head_dim,
-                                      in_channels=in_channels, out_channels=out_channels, num_layers=num_layers,
-                                      cross_attention_dim=cross_attention_dim, sample_size=sample_size, patch_size=patch_size,
-                                      interpolation_scale=interpolation_scale, use_additional_conditions=use_additional_conditions,
-                                      caption_channels=caption_channels, norm_type=norm_type, norm_eps=norm_eps,
-                                      activation_fn=activation_fn, attention_bias=attention_bias)
+        self.config = ModelConfig(num_attention_heads=num_attention_heads, attention_head_dim=attention_head_dim,
+                                  in_channels=in_channels, out_channels=out_channels, num_layers=num_layers,
+                                  cross_attention_dim=cross_attention_dim, sample_size=sample_size, patch_size=patch_size,
+                                  interpolation_scale=interpolation_scale, use_additional_conditions=use_additional_conditions,
+                                  caption_channels=caption_channels, norm_type=norm_type, norm_eps=norm_eps,
+                                  activation_fn=activation_fn, attention_bias=attention_bias)
         self.inner_dim, self.out_channels, self.use_additional_conditions = D, out_channels, use_additional_conditions
         self.attention_head_dim = attention_head_dim
         self.interpolation_scale = interpolation_scale if interpolation_scale is not None else max(sample_size // 64, 1)
@@ -359,11 +367,38 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         return ".attn1." in name or ".attn2." in name
 
     def invalidate_plans(self):
+        self._drop_weight_layouts()
+        self._pos_cache.clear()
+        self._pad_index = None
+
+    def _drop_weight_layouts(self):
         for blk in self.transformer_blocks:
             blk._plans = None
         self._tail_plan = {}
-        self._pos_cache.clear()
-        self._pad_index = None
+
+    def enable_full_finetune(self, enabled: bool = True):
+        """model_type=full: every parameter trains, the blocks' `scale_shift_table` included.  The blocks switch to the full
+        fine-tune schedule (pixart/fullft.py); the padded / fused / transposed weight layouts are rebuilt after every
+        optimizer step (`after_optimizer_step`) because the base weights now change."""
+        if enabled and self.lora_linears():
+            raise NotImplementedError("full fine-tune and LoRA adapters are mutually exclusive on the libstb200 path")
+        self._full_ft = bool(enabled)
+        for p in self.parameters():
+            p.requires_grad_(bool(enabled))
+        for blk in self.transformer_blocks:
+            blk._full_ft = bool(enabled)
+        self.invalidate_plans()
+        return self
+
+    def after_optimizer_step(self):
+        if getattr(self, "_full_ft", False):
+            self._drop_weight_layouts()
+
+    def before_graph_capture(self):
+        """training.step.GraphedTrainStep: in full fine-tune the weight layouts are rebuilt INSIDE the captured step.  The
+        positional tables and the pad index do not depend on the weights and stay (building them copies from the host)."""
+        if getattr(self, "_full_ft", False):
+            self._drop_weight_layouts()
 
     # ---- forward --------------------------------------------------------------------------------
     def _pos(self, hp: int, wp: int, dtype, device) -> torch.Tensor:
@@ -416,13 +451,20 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         # 1. input: PatchEmbed conv2x2/s2 == GEMM over (c, dy, dx) features, + sincos table in the epilogue
         x = _packed_latents if _packed_latents is not None else \
             hidden_states.to(dt).view(B, C, hp, 2, wp, 2).permute(0, 2, 4, 1, 3, 5).reshape(B, S, C * 4).contiguous()
-        w_pe = self.pos_embed.proj.weight.detach().reshape(D, C * 4)
-        h = ops.gemm([x], [w_pe], self.pos_embed.proj.bias.detach(), epi=ops.EPI_ADD_RES,
-                     res=self._pos(hp, wp, dt, dev).expand(B, S, D))
+        full = getattr(self, "_full_ft", False) and torch.is_grad_enabled()
+        pos = self._pos(hp, wp, dt, dev).expand(B, S, D)
+        if full:
+            from .fullft import CaptionProjectionFullFn, PatchEmbedFullFn
+            h = PatchEmbedFullFn.apply(x, pos, self.pos_embed.proj.weight, self.pos_embed.proj.bias)
+        else:
+            w_pe = self.pos_embed.proj.weight.detach().reshape(D, C * 4)
+            h = ops.gemm([x], [w_pe], self.pos_embed.proj.bias.detach(), epi=ops.EPI_ADD_RES, res=pos)
         t6, embedded = self._conditioning(timestep.to(dev), added_cond_kwargs, B, dt)
         ctx = encoder_hidden_states.to(dt).contiguous()
         if self.caption_projection is not None:
-            ctx = self.caption_projection(ctx)
+            cp = self.caption_projection
+            ctx = CaptionProjectionFullFn.apply(ctx, cp.linear_1.weight, cp.linear_1.bias, cp.linear_2.weight,
+                                                cp.linear_2.bias) if full else cp(ctx)
         # 2. cross-attention key mask -> the padded q/k column (module docstring)
         kbias = None
         if encoder_attention_mask is not None:
@@ -443,18 +485,41 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         mod = (self.scale_shift_table[None] + embedded[:, None].to(self.scale_shift_table.dtype)).to(dt)  # [B, 2, D] (shift | scale)
         mod = torch.cat([mod[:, 1], mod[:, 0]], dim=1).contiguous()                                         # TailFn wants (scale | shift)
         keep = self.out_channels // 2 if _packed_output == "eps_half" else self.out_channels
-        tp = self._tail_plan.get(keep)
-        if tp is None:
-            w, b = self.proj_out.weight.detach(), self.proj_out.bias.detach()
-            if keep != self.out_channels:   # PixartSigma keeps `.chunk(2, dim=1)[0]` only (pixart/model.py:313): skip the rest
-                sel = (torch.arange(4, device=dev)[:, None] * self.out_channels + torch.arange(keep, device=dev)[None, :]).reshape(-1)
-                w, b = w[sel].contiguous(), b[sel].contiguous()
-            tp = {"w_proj": w, "b_proj": b, "w_proj_t": _wt(w)}
-            self._tail_plan[keep] = tp
-        out = TailFn.apply(h, mod, {"S_txt": 0, **tp})          # [B, S, 4 * keep] in (dy, dx, c) order
+        if full:
+            out = self._tail_full(h, mod, keep)
+        else:
+            out = self._tail(h, mod, keep)
         if not _packed_output:
             Co = self.out_channels
             out = torch.einsum("nhwpqc->nchpwq", out.reshape(B, hp, wp, 2, 2, Co)).reshape(B, Co, hp * 2, wp * 2)
         if not return_dict:
             return (out,)
         return SimpleNamespace(sample=out)
+
+    def _tail_rows(self, keep: int, dev) -> Optional[torch.Tensor]:
+        """The proj_out rows of the first `keep` output channels ((dy, dx, c) row order); None: every row."""
+        if keep == self.out_channels:
+            return None
+        return (torch.arange(4, device=dev)[:, None] * self.out_channels + torch.arange(keep, device=dev)[None, :]).reshape(-1)
+
+    def _tail_full(self, h, mod, keep):
+        """Full fine-tune tail: gradients for proj_out and the modulation.  Only the kept rows are computed; the gather
+        hands the learned-sigma rows an explicit zero gradient, as the reference's `.chunk(2, dim=1)[0]` does."""
+        from ..sd3.fullft import TailFullFn
+        w, b = self.proj_out.weight, self.proj_out.bias
+        sel = self._tail_rows(keep, h.device)
+        if sel is not None:
+            w, b = w[sel], b[sel]
+        return TailFullFn.apply(h, mod, w, b, 0)
+
+    def _tail(self, h, mod, keep):
+        dev = h.device
+        tp = self._tail_plan.get(keep)
+        if tp is None:
+            w, b = self.proj_out.weight.detach(), self.proj_out.bias.detach()
+            sel = self._tail_rows(keep, dev)
+            if sel is not None:   # PixartSigma keeps `.chunk(2, dim=1)[0]` only (pixart/model.py:313): skip the rest
+                w, b = w[sel].contiguous(), b[sel].contiguous()
+            tp = {"w_proj": w, "b_proj": b, "w_proj_t": _wt(w)}
+            self._tail_plan[keep] = tp
+        return TailFn.apply(h, mod, {"S_txt": 0, **tp})          # [B, S, 4 * keep] in (dy, dx, c) order

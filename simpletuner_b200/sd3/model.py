@@ -19,6 +19,7 @@ class SD3(StepWrapper):
     DENOISER = SD3Transformer2DModel
     DEFAULT_CONFIG = staticmethod(default_config)
     PACKED_LAYOUT = "packed_dydxc"
+    FULL_FINETUNE = True
     REFUSED_BATCH_KEYS = CONDITIONING_INPUTS
 
     def model_predict(self, prepared_batch: Dict[str, Any]) -> Dict[str, Any]:

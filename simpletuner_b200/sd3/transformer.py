@@ -28,6 +28,7 @@ from .. import ops
 from ..flux.blocks import DoubleBlockFn, TailFn, _wt
 from ..flux.transformer import (_ATTN, AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, Linear, RMSNormWeight, _AdaNorm,
                                 _FeedForward, _TimestepEmbedding, _attn_plan, _lora_list, _mlp_plan, _sinusoid)
+from ..pretrained import ModelConfig, PretrainedIOAPI
 
 SD3_LORA_TARGETS = ["to_k", "to_q", "to_v", "to_out.0"]  # SD3.DEFAULT_LORA_TARGET, reference sd3/model.py:122
 _ADAPTABLE_SUFFIXES = tuple("." + t for t in _ATTN)
@@ -145,7 +146,7 @@ class _TimeTextEmbed(nn.Module):
         self.text_embedder = _TimestepEmbedding(pooled_dim, dim, dtype)
 
 
-class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, nn.Module):
+class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, PretrainedIOAPI, nn.Module):
     _no_split_modules = ["JointTransformerBlock"]
     _DEFAULT_LORA_TARGETS = SD3_LORA_TARGETS
 
@@ -159,12 +160,12 @@ class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, n
             raise NotImplementedError("libstb200 SD3 path supports patch_size=2")
         if attention_head_dim not in (64, 128):
             raise NotImplementedError("libstb200 attention supports head_dim 64 / 128")
-        self.config = SimpleNamespace(sample_size=sample_size, patch_size=patch_size, in_channels=in_channels,
-                                      num_layers=num_layers, attention_head_dim=attention_head_dim,
-                                      num_attention_heads=num_attention_heads, joint_attention_dim=joint_attention_dim,
-                                      caption_projection_dim=caption_projection_dim, pooled_projection_dim=pooled_projection_dim,
-                                      out_channels=out_channels, pos_embed_max_size=pos_embed_max_size,
-                                      dual_attention_layers=tuple(dual_attention_layers), qk_norm=qk_norm)
+        self.config = ModelConfig(sample_size=sample_size, patch_size=patch_size, in_channels=in_channels,
+                                  num_layers=num_layers, attention_head_dim=attention_head_dim,
+                                  num_attention_heads=num_attention_heads, joint_attention_dim=joint_attention_dim,
+                                  caption_projection_dim=caption_projection_dim, pooled_projection_dim=pooled_projection_dim,
+                                  out_channels=out_channels, pos_embed_max_size=pos_embed_max_size,
+                                  dual_attention_layers=tuple(dual_attention_layers), qk_norm=qk_norm)
         self.out_channels = out_channels if out_channels is not None else in_channels
         self.inner_dim = D = num_attention_heads * attention_head_dim
         if caption_projection_dim != D:

@@ -9,5 +9,6 @@ Nothing here imports the reference at module import time: `install()` does, and 
 combined with the reference family class (`make_b200_family(RefFlux, "flux")`), so the same code is testable against a
 stub that reproduces `ModelFoundation.load_model`'s hook order (tests/test_shim_cpu.py, tests/test_shim_gpu.py).
 """
-from .foundation import B200FoundationMixin, FAMILIES, OPT_IN_FAMILIES, install, install_lycoris, make_b200_family  # noqa: F401
+from .foundation import (B200FoundationMixin, FAMILIES, OPT_IN_FAMILIES, install, install_lycoris, make_b200_family,  # noqa: F401
+                         track_full_finetune)
 from .vae import B200VAEMixin  # noqa: F401

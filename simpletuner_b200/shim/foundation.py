@@ -16,6 +16,7 @@ exactly like the unmodified reference).
 from __future__ import annotations
 
 import logging
+import weakref
 from dataclasses import dataclass
 from typing import Any, Callable, Dict, Optional, Sequence, Tuple
 
@@ -165,19 +166,25 @@ class B200FoundationMixin:
         if dtype != torch.bfloat16:
             raise NotImplementedError(f"libstb200 computes in bf16; weight_dtype={dtype}")
         step_cls = spec.step()
-        step_cls.validate_config(self.config)                      # raises NotImplementedError on unsupported options
+        full = str(getattr(self.config, "model_type", "lora")) == "full"
+        # both raise NotImplementedError on unsupported options (full fine-tuning: outside SD3 / PixArt too)
+        (step_cls.validate_full_finetune if full else step_cls.validate_config)(self.config)
         if lora_type(self.config) == "lycoris" and not _LYCORIS_ROUTED:
             # trainer.py:3391 calls the third-party `lycoris.create_lycoris` on the trained component; that wrapper only knows
             # torch.nn modules.  Only with `install_lycoris()` (which routes B200 denoisers to simpletuner_b200.lycoris) may
             # the swap happen for a LyCORIS run (validate_config admits it only where the block schedules carry LoKr).
             raise NotImplementedError("LyCORIS run: call simpletuner_b200.shim.install_lycoris() first (Flux LoKr only)")
         den = spec.denoiser()(**kwargs)
-        den.lora_target_linears(step_cls.lora_targets(self.config))     # a target the fused path cannot adapt raises here
+        if not full:
+            den.lora_target_linears(step_cls.lora_targets(self.config))  # a target the fused path cannot adapt raises here
         missing, unexpected = den.load_state_dict(ref.state_dict(), strict=False)
         missing = [k for k in missing if "lora_" not in k]
         unexpected = [k for k in unexpected if "lora_" not in k]
         if missing or unexpected:
             raise NotImplementedError(f"state-dict mismatch (missing {missing[:3]}, unexpected {unexpected[:3]})")
+        if full:
+            den.enable_full_finetune()
+            track_full_finetune(den)
         den.to(self.accelerator.device)
         # apply_gradient_checkpointing_settings() ran BEFORE this hook on the reference module (common.py:3545): carry over
         if getattr(ref, "gradient_checkpointing", False):
@@ -225,6 +232,29 @@ class B200FoundationMixin:
         if step is None:
             return super().loss_with_logs(prepared_batch, model_output, apply_conditioning_mask=apply_conditioning_mask)
         return step.loss_with_logs(prepared_batch, model_output, apply_conditioning_mask=apply_conditioning_mask)
+
+
+# Full fine-tune denoisers whose derived weight layouts must follow every optimizer step.  The reference trainer steps its
+# optimizer itself (trainer.py:7239), so one process-wide optimizer post-hook calls `after_optimizer_step()` on each; the
+# parameters' version counters cannot stand in for it, because the fused AdamW kernels write through `data_ptr`.
+_FULL_FT_MODELS: "weakref.WeakSet" = weakref.WeakSet()
+_STEP_HOOK = None
+
+
+def _after_optimizer_step(optimizer, args, kwargs):
+    for den in list(_FULL_FT_MODELS):
+        den.after_optimizer_step()
+
+
+def track_full_finetune(den) -> None:
+    """Rebuild `den`'s derived layouts after every optimizer step of this process (weakly referenced: a freed model is
+    dropped).  TrainStep's own `after_optimizer_step()` call comes on top; the second drop of the layouts is a no-op."""
+    global _STEP_HOOK
+    from torch.optim import optimizer
+
+    _FULL_FT_MODELS.add(den)
+    if _STEP_HOOK is None:
+        _STEP_HOOK = optimizer.register_optimizer_step_post_hook(_after_optimizer_step)
 
 
 def make_b200_family(reference_cls: type, family: str) -> type:
