@@ -37,7 +37,8 @@ def adamw_bf16_step(p: Tensor, grad: Tensor, shift: Tensor, exp_avg: Tensor, exp
     scalar_semantics: PyTorch itself evaluates three of these ops differently on CPU and CUDA —
       * bf16 `add_(scalar / alpha)`: the CPU kernels cast the Python scalar to bf16 first, the CUDA kernels keep it in fp32
         (`sqrt().add_(eps)`, `shift.add_(p, alpha=-decay)`);
-      * `addcdiv_`: CPU computes `self + (value * t1) / t2`, CUDA `self + value * (t1 / t2)` (fused multiply-add).
+      * `addcdiv_`: CPU computes `self + (value * t1) / t2`, CUDA `self + value * (t1 / t2)` (fused multiply-add);
+      * `addcmul_`: CPU computes `self + (value * t1) * t2`, CUDA `self + value * (t1 * t2)`.
     "cpu" follows the former (bit-exact against the reference executed here, tests/golden/adamw_bf16_golden.pt),
     "cuda" the latter — what the reference does on a GPU and what `stb_adamw_bf16_multi` implements."""
     cuda = scalar_semantics == "cuda"
@@ -45,7 +46,12 @@ def adamw_bf16_step(p: Tensor, grad: Tensor, shift: Tensor, exp_avg: Tensor, exp
     res = grad.to(torch.float32)
     res.add_(exp_avg, alpha=1 - beta1)                       # other + alpha * input  (quirk Q-opt)
     exp_avg.copy_(copy_stochastic(res, rnd[0]))
-    exp_avg_sq.mul_(beta2).addcmul_(grad, grad.conj(), value=1 - beta2)
+    if cuda:   # CUDA addcmul is a + value * (b * c): g * g rounded alone, then one FMA (fp64 sum rounded to fp32)
+        v1, gf = exp_avg_sq.mul_(beta2).double(), grad.float()
+        value = float(torch.tensor(1 - beta2, dtype=torch.float32))
+        exp_avg_sq.copy_((v1 + value * (gf * gf).double()).float().to(torch.bfloat16))
+    else:
+        exp_avg_sq.mul_(beta2).addcmul_(grad, grad.conj(), value=1 - beta2)
     denom_correction = (1 - beta2 ** step) ** 0.5
     res = shift.to(torch.float32)
     if cuda:

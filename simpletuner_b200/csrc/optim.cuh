@@ -47,6 +47,8 @@ adamw_bf16_multi_kernel(const long long* __restrict__ ptrs, const long long* __r
   __nv_bfloat16* s = reinterpret_cast<__nv_bfloat16*>(ptrs[4 * T + t]);
   __nv_bfloat16* e = ema ? reinterpret_cast<__nv_bfloat16*>(ema[t]) : nullptr;
   const float dec = decay[t];
+  // per-tensor keys: t is the index within this launch, so the host gives every launch of one step its own seed
+  // (training/optim.py launch_seed: optimizer seed, step, `only=` chunk salt and param-group ordinal)
   const uint32_t key0 = hash_u32(seed ^ (uint64_t(uint32_t(t)) << 40)), key1 = hash_u32((seed + 0x632BE59BD9B4E019ull) ^ (uint64_t(uint32_t(t)) << 17));
   const long long roff = rnd_off ? rnd_off[t] : 0;
   // one element of the update, shared by the vector and the scalar path
@@ -61,7 +63,7 @@ adamw_bf16_multi_kernel(const long long* __restrict__ ptrs, const long long* __r
       r0 = uint32_t(rnd[0 * rnd_plane + roff + i]), r1 = uint32_t(rnd[1 * rnd_plane + roff + i]);
       r2 = uint32_t(rnd[2 * rnd_plane + roff + i]), r3 = uint32_t(rnd[3 * rnd_plane + roff + i]);
     } else {
-      // two murmur3 finalisers over a Weyl-sequenced element counter, keyed per (seed, step, tensor): 64 random bits for
+      // two murmur3 finalisers over a Weyl-sequenced element counter, keyed per (launch seed, tensor): 64 random bits for
       // ~14 integer instructions (the splitmix64 pair this replaces made the kernel instruction-bound, 3.2 TB/s)
       const uint32_t c = uint32_t(i) * 0x9E3779B1u + uint32_t(uint64_t(i) >> 32) * 0x7FEB352Du;
       const uint32_t h0 = mix32(c ^ key0), h1 = mix32(c + key1);
@@ -70,9 +72,11 @@ adamw_bf16_multi_kernel(const long long* __restrict__ ptrs, const long long* __r
     // exp_avg.mul_(beta1); add_stochastic_(exp_avg, grad, alpha = 1 - beta1)  ->  grad + alpha * exp_avg
     const float m1 = bf16r(mv * beta1);
     const float m2 = stochastic_bf16(fmaf(alpha1, m1, gv), r0);
-    // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value = 1 - beta2)
+    // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value = 1 - beta2): torch's CUDA addcmul is a + value * (b * c), so
+    // g * g is rounded on its own (exact unless it under- or overflows) and then one FMA (the CPU kernel's (value * b) * c
+    // differs in about 6 of 10^4 elements and makes g^2 = inf only where (value * g) * g overflows)
     const float v1 = bf16r(vv * beta2);
-    const float v2 = bf16r(fmaf(__fmul_rn(alpha2, gv), gv, v1));
+    const float v2 = bf16r(fmaf(alpha2, __fmul_rn(gv, gv), v1));
     // addcdiv_stochastic_(shift, exp_avg, sqrt(exp_avg_sq) + eps, value = -lr * sqrt(1 - beta2^step))
     const float den = bf16r(bf16r(sqrtf(v2)) + eps);
     const float s1 = stochastic_bf16(fmaf(value, __fdiv_rn(m2, den), sv), r1);

@@ -6,7 +6,7 @@ decay (`decay_threshold = 5e-3`, random starting phase per tensor) and `step(zer
 runs ~25 eager kernels per parameter tensor per step (13k launches for the 532 Flux LoRA matrices); here the whole step is
 ONE `stb_adamw_bf16_multi` launch over a pointer table.  Arithmetic follows the reference's CUDA path rounding for
 rounding (oracle/adamw_bf16_oracle.py, scalar_semantics="cuda"); the stochastic-rounding integers come from a
-counter-based generator keyed by (seed, step, tensor, element) instead of `torch.randint_like` per call, i.e. the same
+counter-based generator keyed by (seed, step, chunk salt, param group, tensor, element) instead of `torch.randint_like` per call, i.e. the same
 distribution but not the same Philox stream.  bf16 CUDA parameters only; there is no CPU fallback.
 """
 from __future__ import annotations
@@ -19,6 +19,13 @@ from torch.optim.optimizer import Optimizer
 
 from .. import _lib
 from ..ops import _stream, check
+
+
+def launch_seed(seed: int, step: int, salt: int = 0, group: int = 0) -> int:
+    """The 64-bit seed of one optimizer launch.  The kernel keys tensor t by its index within the launch, so every launch
+    of one step (each `only=` chunk, each param group) needs its own seed: `salt` numbers the chunks and `group` is the
+    param group's ordinal, whose term is zero for group 0 (a single-group run keeps its rounding stream)."""
+    return (seed * 0x9E3779B1 + step * 0x85EBCA77 + salt * 0xC2B2AE3D27D4EB4F + group * 0xD6E8FEB86659FD93) & 0xFFFFFFFFFFFFFFFF
 
 
 def build_block_map(sizes: List[int], chunk: int) -> Tuple[List[int], List[int]]:
@@ -93,7 +100,7 @@ class AdamWBF16(Optimizer):
             grad_clamp = None
         ema_decay = ema.begin_step(ema_global_step) if ema is not None else None
         ema_done = ema is None or ema_decay is None
-        for group in self.param_groups:
+        for gi, group in enumerate(self.param_groups):
             beta1, beta2 = group["betas"]
             ps = [p for p in group["params"] if p.grad is not None and (only_ids is None or id(p) in only_ids)]
             if not ps:
@@ -152,7 +159,7 @@ class AdamWBF16(Optimizer):
             if _rnd is not None:
                 assert _rnd.dtype == torch.int32 and _rnd.is_cuda and _rnd.is_contiguous() and _rnd.shape == (4, pl["total"])
                 rnd_ptr, rnd_plane = _rnd.data_ptr(), pl["total"]
-            seed = (self._seed * 0x9E3779B1 + int(stepf) * 0x85EBCA77 + int(salt) * 0xC2B2AE3D27D4EB4F) & 0xFFFFFFFFFFFFFFFF
+            seed = launch_seed(self._seed, int(stepf), int(salt), gi)
             check(_lib.lib().stb_adamw_bf16_multi(
                 pl["ptrs"].data_ptr(), pl["sizes"].data_ptr(), pl["decay"].data_ptr(), pl["blk_tensor"].data_ptr(),
                 pl["blk_off"].data_ptr(), pl["num_blocks"], pl["T"], float(beta1), float(beta2), stepf, float(lr),

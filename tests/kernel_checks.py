@@ -2379,3 +2379,312 @@ for _m in (1, 3, 8):
                                                  window=_p == 0.1)
 CHECKS["dropout_m3_k8_window"] = _case(check_dropout, members=3, B=3, S=33, K=8, p=0.5, window=True, seed=99, stream0=0xFFFFFFFE)
 CHECKS["dropout_m3_flux_3072"] = _case(check_dropout, members=3, B=1, S=4608, K=3072, p=0.1, seed=5, stream0=3)
+
+
+# --------------------------------------------------------------------------------------------- AdamW-bf16 reference model
+# stb_adamw_bf16_multi runs through AdamWBF16.step, its production path, and is compared bit for bit with the reference's
+# own eager op chain on copies of the same CUDA tensors: clip_grad_value_ when a clamp is set, the oracle's
+# adamw_bf16_step with scalar_semantics="cpu" (the op sequence of the reference's `_make_step`, pinned to it by
+# tests/golden/adamw_bf16_golden.pt; on CUDA tensors it runs torch's CUDA kernels, so it rounds as the reference does on
+# a GPU), then EMAModel.step.  The stochastic-rounding integers of the production path are replayed in numpy
+# (adamw_rnd_np: the two hash_u32 keys per tensor, the Weyl counter with its high-32-bit term, the two mix32 and the
+# halving into r0..r3) from the launch seed, restated here (adamw_seed) rather than imported, so a change to the
+# generator or to the seed formula fails.  p, exp_avg, exp_avg_sq, shift and the EMA shadows must hold the same bits;
+# any NaN matches any NaN (__float2bfloat16 and torch's cast give different payloads).  Each tensor lives in one flat
+# buffer per role, at a 16-byte boundary or, where the case asks, 2 bytes past it (the kernel's scalar path); the rest of
+# every buffer must stay unchanged.  Every case starts from random, non-zero exp_avg / exp_avg_sq / shift.
+# A NaN reaching a stochastic rounding becomes -0.0: fp32 arithmetic gives the NaN 0x7FFFFFFF, adding a nonzero 16-bit
+# integer wraps it to 0x8000xxxx and the mask leaves 0x80000000 (only r = 0 keeps the NaN).  The reference's
+# copy_stochastic_ does the same integer arithmetic, so it is matched, not changed; n_nan_neg0 counts the exp_avg
+# elements of a NaN gradient that came out -0.
+_M64 = 0xFFFFFFFFFFFFFFFF
+ADAMW_ROLES = ("p", "g", "m", "v", "s", "e")       # param, grad, exp_avg, exp_avg_sq, shift, EMA shadow
+BF16_MAX = 3.3895313892515355e38
+
+
+def adamw_seed(seed, step, salt=0, group=0):
+    """training/optim.py launch_seed, restated: the 64-bit seed of the launch of `group` / chunk `salt` at `step`."""
+    return (seed * 0x9E3779B1 + int(step) * 0x85EBCA77 + salt * 0xC2B2AE3D27D4EB4F + group * 0xD6E8FEB86659FD93) & _M64
+
+
+def hash_u32_py(x):
+    """optim.cuh hash_u32 (splitmix64 finaliser, upper 32 bits) on a Python int."""
+    x = (x + 0x9E3779B97F4A7C15) & _M64
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & _M64
+    return (x ^ (x >> 31)) >> 32
+
+
+def adamw_keys(seed64, t):
+    """(key0, key1) of launch tensor t."""
+    t = t & 0xFFFFFFFF
+    return hash_u32_py(seed64 ^ ((t << 40) & _M64)), hash_u32_py(((seed64 + 0x632BE59BD9B4E019) & _M64) ^ (t << 17))
+
+
+def adamw_rnd_np(seed64, t, n, first=0):
+    """The integers optim.cuh draws for elements first .. first + n - 1 of launch tensor t: int32 [4, n] (r0..r3)."""
+    import numpy as np
+    k0, k1 = adamw_keys(seed64, t)
+    i = np.arange(first, first + n, dtype=np.uint64)
+    lo, hi = (i & np.uint64(0xFFFFFFFF)).astype(np.uint32), (i >> np.uint64(32)).astype(np.uint32)
+    c = lo * np.uint32(0x9E3779B1) + hi * np.uint32(0x7FEB352D)
+    h0, h1 = mix32_np(c ^ np.uint32(k0)), mix32_np(c + np.uint32(k1))
+    low, sh = np.uint32(0xFFFF), np.uint32(16)
+    return np.stack([h0 & low, h0 >> sh, h1 & low, h1 >> sh]).astype(np.int32)
+
+
+def _adamw_edges(n, seed):
+    """Gradient / state overrides by element class i % 16 (sign alternating every 16 elements): zero and -0 gradients
+    with zero moments (0 / 0 at eps 0), |g| = 2^-60 / 2^-65 (alpha2 g^2 a subnormal), 2^-70 / 2^-100 (underflow), 2^64 /
+    2^100 (exp_avg_sq overflows), +-inf, NaN, +-0.36 / +-0.38 (inside / outside a 0.37 clamp), p at +bf16 max and near
+    -bf16 max with a shift that can round it to inf, and subnormal moments."""
+    i = torch.arange(n)
+    cls, sgn = i % 16, torch.where((i // 16) % 2 == 0, 1.0, -1.0)
+    g = torch.full((n,), math.nan)
+    for c, val in ((2, 2.0 ** -60), (3, 2.0 ** -65), (4, 2.0 ** -70), (5, 2.0 ** -100), (6, 2.0 ** 64), (7, 2.0 ** 100),
+                   (11, 0.36), (12, 0.38), (15, 2.0 ** -65)):
+        g = torch.where(cls == c, sgn * val, g)
+    g = torch.where(cls == 0, 0.0, torch.where(cls == 1, -0.0, g))
+    g = torch.where(cls == 8, math.inf, torch.where(cls == 9, -math.inf, g))
+    rest = (cls == 13) | (cls == 14)
+    g = torch.where(rest, torch.randn(n, generator=torch.Generator().manual_seed(seed)) * 0.02, g)
+    near_max = -torch.tensor([0x7F7D], dtype=torch.int16).view(torch.bfloat16).float()
+    p = {13: BF16_MAX, 14: float(near_max)}
+    s = {13: 2.0 ** 119, 14: -(2.0 ** 120)}
+    return cls, g, p, s
+
+
+def _adamw_values(kind, sizes, steps, seed):
+    """CPU bf16 starting values {role: [tensor per size]} and gradients init["g"][step][tensor]."""
+    gen = torch.Generator().manual_seed(seed)
+    rn = lambda n, s: torch.randn(n, generator=gen) * s
+    init = {r: [] for r in ADAMW_ROLES if r != "g"}
+    init["g"] = [[] for _ in range(steps)]
+    for t, n in enumerate(sizes):
+        p, m, v, s = rn(n, 0.05), rn(n, 0.01), rn(n, 0.02) ** 2 * 0.05, rn(n, 1e-4)
+        e = p + rn(n, 1e-3)
+        gs = [rn(n, 0.02) for _ in range(steps)]
+        if kind == "edges":
+            cls, g_e, p_e, s_e = _adamw_edges(n, seed + t)
+            gs = [torch.where(torch.isnan(g_e) & ~((cls == 10)), g, g_e) for g in gs]
+            zero = (cls == 0) | (cls == 1)
+            m, v = torch.where(zero, 0.0, m), torch.where(zero, 0.0, v)
+            m, v = torch.where(cls == 15, 2.0 ** -130, m), torch.where(cls == 15, 2.0 ** -130, v)
+            for c in p_e:
+                p, s, e = torch.where(cls == c, p_e[c], p), torch.where(cls == c, s_e[c], s), torch.where(cls == c, p_e[c], e)
+        for r, x in zip("pmvse", (p, m, v, s, e)):
+            init[r].append(x.bfloat16())
+        for k in range(steps):
+            init["g"][k].append(gs[k].bfloat16())
+    return init
+
+
+def _adamw_place(vals, shifted, seed):
+    """One flat CUDA bf16 buffer holding vals[u] at a 16-byte boundary, or 2 bytes past it where shifted[u], with 8 spare
+    elements after each.  Returns (views, buffer, mask of the spare elements); the spare elements hold random values."""
+    starts, pos = [], 0
+    for x, sh in zip(vals, shifted):
+        pos = _pad8(pos) + (1 if sh else 0)
+        starts.append(pos)
+        pos += x.numel() + 8
+    buf = _rand(pos, seed=seed)
+    halo = torch.ones(pos, dtype=torch.bool, device=DEV)
+    views = []
+    for x, a in zip(vals, starts):
+        halo[a:a + x.numel()] = False
+        views.append(buf[a:a + x.numel()])
+        views[-1].copy_(x.to(DEV))
+    return views, buf, halo
+
+
+def _cat_bits(xs):
+    return torch.cat([x.detach().reshape(-1) for x in xs])
+
+
+def check_adamw(name, sizes, *, steps=2, step0=0, beta1=0.9, beta2=0.999, eps=1e-8, lr=1e-4, clamp=None, ema=None,
+                shifted=(), mixed=False, values="normal", decays=None, wd_lr=2e-3, chunks=1, groups=1, golden=False,
+                repeat=False, seed=11):
+    """AdamWBF16.step against the reference chain, bit for bit (above).
+    sizes: the tensors of one param group.  groups=2: a second group holding identical copies (same values, same
+    gradients): each group must match its own replay, and after the first step the number of exp_avg elements that
+    differ between the groups must be within 6 sigma of what independent streams give (sum of 2 q (1 - q), q the
+    rounding-up probability of each element's fp32 value), which is far from 0.  chunks: each step is `chunks` calls
+    with `only=` a contiguous slice of the tensors and salt 0, 1, ...  decays: per tensor, whether accumulated_decay is
+    preset so that the tensor's delayed weight decay fires on the first step (weight_decay * lr = wd_lr, 2e-3 by default:
+    the others fire later; above 5e-3 every tensor decays on every step).  ema: 1 - decay of a fused EMA update (shadows in their own buffer).  shifted: roles placed 2 bytes past a
+    16-byte boundary (mixed: odd tensors only).  golden: p0, gradients and random integers of the CPU golden, through
+    `_rnd`.  repeat: the production path runs twice and must give the same bits."""
+    import numpy as np
+    from oracle import adamw_bf16_oracle as A
+    from simpletuner_b200.training.ema import EMAModel
+    from simpletuner_b200.training.optim import AdamWBF16
+
+    T = len(sizes)
+    init = _adamw_values(values, sizes, steps, seed)
+    golden_rnd = None
+    if golden:
+        from pathlib import Path
+        G = torch.load(Path(__file__).parent / "golden" / "adamw_bf16_golden.pt")
+        assert sum(sizes) == G["p0"].numel() and groups == 1 and chunks == 1
+        cuts = [0] + list(np.cumsum(sizes))
+        flat = G["p0"].flatten()
+        init["p"] = [flat[a:b].clone() for a, b in zip(cuts[:-1], cuts[1:])]
+        steps = len(G["decays"])
+        init["g"] = [[G[f"step{k}.grad"].flatten()[a:b].clone() for a, b in zip(cuts[:-1], cuts[1:])] for k in range(steps)]
+        golden_rnd = [G[f"step{k}.rnd"].reshape(4, -1).to(DEV).contiguous() for k in range(steps)]
+        hp = G["hp"]
+        beta1, beta2, eps, lr = hp["beta1"], hp["beta2"], hp["eps"], hp["lr"]
+    U = groups * T
+    vals = {r: [init[r][u % T] for u in range(U)] for r in "pmvse"}
+    grads = [[init["g"][k][u % T] for u in range(U)] for k in range(steps)]
+    wd = 0.0 if decays is None else wd_lr / lr
+    acc0 = [4e-3 if decays is not None and decays[u % T] else 0.0 for u in range(U)]
+    chunk_ts = [list(c) for c in np.array_split(np.arange(T), chunks)]
+    moved = lambda role, u: role in shifted and (not mixed or u % 2 == 1)
+
+    def production():
+        views, bufs = {}, {}
+        for k, r in enumerate(ADAMW_ROLES):
+            src = vals[r] if r != "g" else grads[0]
+            views[r], buf, halo = _adamw_place(src, [moved(r, u) for u in range(U)], seed=900 + k)
+            bufs[r] = (buf, halo, buf[halo].clone())
+        params = [torch.nn.Parameter(x) for x in views["p"]]
+        opt = AdamWBF16([{"params": params[gi * T:(gi + 1) * T]} for gi in range(groups)], lr=lr, betas=(beta1, beta2),
+                        eps=eps, weight_decay=wd, seed=seed)
+        for u, p_ in enumerate(params):
+            opt.state[p_].update(step=float(step0), exp_avg=views["m"][u], exp_avg_sq=views["v"][u], shift=views["s"][u],
+                                 accumulated_decay=acc0[u])
+            p_.grad = views["g"][u]
+        em = None
+        if ema is not None:
+            em = EMAModel(params, decay=1.0 - ema, warmup_steps=1)
+            em.shadow_params = list(views["e"])
+        return {"views": views, "bufs": bufs, "params": params, "opt": opt, "ema": em}
+
+    def prod_step(run, k):
+        for u in range(U):
+            run["views"]["g"][u].copy_(grads[k][u].to(DEV))
+        for c, ts in enumerate(chunk_ts):
+            only = None if chunks == 1 else [run["params"][gi * T + t] for gi in range(groups) for t in ts]
+            run["opt"].step(_rnd=golden_rnd[k] if golden else None, grad_clamp=clamp, ema=run["ema"], only=only, salt=c)
+
+    runs = [production() for _ in range(2 if repeat else 1)]
+    rp = [torch.nn.Parameter(x.to(DEV, copy=True)) for x in vals["p"]]
+    rs, rm, rv = ([x.to(DEV, copy=True) for x in vals[r]] for r in "smv")
+    r_ema = EMAModel(rp, decay=1.0 - ema, warmup_steps=1) if ema is not None else None
+    if r_ema is not None:
+        r_ema.shadow_params = [x.to(DEV, copy=True) for x in vals["e"]]
+    acc = list(acc0)
+    offs = [0] + list(np.cumsum(sizes))
+    parts, counts = [], {"n_scalar": 0, "n_nan_neg0": 0, "n_decayed": 0, "n_inf": 0}
+    extra = {}
+    for k in range(steps):
+        for run in runs:
+            prod_step(run, k)
+        stepk = step0 + k + 1
+        with torch.no_grad():
+            for u in range(U):
+                rp[u].grad = grads[k][u].to(DEV, copy=True)
+            if clamp is not None:
+                torch.nn.utils.clip_grad_value_(rp, clamp)
+            for gi in range(groups):
+                for c, ts in enumerate(chunk_ts):
+                    seed64 = adamw_seed(seed, stepk, c, gi)
+                    for j, t in enumerate(ts):
+                        u, n = gi * T + t, sizes[t]
+                        dec, acc[u] = A.decay_schedule(acc[u], wd, lr)
+                        if golden:
+                            rnd = golden_rnd[k][:, offs[t]:offs[t] + n]
+                        else:
+                            rnd = torch.from_numpy(adamw_rnd_np(seed64, j, n)).to(DEV)
+                        if k == 0 and groups == 2 and gi == 1 and c == 0 and j == 0:
+                            extra.update(_adamw_group_stats(rp, rm, T, beta1, chunk_ts))
+                        A.adamw_bf16_step(rp[u], rp[u].grad, rs[u], rm[u], rv[u], beta1=beta1, beta2=beta2, step=float(stepk),
+                                          lr=lr, eps=eps, decay_this_iteration=dec, rnd=list(rnd), scalar_semantics="cpu")
+                        counts["n_scalar"] += n if any(moved(r, u) for r in ADAMW_ROLES if r != "e" or ema is not None) \
+                            else n % 8
+                        counts["n_decayed"] += n if dec > 0 else 0
+                        counts["n_nan_neg0"] += int((torch.isnan(rp[u].grad) & (rm[u].view(torch.int16) == -32768)).sum())
+            if r_ema is not None:
+                r_ema.step(rp)
+        torch.cuda.synchronize()
+        counts["n_inf"] += sum(int(torch.isinf(x).sum()) for xs in (rp, rm, rv, rs) for x in xs)
+        run = runs[0]
+        want = {"p": rp, "m": rm, "v": rv, "s": rs, "e": r_ema.shadow_params if r_ema is not None else None}
+        for r in "pmvse":
+            if want[r] is not None:
+                parts.append(_bits(f"{r}_step{k}", _cat_bits(run["views"][r]), _cat_bits(want[r])))
+        if repeat:
+            extra["repeatable"] = extra.get("repeatable", True) and all(
+                torch.equal(_cat_bits(runs[0]["views"][r]).view(torch.int16), _cat_bits(runs[1]["views"][r]).view(torch.int16))
+                for r in "pmvse")
+        if k == 0 and groups == 2:
+            mg = _cat_bits(run["views"]["m"]).view(torch.int16)
+            half = mg.numel() // 2
+            extra["groups_n_diff"] = int((mg[:half] != mg[half:]).sum())
+            lo, hi = extra["groups_expect"] - 6 * extra["groups_sigma"], extra["groups_expect"] + 6 * extra["groups_sigma"]
+            extra["groups_independent"] = bool(lo <= extra["groups_n_diff"] <= hi and extra["groups_expect"] > 100)
+    for run in runs:
+        extra["halo_clean"] = extra.get("halo_clean", True) and all(torch.equal(b[halo], b0) for b, halo, b0 in run["bufs"].values())
+        if run["ema"] is not None:
+            extra["ema_decay_used"] = run["ema"].cur_decay_value
+    return _combine(name, parts, **extra, **counts, numel=groups * sum(sizes))
+
+
+def _adamw_group_stats(rp, rm, T, beta1, chunk_ts):
+    """Expected number (and sigma) of group 0 / group 1 exp_avg elements that differ after the first step if the two
+    groups' streams are independent: the fp32 value before the exp_avg rounding is grad + (1 - beta1) bf16(beta1 m),
+    the same in both groups (identical copies, group 0 not yet stepped in rm for group 1's tensors); it rounds up with
+    probability q = low 16 bits / 2^16, and two independent draws differ with probability 2 q (1 - q)."""
+    q = []
+    for t in range(T):
+        u = T + t
+        res = rp[u].grad.float().add_(rm[u].mul(beta1), alpha=1 - beta1)
+        low = (res.view(torch.int32) & 0xFFFF).double() / 65536.0
+        q.append(torch.where(torch.isfinite(res), low, torch.zeros_like(low)))
+    q = torch.cat(q)
+    pd = 2 * q * (1 - q)
+    return {"groups_expect": float(pd.sum()), "groups_sigma": float((pd * (1 - pd)).sum().sqrt())}
+
+
+# AdamW-bf16: the CPU golden's integers through `_rnd`; sizes around the vector width and the 2048-element block (one
+# launch), and a Flux-LoRA-sized launch (532 tensors, 26M elements) at beta2 0.95 where most tensors decay; every role
+# 2 bytes off a 16-byte boundary in turn, all at once and mixed with aligned tensors; edge values with and without the
+# clamp, at eps 0 and at beta1 = beta2 = 0; beta1 x beta2 x eps x step x lr; per-tensor decay; the fused EMA at
+# 1 - decay of 0, 0.03 and 1; three `only=` chunks; two identical param groups; the same seed twice
+_ADAMW_SIZES = [2049, 8, 333, 4096 + 5]
+CHECKS["adamw_golden_rnd"] = _case(check_adamw, "adamw_golden_rnd", [1000, 1, 3999, 3481], golden=True,
+                                   decays=[True, False, True, False])
+CHECKS["adamw_sizes"] = _case(check_adamw, "adamw_sizes", [1, 7, 8, 9, 2047, 2048, 2049, 8 * 2048 + 3],
+                              decays=[t % 2 == 1 for t in range(8)])
+CHECKS["adamw_flux_lora_532"] = _case(check_adamw, "adamw_flux_lora_532", [3072 * 16 + t % 3 for t in range(532)],
+                                      beta2=0.95, decays=[t % 5 != 0 for t in range(532)], seed=3)
+for _r in ADAMW_ROLES:
+    CHECKS[f"adamw_offset_{_r}"] = _case(check_adamw, f"adamw_offset_{_r}", _ADAMW_SIZES, shifted=(_r,), ema=0.03)
+CHECKS["adamw_offset_all"] = _case(check_adamw, "adamw_offset_all", _ADAMW_SIZES, shifted=ADAMW_ROLES, ema=0.03)
+CHECKS["adamw_offset_mixed"] = _case(check_adamw, "adamw_offset_mixed", _ADAMW_SIZES * 2, shifted=ADAMW_ROLES, mixed=True,
+                                     ema=0.03, decays=[t % 3 == 0 for t in range(8)])
+_EDGE_SIZES = [16 * 130, 16 * 7 + 5, 4096]
+for _nm, _kw in (("plain", {}), ("clamp", dict(clamp=0.37)), ("eps0", dict(eps=0.0)),
+                 ("clamp_eps0_offset", dict(clamp=0.37, eps=0.0, shifted=ADAMW_ROLES)), ("beta0", dict(beta1=0.0, beta2=0.0)),
+                 ("lr1_step1e6", dict(lr=1.0, step0=10 ** 6 - 1)), ("offset_ema", dict(shifted=ADAMW_ROLES, ema=0.03))):
+    CHECKS[f"adamw_edges_{_nm}"] = _case(check_adamw, f"adamw_edges_{_nm}", _EDGE_SIZES, values="edges", steps=3, **_kw)
+for _i, (_b2, _st) in enumerate((_b2, _st) for _b2 in (0.0, 0.95, 0.999, 0.9999) for _st in (1, 2, 1000, 10 ** 6)):
+    _b1, _eps, _lr = (0.0, 0.9)[_i % 2], (0.0, 1e-8, 1e-6)[_i % 3], (1e-4, 1.0)[(_i // 2) % 2]
+    _nm = f"adamw_hp_b1_{_b1:g}_b2_{_b2:g}_eps{_eps:g}_step{_st}_lr{_lr:g}"
+    CHECKS[_nm] = _case(check_adamw, _nm, _ADAMW_SIZES, beta1=_b1, beta2=_b2, eps=_eps, lr=_lr, step0=_st - 1,
+                        decays=[True, False, False, True])
+CHECKS["adamw_decay_per_tensor"] = _case(check_adamw, "adamw_decay_per_tensor", [3000, 2048, 7, 5000, 64],
+                                         decays=[False, True, True, False, True], steps=3, lr=1e-3)
+# every tensor decays on every step, by about 1/3 (a decay far above the default 5e-3 threshold's)
+CHECKS["adamw_decay_third_every_step"] = _case(check_adamw, "adamw_decay_third_every_step", [(1 << 20) + 3, 4099],
+                                               decays=[True, False], wd_lr=1 / 3, steps=3, lr=1e-3)
+for _a in (0.0, 0.03, 1.0):
+    CHECKS[f"adamw_ema_{_a:g}"] = _case(check_adamw, f"adamw_ema_{_a:g}", _ADAMW_SIZES, ema=_a, shifted=("e",), mixed=True)
+CHECKS["adamw_chunks3_clamp"] = _case(check_adamw, "adamw_chunks3_clamp", [2049, 8, 333, 4101, 1, 9000, 64], chunks=3,
+                                      clamp=0.03, decays=[t % 2 == 0 for t in range(7)])
+CHECKS["adamw_two_groups"] = _case(check_adamw, "adamw_two_groups", [4096, 2049, 20000, 7], groups=2, steps=1)
+CHECKS["adamw_two_groups_chunks3"] = _case(check_adamw, "adamw_two_groups_chunks3", [4096, 2049, 20000, 7, 333], groups=2,
+                                           chunks=3, steps=1)
+CHECKS["adamw_repeat_offset_mixed"] = _case(check_adamw, "adamw_repeat_offset_mixed", _ADAMW_SIZES * 3, shifted=ADAMW_ROLES,
+                                            mixed=True, repeat=True, ema=0.03, steps=3)

@@ -34,7 +34,7 @@ def test_library_exports_every_declared_symbol():
 _BOOKKEEPING = {"stb_version", "stb_last_error", "stb_launch_count", "stb_reset_launch_count", "stb_skinny_tn_workspace",
                 "stb_adamw_bf16_chunk"}
 # GPU tests outside the kernel_checks registry that compare a wrapper with a reference
-_GPU_TEST_FILES = ("test_adamw_bf16.py", "test_lora_dropout_gpu.py", "test_text_encoders.py")
+_GPU_TEST_FILES = ("test_lora_dropout_gpu.py", "test_text_encoders.py")
 
 
 def _wrappers():
