@@ -18,9 +18,11 @@ Gradient checkpointing with an interval is the way to trade this memory for comp
 The hidden state travels as ONE joint buffer [B, S_txt + S_img, D] (text tokens first, as the
 reference concatenates them for attention, :166-168) so no torch.cat / split copies are needed.
 
-Base weights are frozen (LoRA training, BASELINE config 2): gradients are produced for the LoRA
+In LoRA training (BASELINE config 2) the base weights are frozen: gradients are produced for the LoRA
 A/B matrices and for the hidden state only; no gradient flows to temb / the adaLN linears because
-none of their parameters is trainable in that configuration (full fine-tune is a later row).
+none of their parameters is trainable in that configuration.  Full fine-tune (`st["full"]`, SD3 and PixArt) runs the
+same schedules with each Linear's (weight, bias) in its adapter slots (WgradPack) and also returns the modulation
+gradients.
 """
 from __future__ import annotations
 
@@ -132,34 +134,48 @@ def pack_lora(params: List[Optional[Tuple[torch.Tensor, torch.Tensor]]], n_out: 
 
 
 @dataclass
-class LokrPack:
-    """LyCORIS LoKr members of one fused projection group (simpletuner_b200/lycoris.py).  The adapted weights are already
-    inside the plan's projection matrices, so forward / dgrad are adapter-free; only the factor gradients need the pack."""
-    members: List[Optional[Tuple[torch.Tensor, torch.Tensor, float]]]   # (w1 [a, c], w2 [b, d], scale * multiplier)
-    n_out: int
-    k_in: int
+class WgradPack:
+    """Members of one fused projection group whose gradients come from the group's full weight gradient dW = dy^T x: LyCORIS
+    LoKr factor pairs (simpletuner_b200/lycoris.py) or, in full fine-tune, the member's own (weight, bias).  Either way the
+    weights the GEMMs read are already the plan's projection matrices, so forward / dgrad are adapter-free."""
+    members: List[Optional[tuple]]   # LoKr: (w1 [a, c], w2 [b, d], scale * multiplier); full: (weight, bias)
+    n_out: int                       # rows per member
+    full: bool = False
+    row_index: Optional[torch.Tensor] = None  # as LoraPack: member-local output row -> row of the (head-dim padded) projection
+    col_index: Optional[torch.Tensor] = None  # input feature -> column of the (head-dim padded) activation
 
 
-def make_pack(params, n_out: int, k_in: int, scaling: float, device, lokr_scales=None, **kw):
-    """LoRA pack (pack_lora) or, when `lokr_scales[m]` is set for the present members, a LokrPack."""
-    if lokr_scales is not None and any(s is not None for s in lokr_scales):
-        mem = [None if p is None else (p[0], p[1], float(sc)) for p, sc in zip(params, lokr_scales)]
-        return LokrPack(mem, n_out, k_in) if any(m is not None for m in mem) else None
-    return pack_lora(params, n_out, k_in, scaling, device, **kw)
+def make_pack(params, n_out: int, k_in: int, scaling: float, device, lokr_scales=None, full: bool = False,
+              row_index: Optional[torch.Tensor] = None, col_index: Optional[torch.Tensor] = None):
+    """LoRA pack (pack_lora) or a WgradPack: of LoKr factors when `lokr_scales[m]` is set for the present members, of
+    (weight, bias) pairs when `full`."""
+    if full or (lokr_scales is not None and any(s is not None for s in lokr_scales)):
+        mem = list(params) if full else [None if p is None else (p[0], p[1], float(sc)) for p, sc in zip(params, lokr_scales)]
+        return WgradPack(mem, n_out, full, row_index, col_index) if any(m is not None for m in mem) else None
+    return pack_lora(params, n_out, k_in, scaling, device, row_index=row_index, col_index=col_index)
 
 
-def _lokr_grads(pack: LokrPack, x: torch.Tensor, dy: torch.Tensor):
-    """Factor gradients through delta W = kron(w1, w2) * scale: the full weight gradient of the group (one MN-major wgmma
-    GEMM, dy^T x), contracted per member against the other Kronecker factor."""
+def _wgrad_grads(pack: WgradPack, x: torch.Tensor, dy: torch.Tensor):
+    """The full weight gradient of the group (one MN-major wgmma GEMM, dy^T x), split per member: a full member takes its
+    rows of dW and of the bias gradient (gathered back to the real rows / columns of padded heads), a LoKr member contracts
+    its rows against the other Kronecker factor (delta W = kron(w1, w2) * scale)."""
     from ..lycoris import lokr_factor_grads
     dW = ops.wgrad_full(dy, x)                       # [members * n_out, K] bf16
+    db = ops.colsum2(dy)[0].sum(0).to(torch.bfloat16) if pack.full else None
     out = []
     for m, mem in enumerate(pack.members):
+        rows = slice(m * pack.n_out, (m + 1) * pack.n_out)
         if mem is None:
             out.append((None, None))
-            continue
-        w1, w2, sc = mem
-        out.append(lokr_factor_grads(dW[m * pack.n_out:(m + 1) * pack.n_out], w1, w2, sc))
+        elif not pack.full:
+            out.append(lokr_factor_grads(dW[rows], *mem))
+        else:
+            dw, dbm = dW[rows], db[rows]
+            if pack.row_index is not None:
+                dw, dbm = dw.index_select(0, pack.row_index), dbm.index_select(0, pack.row_index)
+            if pack.col_index is not None:
+                dw = dw.index_select(1, pack.col_index)
+            out.append((dw, dbm))
     return out
 
 
@@ -196,9 +212,9 @@ def _lora_grads(pack: LoraPack, x: torch.Tensor, t_down: torch.Tensor, dy: torch
                 drop: Optional[LoraDrop] = None):
     """dA_stack [R, K] = T'^T x  (T' = dy B_ext, scaling already inside);  dB_ext^T [R, N] = T^T dy.
     With dropout dA_m contracts T'_m with the SAME masked copy of x the forward used (masks regenerated, not stored)."""
-    if isinstance(pack, LokrPack):
+    if isinstance(pack, WgradPack):
         assert drop is None and not isinstance(x, (tuple, list))
-        return _lokr_grads(pack, x, dy)
+        return _wgrad_grads(pack, x, dy)
     R = pack.a_stack.shape[0]
     wide = R > 128        # ranks above 40: the fused q|k|v rank block no longer fits one 128-wide weight-gradient tile
     if isinstance(x, (tuple, list)):        # the adapted Linear reads cat(x, -1) (single-block proj_out): one product per part
@@ -259,7 +275,7 @@ def _lora_dgrad_dropout(dx: torch.Tensor, t_up: torch.Tensor, pack: LoraPack, dr
 # ------------------------------------------------------------------------------------------------
 def _linear_lora_fwd(x, w, b, pack: Optional[LoraPack], drop: Optional[LoraDrop] = None, **kw):
     """y = x W^T + b (+ T B_ext^T as an extra K-segment).  Returns (y, T or None)."""
-    if pack is None or isinstance(pack, LokrPack):
+    if pack is None or isinstance(pack, WgradPack):
         return ops.gemm([x], [w], b, **kw), None
     t = _lora_down(x, pack, drop)
     return ops.gemm([x, t], [w, pack.b_ext], b, **kw), t
@@ -267,7 +283,7 @@ def _linear_lora_fwd(x, w, b, pack: Optional[LoraPack], drop: Optional[LoraDrop]
 
 def _linear_lora_dgrad(dy, w_t, pack: Optional[LoraPack], drop: Optional[LoraDrop] = None, **kw):
     """dx = dy W (+ (dy B_ext) A_stack).  Returns (dx, T' or None)."""
-    if pack is None or isinstance(pack, LokrPack):
+    if pack is None or isinstance(pack, WgradPack):
         return ops.gemm([dy], [w_t], None, **kw), None
     t_up = ops.gemm([dy], [pack.b_ext_t])
     if drop is None:
@@ -277,16 +293,16 @@ def _linear_lora_dgrad(dy, w_t, pack: Optional[LoraPack], drop: Optional[LoraDro
     return dx, t_up
 
 
-def _pack1(a, b, n_out: int, k_in: int, scaling: float, device, lokr_scale=None):
-    """Pack of a single adapted Linear (MLP projections, proj_out, x_embedder)."""
-    return None if a is None else make_pack([(a, b)], n_out, k_in, scaling, device, [lokr_scale])
+def _pack1(a, b, n_out: int, k_in: int, scaling: float, device, lokr_scale=None, full: bool = False):
+    """Pack of a single adapted Linear (MLP projections, proj_out, x_embedder); full: (a, b) = (weight, bias)."""
+    return None if a is None else make_pack([(a, b)], n_out, k_in, scaling, device, [lokr_scale], full)
 
 
 def _dgrad_through_gelu(dy, w_t, pack: Optional[LoraPack], drop: Optional[LoraDrop], pre):
     """d_pre = (dy W (+ LoRA branch)) * gelu'(pre).  Returns (d_pre, T' or None).  Without dropout the LoRA branch is one more
     K-segment and the activation gradient stays in the GEMM epilogue; with dropout the masked branch is added to the
     un-activated gradient first."""
-    if pack is None or drop is None or isinstance(pack, LokrPack):
+    if pack is None or drop is None or isinstance(pack, WgradPack):
         return _linear_lora_dgrad(dy, w_t, pack, None, epi=ops.EPI_MUL_DGELU, aux=pre)
     d_act, t_up = _linear_lora_dgrad(dy, w_t, pack, drop)
     return ops.mul_dgelu_tanh(d_act, pre, out=d_act), t_up
@@ -338,6 +354,20 @@ def _lnm_bwd(d, x, segs, isc: int, add=None, out=None):
     return out
 
 
+def _dmod_gate(dm, dy, y, ig: int):
+    """Full fine-tune: d gate (chunk ig of dm [B, kD] fp32) of out = res + gate * y, as sum_s dy * y."""
+    D = y.shape[2]
+    dm[:, ig * D:(ig + 1) * D] = ops.colsum2(dy, y, want_sum=False)[1]
+
+
+def _dmod_shift_scale(dm, d_nx, x, ish: int, isc: int):
+    """Full fine-tune: d shift / d scale (chunks ish / isc of dm) of nx = LayerNorm(x) (1 + scale) + shift, as sum_s d_nx and
+    sum_s d_nx * LayerNorm(x); LayerNorm(x) comes from the modulate kernel with zero shift / scale."""
+    B, _, D = x.shape
+    zero = torch.zeros((B, D), device=x.device, dtype=torch.bfloat16)
+    dm[:, ish * D:(ish + 1) * D], dm[:, isc * D:(isc + 1) * D] = ops.colsum2(d_nx, ops.ln_modulate_fwd(x, zero, zero, EPS))
+
+
 def _gate_mul(x, segs, ig: int):
     if len(segs) == 1:
         return ops.gate_mul(x, _chunk(segs[0][1], ig, x.shape[2]))
@@ -360,13 +390,15 @@ def _gemm_gate_res(a_list, w_list, bias, segs, ig: int, res, out=None, nan_to_nu
     return out
 
 
-def _linear_lora_gate_res(x, w, b, pack, drop, segs, ig: int, res, out, nan_to_num=False):
+def _linear_lora_gate_res(x, w, b, pack, drop, segs, ig: int, res, out, nan_to_num=False, aux=None):
     """_linear_lora_fwd with the GATE_RES epilogue over segments: the LoRA down-projection (and its dropout mask) spans
-    the whole stream, the base GEMM runs per segment.  Returns T or None."""
+    the whole stream, the base GEMM runs per segment.  aux (one segment only): receives the pre-gate output.  Returns T
+    or None."""
     if len(segs) == 1:
         return _linear_lora_fwd(x, w, b, pack, drop, out=out, epi=ops.EPI_GATE_RES, gate=_chunk(segs[0][1], ig, res.shape[2]),
-                                res=res, nan_to_num=nan_to_num)[1]
-    if pack is None or isinstance(pack, LokrPack):
+                                res=res, nan_to_num=nan_to_num, aux=aux)[1]
+    assert aux is None
+    if pack is None or isinstance(pack, WgradPack):
         _gemm_gate_res([x], [w], b, segs, ig, res, out, nan_to_num)
         return None
     t = _lora_down(x, pack, drop)
@@ -407,9 +439,11 @@ def _qk_fwd(qkv, D, H, hd, img_plan: AttnPlan, txt_plan: Optional[AttnPlan], S_t
     return ops.qk_rmsnorm_rope_fwd(qkv, D, H, hd, img_plan.norm_q, img_plan.norm_k, tq, tk, S_txt, cos, sin, EPS)
 
 
-def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, sin, qk=None, key_bias=None):
+def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, sin, qk=None, key_bias=None, dw=None):
     """Returns d_qkv [B, S, 3D] given d_o.  `qk` = the (q, k) pair saved by the forward (spending 2 B S D bytes per block
-    is cheaper than re-running the RMSNorm + RoPE pass in backward); recomputed when absent.  key_bias: the forward's."""
+    is cheaper than re-running the RMSNorm + RoPE pass in backward); recomputed when absent.  key_bias: the forward's.
+    dw (full fine-tune): zeroed fp32 [4, hd] that receives the RMSNorm weight gradients (norm_q, norm_k, the text
+    stream's norm_added_q, norm_added_k)."""
     B, S, _ = qkv.shape
     q, k = qk if qk is not None else _qk_fwd(qkv, D, H, hd, img_plan, txt_plan, S_txt, cos, sin)
     v = qkv[:, :, 2 * D:].unflatten(-1, (H, hd))
@@ -427,7 +461,8 @@ def _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, img_plan, txt_plan, S_txt, cos, s
     del q, k
     tq = txt_plan.norm_q if txt_plan is not None else None
     tk = txt_plan.norm_k if txt_plan is not None else None
-    ops.qk_rmsnorm_rope_bwd(dq, dk, qkv, D, H, hd, img_plan.norm_q, img_plan.norm_k, tq, tk, S_txt, cos, sin, EPS, dsrc=d_qkv)
+    ops.qk_rmsnorm_rope_bwd(dq, dk, qkv, D, H, hd, img_plan.norm_q, img_plan.norm_k, tq, tk, S_txt, cos, sin, EPS, dsrc=d_qkv,
+                            dw=dw)
     return d_qkv
 
 
@@ -441,14 +476,19 @@ class DoubleBlockFn(torch.autograd.Function):
     attention is permutation-invariant without RoPE, so the [image, text] order of JointAttnProcessor2_0 is
     irrelevant).  `st` flags: `nan_to_num_txt` (Flux), `dual` (SD3.5 image-only attn2 fed by a second
     modulation of LayerNorm(h): mod_img then has 9 chunks), `context_pre_only` (SD3 last block: the text
-    stream only feeds q/k/v; mod_txt = [scale | shift] as AdaLayerNormContinuous chunks it).
+    stream only feeds q/k/v; mod_txt = [scale | shift] as AdaLayerNormContinuous chunks it), `full` (full
+    fine-tune, SD3: see below).
 
-    inputs: h, mod_img [B, 6D|9D], mod_txt [B, 6D|2D] (adaLN vectors, no grad), cos, sin (or None), st, then the
+    inputs: h, mod_img [B, 6D|9D], mod_txt [B, 6D|2D] (adaLN vectors), cos, sin (or None), st, then the
     flat LoRA tensors (None where not adapted) in the order
       img : to_q.A, to_q.B, to_k.A, to_k.B, to_v.A, to_v.B, to_out.A, to_out.B            [0..7]
       txt : add_q.A, add_q.B, add_k.*, add_v.*, to_add_out.A, to_add_out.B               [8..15]
       attn2: to_q.A, to_q.B, to_k.*, to_v.*, to_out.A, to_out.B                          [16..23]
       mlp : ff.net.0.proj.A, .B, ff.net.2.A, .B, ff_context.net.0.proj.A, .B, ff_context.net.2.A, .B   [24..31]
+    Full fine-tune: each (A, B) slot holds that Linear's (weight, bias) and gets its gradient from the group's dW
+    (WgradPack); slots [32..37] hold the q / k RMSNorm weights (norm_q, norm_k, norm_added_q, norm_added_k, attn2's norm_q,
+    norm_k), and mod_img / mod_txt get their gradients (shift / scale / gate column sums; the GATE_RES epilogues also write
+    the pre-gate outputs for the gates).
     """
 
     @staticmethod
@@ -463,13 +503,14 @@ class DoubleBlockFn(torch.autograd.Function):
         dev = h.device
         drop: Optional[LoraDrop] = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
+        full = st.get("full", False)
+        ls = st.get("lokr_scales")                   # per (A, B) pair of the flat list: LoKr scale, or None for LoRA
+        assert not (full and (st.get("img_segs") or drop is not None or ls)), "full fine-tune: no segments, dropout or LoKr"
         n_lora_in = len(lora)
         lora = list(lora) + [None] * (32 - len(lora))
         segs = {"txt": _segments(mod_txt, None, S_txt), "img": _segments(mod_img, st.get("img_segs"), S - S_txt)}
         streams = (("txt", slice(0, S_txt), mod_txt, 8), ("img", slice(S_txt, S), mod_img, 0))
         mlp_base = {"img": 24, "txt": 28}
-
-        ls = st.get("lokr_scales")                   # per (A, B) pair of the flat list: LoKr scale, or None for LoRA
         lsc = (lambda i: ls[i // 2] if ls is not None and i // 2 < len(ls) else None)
 
         def lp(base, n_members, n_out, k_in):
@@ -477,7 +518,7 @@ class DoubleBlockFn(torch.autograd.Function):
             for m in range(n_members):
                 a, b = lora[base + 2 * m], lora[base + 2 * m + 1]
                 ps.append(None if a is None else (a, b))
-            return make_pack(ps, n_out, k_in, scaling, dev, [lsc(base + 2 * m) for m in range(n_members)])
+            return make_pack(ps, n_out, k_in, scaling, dev, [lsc(base + 2 * m) for m in range(n_members)], full)
 
         def mod_shift_scale(name):      # chunk indices of (shift, scale)
             return (1, 0) if name == "txt" and pre_only else (0, 1)
@@ -505,6 +546,9 @@ class DoubleBlockFn(torch.autograd.Function):
         o = o.view(B, S, D)
         h1 = torch.empty_like(h)
         h2 = torch.empty_like(h)
+        y_attn = torch.empty_like(h) if full else None      # pre-gate outputs of the gated linears: the gate gradients
+        y_mlp = torch.empty_like(h) if full else None
+        y_at = (lambda y, sl: y[:, sl] if y is not None else None)
         for name, sl, mod, base in streams:
             ap = plans[name + "_attn"]
             if name == "txt" and pre_only:
@@ -513,8 +557,8 @@ class DoubleBlockFn(torch.autograd.Function):
                 small[name + "_t_out"] = None
                 continue
             small[name + "_t_out"] = _linear_lora_gate_res(o[:, sl], ap.w_out, ap.b_out, packs[name + "_out"], dr(base + 6),
-                                                           segs[name], 2, res=h[:, sl], out=h1[:, sl])
-        qkv2 = o2 = lse2 = None
+                                                           segs[name], 2, res=h[:, sl], out=h1[:, sl], aux=y_at(y_attn, sl))
+        qkv2 = o2 = lse2 = y_attn2 = None
         if dual:
             isl = slice(S_txt, S)
             a2: AttnPlan = plans["img_attn2"]
@@ -528,9 +572,10 @@ class DoubleBlockFn(torch.autograd.Function):
             o2, lse2 = ops.attn_fwd(q2, k2, qkv2[:, :, 2 * D:].unflatten(-1, (H, hd)))
             del q2, k2
             o2 = o2.view(B, S - S_txt, D)
+            y_attn2 = torch.empty_like(o2) if full else None
             # h1_img += gate_msa2 * to_out2(o2)   (in place: every element is read then written by one thread)
             _, t = _linear_lora_fwd(o2, a2.w_out, a2.b_out, packs["a2_out"], dr(22), out=h1[:, isl], epi=ops.EPI_GATE_RES,
-                                    gate=mod_img[:, 8 * D:9 * D], res=h1[:, isl])
+                                    gate=mod_img[:, 8 * D:9 * D], res=h1[:, isl], aux=y_attn2)
             small["a2_t_out"] = t
         mlp_pre = {}
         for name, sl, mod, base in streams:
@@ -541,13 +586,14 @@ class DoubleBlockFn(torch.autograd.Function):
             nh2 = _lnm_fwd(h1[:, sl], segs[name], 3, 4)
             pre = torch.empty((B, sl.stop - sl.start, 4 * D), device=dev, dtype=torch.bfloat16)
             mb = mlp_base[name]
-            pk1 = packs[name + "_fc1"] = _pack1(lora[mb], lora[mb + 1], 4 * D, D, scaling, dev, lsc(mb))
-            pk2 = packs[name + "_fc2"] = _pack1(lora[mb + 2], lora[mb + 3], D, 4 * D, scaling, dev, lsc(mb + 2))
+            pk1 = packs[name + "_fc1"] = _pack1(lora[mb], lora[mb + 1], 4 * D, D, scaling, dev, lsc(mb), full)
+            pk2 = packs[name + "_fc2"] = _pack1(lora[mb + 2], lora[mb + 3], D, 4 * D, scaling, dev, lsc(mb + 2), full)
             act, t = _linear_lora_fwd(nh2, mp.w1, mp.b1, pk1, dr(base + 3), epi=ops.EPI_GELU, aux=pre)
             small[name + "_t_fc1"] = t
             del nh2
             small[name + "_t_fc2"] = _linear_lora_gate_res(act, mp.w2, mp.b2, pk2, dr(base + 4), segs[name], 5, res=h1[:, sl],
-                                                           out=h2[:, sl], nan_to_num=(name == "txt" and nan_txt))
+                                                           out=h2[:, sl], nan_to_num=(name == "txt" and nan_txt),
+                                                           aux=y_at(y_mlp, sl))
             del act
             mlp_pre[name] = pre
         ctx.st = st
@@ -561,13 +607,14 @@ class DoubleBlockFn(torch.autograd.Function):
                               keep(qkv2), keep(o2), keep(lse2), keep(small.get("a2_t_qkv")), keep(small.get("a2_t_out")),
                               q if keep_qk else E, k if keep_qk else E,
                               keep(small.get("txt_t_fc1")), keep(small.get("txt_t_fc2")), keep(small.get("img_t_fc1")),
-                              keep(small.get("img_t_fc2")), keep(nh_joint))
+                              keep(small.get("img_t_fc2")), keep(nh_joint), keep(y_attn), keep(y_mlp), keep(y_attn2))
         return h2
 
     @staticmethod
     def backward(ctx, dh2):
         (h, mod_img, mod_txt, cos, sin, qkv, o, lse, h1, pre_txt, pre_img, t_qkv_txt, t_qkv_img, t_out_txt, t_out_img,
-         qkv2, o2, lse2, t_qkv_a2, t_out_a2, q_saved, k_saved, t_fc1_txt, t_fc2_txt, t_fc1_img, t_fc2_img, nh_saved) = ctx.saved_tensors
+         qkv2, o2, lse2, t_qkv_a2, t_out_a2, q_saved, k_saved, t_fc1_txt, t_fc2_txt, t_fc1_img, t_fc2_img, nh_saved,
+         y_attn, y_mlp, y_attn2) = ctx.saved_tensors
         qk_saved = (q_saved, k_saved) if q_saved.numel() else None
         cos = cos if cos.numel() else None
         sin = sin if sin.numel() else None
@@ -580,12 +627,16 @@ class DoubleBlockFn(torch.autograd.Function):
         dual = st.get("dual", False)
         drop: Optional[LoraDrop] = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
+        full = st.get("full", False)
         dh2 = dh2.contiguous()
         segs = {"txt": _segments(mod_txt, None, S_txt), "img": _segments(mod_img, st.get("img_segs"), S - S_txt)}
+        # d mod (full fine-tune): fp32 column sums, every chunk written
+        dms = {"txt": torch.zeros_like(mod_txt, dtype=torch.float32), "img": torch.zeros_like(mod_img, dtype=torch.float32)} \
+            if full else None
         streams = (("txt", slice(0, S_txt), mod_txt, 8, pre_txt, t_qkv_txt, t_out_txt),
                    ("img", slice(S_txt, S), mod_img, 0, pre_img, t_qkv_img, t_out_img))
         mlp_t = {"txt": (28, t_fc1_txt, t_fc2_txt), "img": (24, t_fc1_img, t_fc2_img)}
-        grads: List[Optional[torch.Tensor]] = [None] * 32
+        grads: List[Optional[torch.Tensor]] = [None] * 38
         dh1 = torch.empty_like(h)
         d_o = torch.empty_like(o)
         for name, sl, mod, base, pre, t_qkv, t_out in streams:
@@ -596,6 +647,8 @@ class DoubleBlockFn(torch.autograd.Function):
                 continue
             mp: MlpPlan = plans[name + "_mlp"]
             # ---- MLP branch: h2 = h1 + gate_mlp * fc2(gelu(fc1(LNmod(h1))))
+            if full:
+                _dmod_gate(dms[name], dh2[:, sl], y_mlp[:, sl], 5)
             g2 = _gate_mul(dh2[:, sl], segs[name], 5)
             mb, t_fc1, t_fc2 = mlp_t[name]
             pk1, pk2 = packs.get(name + "_fc1"), packs.get(name + "_fc2")
@@ -611,9 +664,13 @@ class DoubleBlockFn(torch.autograd.Function):
                 (grads[mb], grads[mb + 1]), = _lora_grads(pk1, nh2, t_fc1, d_pre, t_up, dr(base + 3))
                 del nh2
             del d_pre
+            if full:
+                _dmod_shift_scale(dms[name], d_nh2, h1[:, sl], 3, 4)
             _lnm_bwd(d_nh2, h1[:, sl], segs[name], 4, add=dh2[:, sl], out=dh1[:, sl])
             del d_nh2
             # ---- attention output projection: h1 = h + gate_msa * to_out(o)
+            if full:
+                _dmod_gate(dms[name], dh1[:, sl], y_attn[:, sl], 2)
             g1 = _gate_mul(dh1[:, sl], segs[name], 2)
             pk = packs[name + "_out"]
             _, t_up = _linear_lora_dgrad(g1, ap.w_out_t, pk, dr(base + 6), out=d_o[:, sl])
@@ -626,6 +683,8 @@ class DoubleBlockFn(torch.autograd.Function):
         if dual:
             isl = slice(S_txt, S)
             a2: AttnPlan = plans["img_attn2"]
+            if full:
+                _dmod_gate(dms["img"], dh1[:, isl], y_attn2, 8)
             g = ops.gate_mul(dh1[:, isl], mod_img[:, 8 * D:9 * D])
             pk = packs["a2_out"]
             d_o2, t_up = _linear_lora_dgrad(g, a2.w_out_t, pk, dr(22))
@@ -633,7 +692,10 @@ class DoubleBlockFn(torch.autograd.Function):
                 (da, db), = _lora_grads(pk, o2, t_out_a2, g, t_up, dr(22))
                 grads[22], grads[23] = da, db
             del g
-            d_qkv2 = _attn_core_bwd(qkv2, o2, d_o2, lse2, D, H, hd, a2, None, 0, None, None)
+            dw2 = torch.zeros((4, hd), device=h.device, dtype=torch.float32) if full and a2.norm_q is not None else None
+            d_qkv2 = _attn_core_bwd(qkv2, o2, d_o2, lse2, D, H, hd, a2, None, 0, None, None, dw=dw2)
+            if dw2 is not None:
+                grads[36], grads[37] = dw2.to(torch.bfloat16)[:2]
             del d_o2
             pk = packs["a2_qkv"]
             d_nh2a, t_up = _linear_lora_dgrad(d_qkv2, a2.w_qkv_t, pk, dr(16))
@@ -643,19 +705,26 @@ class DoubleBlockFn(torch.autograd.Function):
                     grads[16 + 2 * m], grads[16 + 2 * m + 1] = da, db
                 del nh2a
             del d_qkv2
+            if full:
+                _dmod_shift_scale(dms["img"], d_nh2a, h[:, isl], 6, 7)
         # ---- joint attention core
+        dw = torch.zeros((4, hd), device=h.device, dtype=torch.float32) if full and plans["img_attn"].norm_q is not None else None
         d_qkv = _attn_core_bwd(qkv, o, d_o, lse, D, H, hd, plans["img_attn"], plans["txt_attn"], S_txt, cos, sin, qk=qk_saved,
-                               key_bias=st.get("key_bias"))
+                               key_bias=st.get("key_bias"), dw=dw)
+        if dw is not None:
+            grads[32:36] = dw.to(torch.bfloat16)
         del qk_saved, q_saved, k_saved
         dh = torch.empty_like(h)
         for name, sl, mod, base, pre, t_qkv, t_out in streams:
             ap = plans[name + "_attn"]
             pk = packs[name + "_qkv"]
-            isc = 0 if name == "txt" and pre_only else 1         # chunk index of the scale
+            ish, isc = (1, 0) if name == "txt" and pre_only else (0, 1)     # chunk indices of (shift, scale)
             d_nh, t_up = _linear_lora_dgrad(d_qkv[:, sl], ap.w_qkv_t, pk, dr(base))
             if pk is not None:
                 for m, (da, db) in enumerate(_lora_grads(pk, nh_saved[:, sl], t_qkv, d_qkv[:, sl], t_up, dr(base))):
                     grads[base + 2 * m], grads[base + 2 * m + 1] = da, db
+            if full:
+                _dmod_shift_scale(dms[name], d_nh, h[:, sl], ish, isc)
             _lnm_bwd(d_nh, h[:, sl], segs[name], isc, add=dh1[:, sl], out=dh[:, sl])
             del d_nh
         if dual:
@@ -664,6 +733,8 @@ class DoubleBlockFn(torch.autograd.Function):
         out_grads = []
         for i in range(ctx.n_lora_in):
             out_grads.append(grads[i] if ctx.lora_present[i] else None)
+        if full:
+            return (dh, dms["img"].to(mod_img.dtype), dms["txt"].to(mod_txt.dtype), None, None, None, *out_grads)
         return (dh, None, None, None, None, None, *out_grads)
 
 
@@ -695,7 +766,7 @@ class SingleBlockFn(torch.autograd.Function):
         pk = make_pack(ps, D, D, scaling, dev, [lsc(0), lsc(2), lsc(4)])
         pk_mlp = _pack1(lora[6], lora[7], 4 * D, D, scaling, dev, lsc(6))
         pk_out = _pack1(lora[8], lora[9], D, 5 * D, scaling, dev, lsc(8))
-        if isinstance(pk_out, LokrPack):
+        if isinstance(pk_out, WgradPack):
             raise NotImplementedError("LoKr on the single blocks' proj_out is not part of the LyCORIS presets supported here")
         drop: Optional[LoraDrop] = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
@@ -770,7 +841,7 @@ class SingleBlockFn(torch.autograd.Function):
         # d_nh = d_pre W_mlp + d_qkv W_qkv (+ LoRA branches as one more K-segment)
         t_ups, a_ts = [], []
         t_up_qkv = t_up_mlp = None
-        is_lora = lambda q: q is not None and not isinstance(q, LokrPack)
+        is_lora = lambda q: q is not None and not isinstance(q, WgradPack)
         if is_lora(pk):
             t_up_qkv = ops.gemm([d_qkv], [pk.b_ext_t])
             t_ups.append(t_up_qkv); a_ts.append(pk.a_stack_t)
@@ -805,14 +876,15 @@ class TailFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h, mod, st, *lora):
         """h [B, S, D] joint buffer; mod [B, 2D] = (scale | shift) (AdaLayerNormContinuous chunk order).  lora: the final
-        proj_out's (A, B) — PEFT's suffix rule makes the "proj_out" target of "all+ffs" select it too.  Rows
-        [S_txt, S_end) are projected (S_end: the end of the Kontext scene tokens, default S)."""
+        proj_out's (A, B) — PEFT's suffix rule makes the "proj_out" target of "all+ffs" select it too — or, with
+        st["full"], proj_out's (weight, bias), and d mod is returned too.  Rows [S_txt, S_end) are projected (S_end: the
+        end of the Kontext scene tokens, default S)."""
         D = h.shape[2]
         S_txt, S_end = st["S_txt"], st.get("S_end") or h.shape[1]
         x = h[:, S_txt:S_end]
         nx = ops.ln_modulate_fwd(x, mod[:, D:2 * D], mod[:, 0:D], EPS)
         a, b = (lora[0], lora[1]) if len(lora) >= 2 else (None, None)
-        pk = _pack1(a, b, st["w_proj"].shape[0], D, st.get("lora_scaling", 1.0), h.device)
+        pk = _pack1(a, b, st["w_proj"].shape[0], D, st.get("lora_scaling", 1.0), h.device, full=st.get("full", False))
         out, t = _linear_lora_fwd(nx, st["w_proj"], st["b_proj"], pk, st.get("lora_drop"))
         ctx.st, ctx.pack, ctx.n_lora_in = st, pk, len(lora)
         ctx.save_for_backward(h, mod, t if t is not None else h.new_empty(0))
@@ -830,9 +902,14 @@ class TailFn(torch.autograd.Function):
         if pk is not None:
             nx = ops.ln_modulate_fwd(h[:, S_txt:S_end], mod[:, D:2 * D], mod[:, 0:D], EPS)
             (lg[0], lg[1]), = _lora_grads(pk, nx, t, d_out, t_up, st.get("lora_drop"))
+        dm = None
+        if st.get("full", False):
+            dm = torch.zeros_like(mod, dtype=torch.float32)
+            _dmod_shift_scale(dm, d_nx, h[:, S_txt:S_end], 1, 0)
+            dm = dm.to(mod.dtype)
         dh = torch.zeros_like(h) if S_txt > 0 or S_end < h.shape[1] else torch.empty_like(h)
         ops.ln_modulate_bwd(d_nx, h[:, S_txt:S_end], mod[:, 0:D], add=None, eps=EPS, out=dh[:, S_txt:S_end])
-        return (dh, None, None, *lg)
+        return (dh, dm, None, *lg)
 
 
 class FlowLossFn(torch.autograd.Function):

@@ -20,7 +20,9 @@ The additive -10000 key mask of cross attention (reference :562-564) rides in th
 q[..., 72] = 1 (a bias entry of the padded to_q), k[b, j, :, 72] = -10000 / scale for masked keys — masked keys get
 probability exactly 0 like the reference's fp32 softmax, with no mask operand in the kernel.
 Unsupported (raise): token-wise timesteps, TREAD routes, controlnet residuals, flow-map `r_timestep`, GLIGEN,
-self-attention masks.  Full fine-tune (model_type=full) runs through pixart/fullft.py after `enable_full_finetune()`.
+self-attention masks.  Full fine-tune (model_type=full), after `enable_full_finetune()`, runs the same `PixArtBlockFn` /
+`TailFn` schedules with every Linear's (weight, bias) in the adapter slots (`PixArtTransformerBlock.block_slots`); the
+patch embedding and the caption projection have Functions of their own (`PatchEmbedFullFn`, `CaptionProjectionFullFn`).
 """
 from __future__ import annotations
 
@@ -32,7 +34,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
-from ..flux.blocks import EPS, MlpPlan, TailFn, _linear_lora_dgrad, _linear_lora_fwd, _lora_grads, _t, _wt, pack_lora
+from ..flux.blocks import (EPS, MlpPlan, TailFn, _dmod_gate, _dmod_shift_scale, _linear_lora_dgrad, _linear_lora_fwd, _lora_grads,
+                           _t, _wt, make_pack)
 from ..flux.transformer import (AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, Linear, _FeedForward, _lora_list, _sinusoid,
                                 _TimestepEmbedding)
 from ..pretrained import ModelConfig, PretrainedIOAPI
@@ -71,8 +74,13 @@ class _Attention(nn.Module):
 
 
 class PixArtBlockFn(torch.autograd.Function):
-    """inputs: h [B,S,D], ctx [B,St,Dc] (projected caption, no grad), kbias [B,St] bf16 or None, mod [B,6D], st, then the
-    flat LoRA tensors: attn1 to_q.A,B to_k.A,B to_v.A,B to_out.A,B [0..7]; attn2 likewise [8..15]."""
+    """inputs: h [B,S,D], ctx [B,St,Dc] (projected caption), kbias [B,St] bf16 or None, mod [B,6D], st, then the
+    flat LoRA tensors: attn1 to_q.A,B to_k.A,B to_v.A,B to_out.A,B [0..7]; attn2 likewise [8..15].
+
+    Full fine-tune (st["full"]): each (A, B) slot holds that Linear's (weight, bias), slots [16..19] hold the FeedForward's
+    net.0.proj and net.2 (weight, bias), and every one of them gets its gradient from its group's dW (WgradPack; padded
+    heads are gathered back to the real rows / columns).  The block also returns d mod (shift / scale / gate column sums;
+    the GATE_RES epilogues write the pre-gate outputs for the gates) and d ctx, through the k | v dgrad."""
 
     @staticmethod
     def forward(ctx_, h, enc, kbias, mod, st, *lora):
@@ -85,16 +93,25 @@ class PixArtBlockFn(torch.autograd.Function):
         dev = h.device
         drop = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
+        full = st.get("full", False)
+        assert not (full and drop is not None), "full fine-tune: no LoRA dropout"
+        mp: MlpPlan = pl["mlp"]
 
         def lp(base, n, n_out, k_in, rows):
             ps = []
             for m in range(n):
                 a, b = lora[base + 2 * m], lora[base + 2 * m + 1]
                 ps.append(None if a is None else (a, b))
-            return pack_lora(ps, n_out, k_in, scaling, dev, row_index=ridx if rows else None, col_index=None if rows else ridx)
+            return make_pack(ps, n_out, k_in, scaling, dev, full=full, row_index=ridx if rows else None,
+                             col_index=None if rows else ridx)
 
         pk = {"qkv1": lp(0, 3, Hp, D, True), "out1": lp(6, 1, D, Hp, False), "q2": lp(8, 1, Hp, D, True),
               "kv2": lp(10, 2, Hp, enc.shape[2], True), "out2": lp(14, 1, D, Hp, False)}
+        if full:
+            pk["fc1"] = make_pack([(lora[16], lora[17])], mp.w1.shape[0], D, scaling, dev, full=True)
+            pk["fc2"] = make_pack([(lora[18], lora[19])], D, mp.w1.shape[0], scaling, dev, full=True)
+        y_attn = torch.empty_like(h) if full else None      # pre-gate outputs of the gated linears: the gate gradients
+        y_mlp = torch.empty_like(h) if full else None
         # ---- self attention
         nh = ops.ln_modulate_fwd(h, mod[:, 0:D], mod[:, D:2 * D], EPS)
         qkv, t_qkv = _linear_lora_fwd(nh, pl["w_qkv1"], pl["b_qkv1"], pk["qkv1"], dr(0))
@@ -103,7 +120,7 @@ class PixArtBlockFn(torch.autograd.Function):
         o, lse = ops.attn_fwd(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale=scale)
         o = o.view(B, S, Hp)
         h1, t_out1 = _linear_lora_fwd(o, pl["w_out1"], pl["b_out1"], pk["out1"], dr(3), epi=ops.EPI_GATE_RES,
-                                      gate=mod[:, 2 * D:3 * D], res=h)
+                                      gate=mod[:, 2 * D:3 * D], res=h, aux=y_attn)
         # ---- cross attention on the un-normed stream (ada_norm_single: no norm2 before attn2)
         q2, t_q2 = _linear_lora_fwd(h1, pl["w_q2"], pl["b_q2"], pk["q2"], dr(4))
         kv2, t_kv2 = _linear_lora_fwd(enc, pl["w_kv2"], pl["b_kv2"], pk["kv2"], dr(5))
@@ -115,24 +132,24 @@ class PixArtBlockFn(torch.autograd.Function):
         o2 = o2.view(B, S, Hp)
         h2, t_out2 = _linear_lora_fwd(o2, pl["w_out2"], pl["b_out2"], pk["out2"], dr(7), epi=ops.EPI_ADD_RES, res=h1)
         # ---- feed forward
-        mp: MlpPlan = pl["mlp"]
         nh2 = ops.ln_modulate_fwd(h2, mod[:, 3 * D:4 * D], mod[:, 4 * D:5 * D], EPS)
         pre = torch.empty((B, S, mp.w1.shape[0]), device=dev, dtype=torch.bfloat16)
         act = ops.gemm([nh2], [mp.w1], mp.b1, epi=ops.EPI_GELU, aux=pre)
         del nh2
-        h3 = ops.gemm([act], [mp.w2], mp.b2, epi=ops.EPI_GATE_RES, gate=mod[:, 5 * D:6 * D], res=h2)
+        h3 = ops.gemm([act], [mp.w2], mp.b2, epi=ops.EPI_GATE_RES, gate=mod[:, 5 * D:6 * D], res=h2, aux=y_mlp)
         del act
         ctx_.st, ctx_.pk = st, pk
         ctx_.lora_present = [x is not None for x in lora]
         E = h.new_empty(0)
         keep = lambda t: t if t is not None else E
         ctx_.save_for_backward(h, enc, mod, qkv, o, lse, h1, q2, kv2, o2, lse2, h2, pre, keep(t_qkv), keep(t_out1),
-                               keep(t_q2), keep(t_kv2), keep(t_out2))
+                               keep(t_q2), keep(t_kv2), keep(t_out2), keep(y_attn), keep(y_mlp))
         return h3
 
     @staticmethod
     def backward(ctx_, dh3):
-        (h, enc, mod, qkv, o, lse, h1, q2, kv2, o2, lse2, h2, pre, t_qkv, t_out1, t_q2, t_kv2, t_out2) = ctx_.saved_tensors
+        (h, enc, mod, qkv, o, lse, h1, q2, kv2, o2, lse2, h2, pre, t_qkv, t_out1, t_q2, t_kv2, t_out2, y_attn,
+         y_mlp) = ctx_.saved_tensors
         st, pk = ctx_.st, ctx_.pk
         B, S, D = h.shape
         H, hd, hdp = st["H"], st["hd"], st["hdp"]
@@ -141,16 +158,28 @@ class PixArtBlockFn(torch.autograd.Function):
         pl = st["plans"]
         mp: MlpPlan = pl["mlp"]
         scale = hd ** -0.5
-        grads: List[Optional[torch.Tensor]] = [None] * 16
+        grads: List[Optional[torch.Tensor]] = [None] * len(ctx_.lora_present)
         drop = st.get("lora_drop")
         dr = (lambda off: drop.at(off)) if drop is not None else (lambda off: None)
+        full = st.get("full", False)
+        dm = torch.empty((B, 6 * D), device=h.device, dtype=torch.float32) if full else None   # every chunk is written
         dh3 = dh3.contiguous()
         # ---- feed forward: h3 = h2 + gate_mlp * fc2(gelu(fc1(LNmod(h2))))
+        if full:
+            _dmod_gate(dm, dh3, y_mlp, 5)
         g = ops.gate_mul(dh3, mod[:, 5 * D:6 * D])
+        if full:
+            (grads[18], grads[19]), = _lora_grads(pk["fc2"], ops.gelu_tanh(pre), None, g, None)
         d_pre = ops.gemm([g], [mp.w2_t], None, epi=ops.EPI_MUL_DGELU, aux=pre)
         del g
+        if full:
+            nh2 = ops.ln_modulate_fwd(h2, mod[:, 3 * D:4 * D], mod[:, 4 * D:5 * D], EPS)
+            (grads[16], grads[17]), = _lora_grads(pk["fc1"], nh2, None, d_pre, None)
+            del nh2
         d_nh2 = ops.gemm([d_pre], [mp.w1_t], None)
         del d_pre
+        if full:
+            _dmod_shift_scale(dm, d_nh2, h2, 3, 4)
         dh2 = ops.ln_modulate_bwd(d_nh2, h2, mod[:, 4 * D:5 * D], add=dh3, eps=EPS)
         del d_nh2
         # ---- cross attention: h2 = h1 + to_out2(attn(q2(h1), kv2(ctx)))
@@ -168,12 +197,17 @@ class PixArtBlockFn(torch.autograd.Function):
         if pk["q2"] is not None:
             (grads[8], grads[9]), = _lora_grads(pk["q2"], h1, t_q2, d_q2, t_up, dr(4))
         del d_q2
-        if pk["kv2"] is not None:   # no d ctx: the caption projection is frozen and carries no adapter
-            t_up = ops.gemm([d_kv2], [pk["kv2"].b_ext_t])
+        if pk["kv2"] is not None:
+            t_up = None if full else ops.gemm([d_kv2], [pk["kv2"].b_ext_t])
             for m, (da, db) in enumerate(_lora_grads(pk["kv2"], enc, t_kv2, d_kv2, t_up, dr(5))):
                 grads[10 + 2 * m], grads[11 + 2 * m] = da, db
+        # d ctx in full fine-tune only: otherwise the caption projection is frozen and carries no adapter.  The padded k / v
+        # rows of w_kv2 are zero, so the mask column's dk does not reach it.
+        d_enc = ops.gemm([d_kv2], [pl["w_kv2_t"]], None) if full else None
         del d_kv2
         # ---- self attention: h1 = h + gate_msa * to_out1(attn(qkv(LNmod(h))))
+        if full:
+            _dmod_gate(dm, dh1, y_attn, 2)
         g1 = ops.gate_mul(dh1, mod[:, 2 * D:3 * D])
         d_o, t_up = _linear_lora_dgrad(g1, pl["w_out1_t"], pk["out1"], dr(3))
         if pk["out1"] is not None:
@@ -192,9 +226,11 @@ class PixArtBlockFn(torch.autograd.Function):
                 grads[2 * m], grads[2 * m + 1] = da, db
             del nh
         del d_qkv
+        if full:
+            _dmod_shift_scale(dm, d_nh, h, 0, 1)
         dh = ops.ln_modulate_bwd(d_nh, h, mod[:, D:2 * D], add=dh1, eps=EPS)
         out = [grads[i] if ctx_.lora_present[i] else None for i in range(len(ctx_.lora_present))]
-        return (dh, None, None, None, None, *out)
+        return (dh, d_enc, None, dm.to(mod.dtype) if full else None, None, *out)
 
 
 class PixArtTransformerBlock(nn.Module):
@@ -243,15 +279,65 @@ class PixArtTransformerBlock(nn.Module):
         B, _, D = h.shape
         # reference :98-102 / diffusers: (scale_shift_table[None] + timestep.reshape(B, 6, -1)) in the weight dtype
         mod = (self.scale_shift_table[None] + t6.reshape(B, 6, D)).reshape(B, 6 * D)
+        full = bool(getattr(self, "_full_ft", False))
         st = {"H": self.heads, "hd": self.head_dim, "hdp": self.hdp, "plans": self.plans(), "lora_scaling": lora_scaling,
-              "pad_index": pad_index, "lora_drop": getattr(self, "_lora_drop", None)}
-        if getattr(self, "_full_ft", False):
-            from .fullft import BLOCK_PARAMS, PixArtBlockFullFn
-            params = dict(self.named_parameters())
-            return PixArtBlockFullFn.apply(h, ctx, kbias, mod, st, *[params[n] for n in BLOCK_PARAMS])
+              "pad_index": pad_index, "lora_drop": getattr(self, "_lora_drop", None), "full": full}
+        return PixArtBlockFn.apply(h, ctx, kbias, mod, st, *self.block_slots())
+
+    def block_slots(self):
+        """PixArtBlockFn's flat slot list: the (A, B) of both attentions' projections, or in full fine-tune every Linear's
+        (weight, bias), the FeedForward's included.  `scale_shift_table` trains through torch autograd on `mod`."""
         a1, a2 = self.attn1, self.attn2
-        lora = _lora_list([a1.to_q, a1.to_k, a1.to_v, a1.to_out[0], a2.to_q, a2.to_k, a2.to_v, a2.to_out[0]])
-        return PixArtBlockFn.apply(h, ctx, kbias, mod, st, *lora)
+        lins = [a1.to_q, a1.to_k, a1.to_v, a1.to_out[0], a2.to_q, a2.to_k, a2.to_v, a2.to_out[0]]
+        if not getattr(self, "_full_ft", False):
+            return _lora_list(lins)
+        return [t for lin in lins + [self.ff.net[0].proj, self.ff.net[2]] for t in (lin.weight, lin.bias)]
+
+
+def _bias_grad(dy: torch.Tensor) -> torch.Tensor:
+    return ops.colsum2(dy)[0].sum(0).to(torch.bfloat16)
+
+
+class PatchEmbedFullFn(torch.autograd.Function):
+    """PatchEmbed as the forward runs it (a GEMM over the (c, dy, dx) patch features, + the sincos table in the epilogue)
+    with gradients for the conv weight [D, C, 2, 2] and bias.  No input gradient: the latents are data."""
+
+    @staticmethod
+    def forward(ctx, x, pos, w_pe, b_pe):
+        D = w_pe.shape[0]
+        h = ops.gemm([x], [w_pe.detach().reshape(D, -1)], b_pe.detach(), epi=ops.EPI_ADD_RES, res=pos)
+        ctx.save_for_backward(x)
+        ctx.w_shape = tuple(w_pe.shape)
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        (x,) = ctx.saved_tensors
+        dh = dh.contiguous()
+        return None, None, ops.wgrad_full(dh, x).reshape(ctx.w_shape), _bias_grad(dh)
+
+
+class CaptionProjectionFullFn(torch.autograd.Function):
+    """PixArtAlphaTextProjection: linear_2(gelu_tanh(linear_1(x))) with gradients for both linears.  Its input gradient
+    d ctx is the sum of the blocks' k / v dgrads; the caption embeddings themselves are data."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2):
+        B, St, _ = x.shape
+        pre = torch.empty((B, St, w1.shape[0]), device=x.device, dtype=torch.bfloat16)
+        act = ops.gemm([x], [w1.detach()], b1.detach(), epi=ops.EPI_GELU, aux=pre)
+        out = ops.gemm([act], [w2.detach()], b2.detach())
+        ctx.save_for_backward(x, pre, w2)
+        return out
+
+    @staticmethod
+    def backward(ctx, d_out):
+        x, pre, w2 = ctx.saved_tensors
+        d_out = d_out.contiguous()
+        dw2 = ops.wgrad_full(d_out, ops.gelu_tanh(pre))
+        db2 = _bias_grad(d_out)
+        d_pre = ops.gemm([d_out], [ops.WT(w2.detach())], None, epi=ops.EPI_MUL_DGELU, aux=pre)
+        return None, ops.wgrad_full(d_pre, x), _bias_grad(d_pre), dw2, db2
 
 
 class _PatchEmbed(nn.Module):
@@ -377,8 +463,8 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         self._tail_plan = {}
 
     def enable_full_finetune(self, enabled: bool = True):
-        """model_type=full: every parameter trains, the blocks' `scale_shift_table` included.  The blocks switch to the full
-        fine-tune schedule (pixart/fullft.py); the padded / fused / transposed weight layouts are rebuilt after every
+        """model_type=full: every parameter trains, the blocks' `scale_shift_table` included.  The blocks run PixArtBlockFn in
+        its full fine-tune mode; the padded / fused / transposed weight layouts are rebuilt after every
         optimizer step (`after_optimizer_step`) because the base weights now change."""
         if enabled and self.lora_linears():
             raise NotImplementedError("full fine-tune and LoRA adapters are mutually exclusive on the libstb200 path")
@@ -454,7 +540,6 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         full = getattr(self, "_full_ft", False) and torch.is_grad_enabled()
         pos = self._pos(hp, wp, dt, dev).expand(B, S, D)
         if full:
-            from .fullft import CaptionProjectionFullFn, PatchEmbedFullFn
             h = PatchEmbedFullFn.apply(x, pos, self.pos_embed.proj.weight, self.pos_embed.proj.bias)
         else:
             w_pe = self.pos_embed.proj.weight.detach().reshape(D, C * 4)
@@ -485,10 +570,7 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
         mod = (self.scale_shift_table[None] + embedded[:, None].to(self.scale_shift_table.dtype)).to(dt)  # [B, 2, D] (shift | scale)
         mod = torch.cat([mod[:, 1], mod[:, 0]], dim=1).contiguous()                                         # TailFn wants (scale | shift)
         keep = self.out_channels // 2 if _packed_output == "eps_half" else self.out_channels
-        if full:
-            out = self._tail_full(h, mod, keep)
-        else:
-            out = self._tail(h, mod, keep)
+        out = self._tail(h, mod, keep, full)
         if not _packed_output:
             Co = self.out_channels
             out = torch.einsum("nhwpqc->nchpwq", out.reshape(B, hp, wp, 2, 2, Co)).reshape(B, Co, hp * 2, wp * 2)
@@ -502,24 +584,19 @@ class PixArtTransformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI
             return None
         return (torch.arange(4, device=dev)[:, None] * self.out_channels + torch.arange(keep, device=dev)[None, :]).reshape(-1)
 
-    def _tail_full(self, h, mod, keep):
-        """Full fine-tune tail: gradients for proj_out and the modulation.  Only the kept rows are computed; the gather
-        hands the learned-sigma rows an explicit zero gradient, as the reference's `.chunk(2, dim=1)[0]` does."""
-        from ..sd3.fullft import TailFullFn
-        w, b = self.proj_out.weight, self.proj_out.bias
-        sel = self._tail_rows(keep, h.device)
-        if sel is not None:
-            w, b = w[sel], b[sel]
-        return TailFullFn.apply(h, mod, w, b, 0)
-
-    def _tail(self, h, mod, keep):
-        dev = h.device
+    def _tail(self, h, mod, keep, full):
+        """full: proj_out's kept rows are TailFn's slot, so proj_out and the modulation get gradients; the gather hands the
+        learned-sigma rows an explicit zero gradient, as the reference's `.chunk(2, dim=1)[0]` does."""
         tp = self._tail_plan.get(keep)
+        sel = self._tail_rows(keep, h.device) if tp is None or full else None
         if tp is None:
             w, b = self.proj_out.weight.detach(), self.proj_out.bias.detach()
-            sel = self._tail_rows(keep, dev)
             if sel is not None:   # PixartSigma keeps `.chunk(2, dim=1)[0]` only (pixart/model.py:313): skip the rest
                 w, b = w[sel].contiguous(), b[sel].contiguous()
             tp = {"w_proj": w, "b_proj": b, "w_proj_t": _wt(w)}
             self._tail_plan[keep] = tp
-        return TailFn.apply(h, mod, {"S_txt": 0, **tp})          # [B, S, 4 * keep] in (dy, dx, c) order
+        slot = ()
+        if full:
+            w, b = self.proj_out.weight, self.proj_out.bias
+            slot = (w, b) if sel is None else (w[sel], b[sel])
+        return TailFn.apply(h, mod, {"S_txt": 0, "full": full, **tp}, *slot)          # [B, S, 4 * keep] in (dy, dx, c) order

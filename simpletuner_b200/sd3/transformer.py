@@ -12,8 +12,9 @@ image-only `attn2` (dual_attention_layers) and the `context_pre_only` last block
 The 2x2 stride-2 PatchEmbed conv is a K=64 GEMM on the patchified latents (same (c, dy, dx) feature order as
 Flux `pack_latents`) with the cropped positional table added in the epilogue.
 Unsupported: TREAD routing, controlnet residuals, token-wise timesteps, flow-map / TwinFlow inputs, full
-— they raise so a shim can keep the reference module.  Full fine-tune (model_type=full, BASELINE configs[2]) runs
-through sd3/fullft.py after `enable_full_finetune()`.
+— they raise so a shim can keep the reference module.  Full fine-tune (model_type=full, BASELINE configs[2]), after
+`enable_full_finetune()`, runs the same `DoubleBlockFn` / `TailFn` schedules with every Linear's (weight, bias) in the
+adapter slots (`JointTransformerBlock.block_slots`); only the patch / context embedding has a Function of its own.
 """
 from __future__ import annotations
 
@@ -27,7 +28,7 @@ import torch.nn.functional as F
 from .. import ops
 from ..flux.blocks import DoubleBlockFn, TailFn, _wt
 from ..flux.transformer import (_ATTN, AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, Linear, RMSNormWeight, _AdaNorm,
-                                _FeedForward, _TimestepEmbedding, _attn_plan, _lora_list, _mlp_plan, _sinusoid)
+                                _FeedForward, _TimestepEmbedding, _attn_plan, _mlp_plan, _sinusoid)
 from ..pretrained import ModelConfig, PretrainedIOAPI
 
 SD3_LORA_TARGETS = ["to_k", "to_q", "to_v", "to_out.0"]  # SD3.DEFAULT_LORA_TARGET, reference sd3/model.py:122
@@ -91,40 +92,58 @@ class JointTransformerBlock(nn.Module):
             self._plans = pl
         return self._plans
 
-    FULL_PARAM_ORDER = None
-
-    def full_param_names(self):
-        """Block-local names of every trainable tensor the full fine-tune schedule produces a gradient for (adaLN linears
-        are differentiated by torch autograd outside the block Function)."""
-        if self.FULL_PARAM_ORDER is None:
-            skip = ("norm1.", "norm1_context.")
-            self.FULL_PARAM_ORDER = [n for n, _ in self.named_parameters() if not n.startswith(skip) and ".lora_" not in n]
-        return self.FULL_PARAM_ORDER
+    def block_slots(self):
+        """DoubleBlockFn's flat slot list.  LoRA: the (A, B) of the adapted attention projections.  Full fine-tune: every
+        Linear's (weight, bias) in the same slots, the FeedForwards' too, then the q / k RMSNorm weights; the adaLN linears
+        (`norm1*`) train through torch autograd on the modulation vectors instead."""
+        a, b = self.attn, getattr(self, "attn2", None)
+        g = lambda m, n: getattr(m, n, None)
+        lins = [a.to_q, a.to_k, a.to_v, a.to_out[0], a.add_q_proj, a.add_k_proj, a.add_v_proj, g(a, "to_add_out")]
+        lins += [b.to_q, b.to_k, b.to_v, b.to_out[0]] if b is not None else [None] * 4
+        if not getattr(self, "_full_ft", False):
+            return [t for lin in lins for t in (lin.lora_tensors() if lin is not None else (None, None))]
+        ffc = g(self, "ff_context")
+        lins += [self.ff.net[0].proj, self.ff.net[2], ffc.net[0].proj if ffc else None, ffc.net[2] if ffc else None]
+        norms = [g(a, "norm_q"), g(a, "norm_k"), g(a, "norm_added_q"), g(a, "norm_added_k"), g(b, "norm_q"), g(b, "norm_k")]
+        return [t for lin in lins for t in ((lin.weight, lin.bias) if lin is not None else (None, None))] + \
+            [n.weight if n is not None else None for n in norms]
 
     def forward(self, h, silu_temb, S_txt, lora_scaling):
         mod_img = self.norm1.linear(silu_temb)
         mod_txt = self.norm1_context.linear(silu_temb)
-        if getattr(self, "_full_ft", False):
-            from .fullft import JointBlockFullFn
-            names = self.full_param_names()
-            params = dict(self.named_parameters())
-            st = {"S_txt": S_txt, "H": self.heads, "hd": self.head_dim, "plans": self.plans(),
-                  "context_pre_only": self.context_pre_only, "dual": self.use_dual_attention, "param_names": names}
-            return JointBlockFullFn.apply(h, mod_img, mod_txt, st, *[params[n] for n in names])
         st = {"S_txt": S_txt, "H": self.heads, "hd": self.head_dim, "plans": self.plans(), "lora_scaling": lora_scaling,
               "nan_to_num_txt": False, "context_pre_only": self.context_pre_only, "dual": self.use_dual_attention,
-              "_n_lora": 24, "lora_drop": getattr(self, "_lora_drop", None)}
-        a = self.attn
-        lins = [a.to_q, a.to_k, a.to_v, a.to_out[0], a.add_q_proj, a.add_k_proj, a.add_v_proj]
-        lora = _lora_list(lins)
-        tao = getattr(a, "to_add_out", None)
-        lora += list(tao.lora_tensors()) if tao is not None else [None, None]
-        if self.use_dual_attention:
-            b = self.attn2
-            lora += _lora_list([b.to_q, b.to_k, b.to_v, b.to_out[0]])
-        else:
-            lora += [None] * 8
-        return DoubleBlockFn.apply(h, mod_img, mod_txt, None, None, st, *lora)
+              "lora_drop": getattr(self, "_lora_drop", None), "full": bool(getattr(self, "_full_ft", False))}
+        return DoubleBlockFn.apply(h, mod_img, mod_txt, None, None, st, *self.block_slots())
+
+
+class EmbedFullFn(torch.autograd.Function):
+    """Joint hidden buffer [text | image] from the patchified latents and the text states, with weight gradients:
+    h[:, S_txt:] = patches W_pe^T + b_pe + pos;  h[:, :S_txt] = enc W_ctx^T + b_ctx  (reference sd3/transformer.py:600-640)."""
+
+    @staticmethod
+    def forward(ctx, patches, enc, pos, w_pe, b_pe, w_ctx, b_ctx):
+        B, S_img, _ = patches.shape
+        S_txt = enc.shape[1]
+        D = w_pe.shape[0]
+        h = torch.empty((B, S_txt + S_img, D), device=patches.device, dtype=torch.bfloat16)
+        ops.gemm([patches], [w_pe.detach().reshape(D, -1)], b_pe.detach(), out=h[:, S_txt:], epi=ops.EPI_ADD_RES, res=pos)
+        ops.gemm([enc], [w_ctx.detach()], b_ctx.detach(), out=h[:, :S_txt])
+        ctx.save_for_backward(patches, enc)
+        ctx.S_txt, ctx.w_pe_shape = S_txt, tuple(w_pe.shape)
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        patches, enc = ctx.saved_tensors
+        S_txt = ctx.S_txt
+        dh = dh.contiguous()
+        d_img, d_txt = dh[:, S_txt:], dh[:, :S_txt]
+        dw_pe = ops.wgrad_full(d_img, patches).reshape(ctx.w_pe_shape)
+        db_pe = ops.colsum2(d_img)[0].sum(0).to(torch.bfloat16)
+        dw_ctx = ops.wgrad_full(d_txt, enc)
+        db_ctx = ops.colsum2(d_txt)[0].sum(0).to(torch.bfloat16)
+        return None, None, None, dw_pe, db_pe, dw_ctx, db_ctx
 
 
 class _PatchEmbed(nn.Module):
@@ -197,8 +216,8 @@ class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, P
         self._pos_cache.clear()
 
     def enable_full_finetune(self, enabled: bool = True):
-        """model_type=full (BASELINE configs[2]): every parameter trains.  The joint blocks switch to the full fine-tune
-        schedule (sd3/fullft.py); fused / transposed weight layouts are rebuilt after every optimizer step
+        """model_type=full (BASELINE configs[2]): every parameter trains.  The joint blocks run DoubleBlockFn in its full
+        fine-tune mode; fused / transposed weight layouts are rebuilt after every optimizer step
         (`after_optimizer_step`, called by TrainStep) because the base weights now change."""
         if enabled and self.lora_linears():
             raise NotImplementedError("full fine-tune and LoRA adapters are mutually exclusive on the libstb200 path")
@@ -262,7 +281,6 @@ class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, P
         full = getattr(self, "_full_ft", False) and torch.is_grad_enabled()
         pos = self._cropped_pos(hp, wp, dt).expand(B, S_img, D)
         if full:
-            from .fullft import EmbedFullFn, TailFullFn
             h = EmbedFullFn.apply(x.contiguous(), encoder_hidden_states.to(dt).contiguous(), pos, self.pos_embed.proj.weight,
                                   self.pos_embed.proj.bias, self.context_embedder.weight, self.context_embedder.bias)
         else:
@@ -280,12 +298,10 @@ class SD3Transformer2DModel(AdapterModelAPI, AttnProcessorAPI, LoraDropoutAPI, P
             h = self._run_block(i, blk, h, silu_temb, S_txt, self._lora_scaling)
         if self._tail_plan is None:
             self._tail_plan = {"w_proj": self.proj_out.weight.detach(), "b_proj": self.proj_out.bias.detach(),
-                               "w_proj_t": _wt(self.proj_out.weight.detach(), bool(getattr(self, "_full_ft", False)))}
+                               "w_proj_t": _wt(self.proj_out.weight.detach())}
         mod = self.norm_out.linear(silu_temb)
-        if full:
-            out = TailFullFn.apply(h, mod, self.proj_out.weight, self.proj_out.bias, S_txt)
-        else:
-            out = TailFn.apply(h, mod, {"S_txt": S_txt, **self._tail_plan})  # [B, S_img, p*p*C_out] in (dy, dx, c) order
+        slot = (self.proj_out.weight, self.proj_out.bias) if full else ()
+        out = TailFn.apply(h, mod, {"S_txt": S_txt, "full": full, **self._tail_plan}, *slot)  # [B, S_img, p*p*C_out], (dy, dx, c)
         if not _packed_output:
             Co = self.out_channels
             out = torch.einsum("nhwpqc->nchpwq", out.reshape(B, hp, wp, 2, 2, Co)).reshape(B, Co, hp * 2, wp * 2)

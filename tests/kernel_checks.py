@@ -786,7 +786,8 @@ def check_ln_modulate(B=2, S=64, D=3072, eps=1e-6, window=False, chunks=6, chunk
     Rows 0-3 of every sample are _ln_edge_rows: zero rows must give shift bit for bit.
     window: x, dy, add and out are row / column windows of joint [B, 77 + S + 2, D + 16] buffers (text rows first), the
     halo of out must stay zero.  shift / scale: chunks `chunk`, `chunk + 1` of a [B, chunks D] modulation tensor.
-    add: "add" (a separate residual gradient), None, or "alias" (add is the output buffer, as sd3/fullft.py does).
+    add: "add" (a separate residual gradient), None, or "alias" (add is the output buffer, as the dual-attention backward of
+    flux/blocks.py::DoubleBlockFn does).
     D > 4096 (the VPT = 8 forward) has no backward."""
     def rows(seed, zero=False):
         if not window:

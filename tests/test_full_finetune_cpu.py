@@ -191,3 +191,53 @@ def test_load_state_dict_drops_the_full_finetune_layouts():
     m.after_optimizer_step()
     m.after_optimizer_step()       # a second drop in the same step is a no-op
     assert all(blk._plans is None for blk in m.transformer_blocks)
+
+
+SLOT_CASES = [(SD3Transformer2DModel, SD3_TINY, ("norm1.", "norm1_context.")),
+              (SD3Transformer2DModel, dict(SD3_TINY, dual_attention_layers=(), qk_norm=None), ("norm1.", "norm1_context.")),
+              (PixArtTransformer2DModel, PIXART_TINY, ("scale_shift_table",))]
+SLOT_IDS = ["sd3_dual_qknorm_pre_only", "sd3_no_qknorm", "pixart"]
+
+
+def _attn_linears(blk):
+    """The adapted Linears in the order of the LoRA slot list: attn to_q, to_k, to_v, to_out.0, then SD3's add_q / add_k /
+    add_v / to_add_out and attn2's projections, or PixArt's attn2 projections."""
+    if hasattr(blk, "attn1"):
+        return [lin for a in (blk.attn1, blk.attn2) for lin in (a.to_q, a.to_k, a.to_v, a.to_out[0])]
+    a, b = blk.attn, getattr(blk, "attn2", None)
+    lins = [a.to_q, a.to_k, a.to_v, a.to_out[0], a.add_q_proj, a.add_k_proj, a.add_v_proj, getattr(a, "to_add_out", None)]
+    return lins + ([b.to_q, b.to_k, b.to_v, b.to_out[0]] if b is not None else [None] * 4)
+
+
+@pytest.mark.parametrize("cls,tiny,autograd", SLOT_CASES, ids=SLOT_IDS)
+def test_full_finetune_slots_name_every_block_parameter_once(cls, tiny, autograd):
+    """The full fine-tune slot list of each block holds every block parameter exactly once, outside the modulation path
+    that torch autograd differentiates: a parameter left out would silently get no gradient."""
+    m = cls(**tiny).enable_full_finetune()
+    for blk in m.transformer_blocks:
+        slots = [t for t in blk.block_slots() if t is not None]
+        names = {id(p): n for n, p in blk.named_parameters()}
+        assert len({id(t) for t in slots}) == len(slots), "a parameter sits in two slots"
+        assert all(id(t) in names for t in slots)
+        assert sorted(names[id(t)] for t in slots) == sorted(n for n in names.values() if not n.startswith(autograd))
+
+
+@pytest.mark.parametrize("cls,tiny,autograd", SLOT_CASES, ids=SLOT_IDS)
+def test_lora_slots_and_the_full_finetune_slots_that_replace_them(cls, tiny, autograd):
+    """LoRA slots: the (A, B) of the attention projections in schedule order.  Full fine-tune puts each Linear's (weight,
+    bias) in that Linear's LoRA slots."""
+    m = cls(**tiny)
+    for blk in m.transformer_blocks:
+        for lin in _attn_linears(blk):
+            if lin is not None:
+                lin.add_lora(4, 4.0)
+    for blk in m.transformer_blocks:
+        lins = _attn_linears(blk)
+        lora = blk.block_slots()
+        assert len(lora) == 2 * len(lins) and all(x is y for x, y in zip(lora, [t for lin in lins for t in (
+            lin.lora_tensors() if lin is not None else (None, None))]))
+        blk._full_ft = True
+        full = blk.block_slots()
+        for k, lin in enumerate(lins):
+            w, b = (lin.weight, lin.bias) if lin is not None else (None, None)
+            assert full[2 * k] is w and full[2 * k + 1] is b, k

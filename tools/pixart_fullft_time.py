@@ -78,7 +78,6 @@ def make_batch():
 
 def padded_wgrad_share(step_fn):
     """One full fine-tune step with the padded-layout weight gradients bracketed by CUDA events: (their ms, step ms)."""
-    from simpletuner_b200.pixart import fullft
     spans = []
     real_wgrad, real_sel = ops.wgrad_full, torch.Tensor.index_select
 
@@ -101,12 +100,12 @@ def padded_wgrad_share(step_fn):
         spans.append((e0, e1))
         return out
 
-    fullft.ops.wgrad_full = wgrad
+    ops.wgrad_full = wgrad
     torch.Tensor.index_select = sel
     try:
         ms = events(step_fn, 1)
     finally:
-        fullft.ops.wgrad_full = real_wgrad
+        ops.wgrad_full = real_wgrad
         torch.Tensor.index_select = real_sel
     return sum(a.elapsed_time(b) for a, b in spans), ms, len(spans)
 
