@@ -296,20 +296,20 @@ int stb_colsum2(const void* dy, long long dy_b, long long dy_s, const void* z, l
                 float* dot, int B, int S, int D, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * LoRA weight gradients: out[r, n] += alpha * sum_m L[m, r] * Rm[m, n]   (fp32 out, R in 16..64)
+ * LoRA weight gradients: out[r, n] += alpha * sum_m L[m, r] * Rm[m, n]   (fp32 out [R, N])
  *   dA = s * (dY B)^T X   (L = dY B [M, r], Rm = X  [M, K])
  *   dB^T = s * (X A^T)^T dY (L = X A^T [M, r], Rm = dY [M, N])
  * Autograd of peft lora.Linear (reference common.py:1094-1117).
+ * R is a multiple of 8 up to 128 and N a multiple of 8; L and Rm are 16-byte aligned with row strides (and, when B > 1,
+ * batch strides) that are multiples of 8 elements.  Every (batch, row-split) CTA writes its partial [R, N] into
+ * `workspace` (fp32, at least stb_skinny_tn_workspace(B, S, R, N) elements) with plain stores and a second kernel adds
+ * the slabs to `out` in index order, so the result is the same bit for bit from run to run.  Anything else, a NULL or
+ * short workspace included, returns STB_ERR_ARG before any launch.
  * ------------------------------------------------------------------------------------------- */
-int stb_skinny_tn(const void* L, long long l_b, long long l_s, const void* Rm, long long r_b, long long r_s,
-                  float* out, int B, int S, int R, int N, float alpha, void* stream);
-/* Run-to-run reproducible variant: every (batch, row-split) CTA writes its partial [R, N] into `workspace` (fp32,
- * stb_skinny_tn_workspace(B, S, R, N) elements) with plain stores and a second kernel adds the slabs to `out` in index order —
- * no floating-point atomics.  workspace == NULL is stb_skinny_tn. */
 long long stb_skinny_tn_workspace(int B, int S, int R, int N);
-int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm, long long r_b, long long r_s,
-                     float* out, int B, int S, int R, int N, float alpha, float* workspace, long long workspace_elems,
-                     void* stream);
+int stb_skinny_tn(const void* L, long long l_b, long long l_s, const void* Rm, long long r_b, long long r_s,
+                  float* out, int B, int S, int R, int N, float alpha, float* workspace, long long workspace_elems,
+                  void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * VAE latent encode (diffusers AutoencoderKL.encode as called at reference common.py:2766-2772 from

@@ -140,8 +140,7 @@ SYMBOLS = {
     "stb_dropout_accum": (_I, [_P, _P, _LL, _LL, _I, _I, _I, _I, _F, C.c_uint, C.c_uint, _P]),
     "stb_wgrad_full": (_I, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _I, _I, _I, _I, _F, _I, _P]),
     "stb_colsum2": (_I, [_P, _LL, _LL, _P, _LL, _LL, _P, _P, _I, _I, _I, _P]),
-    "stb_skinny_tn": (_I, [_P, _LL, _LL, _P, _LL, _LL, _P, _I, _I, _I, _I, _F, _P]),
-    "stb_skinny_tn_ws": (_I, [_P, _LL, _LL, _P, _LL, _LL, _P, _I, _I, _I, _I, _F, _P, _LL, _P]),
+    "stb_skinny_tn": (_I, [_P, _LL, _LL, _P, _LL, _LL, _P, _I, _I, _I, _I, _F, _P, _LL, _P]),
     "stb_skinny_tn_workspace": (_LL, [_I, _I, _I, _I]),
     "stb_conv3x3_nhwc": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "stb_conv_in_3ch": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),

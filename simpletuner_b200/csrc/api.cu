@@ -905,66 +905,37 @@ long long stb_skinny_tn_workspace(int B, int S, int R, int N) {
 }
 
 int stb_skinny_tn(const void* L, long long l_b, long long l_s, const void* Rm, long long r_b, long long r_s,
-                  float* out, int B, int S, int R, int N, float alpha, void* stream) {
-  return stb_skinny_tn_ws(L, l_b, l_s, Rm, r_b, r_s, out, B, S, R, N, alpha, nullptr, 0, stream);
-}
-
-int stb_skinny_tn_ws(const void* L, long long l_b, long long l_s, const void* Rm, long long r_b, long long r_s,
-                     float* out, int B, int S, int R, int N, float alpha, float* workspace, long long workspace_elems,
-                     void* stream) {
+                  float* out, int B, int S, int R, int N, float alpha, float* workspace, long long workspace_elems,
+                  void* stream) {
   if (int r = check_device()) return r;
-  if (N & 1) return fail(STB_ERR_ARG, "N must be even");
+  if (!L || !Rm || !out || B < 1 || S < 1 || R < 8 || R > 128 || (R & 7) || N < 8 || (N & 7))
+    return fail(STB_ERR_ARG, "skinny_tn: R must be a multiple of 8 up to 128 and N a positive multiple of 8");
+  if (!aligned16(L) || !aligned16(Rm) || (l_s & 7) || (r_s & 7) || (B > 1 && ((l_b & 7) || (r_b & 7))))
+    return fail(STB_ERR_ARG, "skinny_tn: L and Rm must be 16-byte aligned with strides multiple of 8 elements");
+  int spb, rows;
+  skinny_split(B, S, N, rows, spb);
+  if (!workspace || workspace_elems < (long long)spb * B * R * N)
+    return fail(STB_ERR_ARG, "skinny_tn: workspace missing or smaller than stb_skinny_tn_workspace");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // tensor-core path: both operands TMA-able (16-byte aligned rows), rank block <= 128
-  if (R % 8 == 0 && R <= 128 && N % 8 == 0 && aligned16(L) && aligned16(Rm) && !(l_s & 7) && !(r_s & 7) &&
-      (B == 1 || (!(l_b & 7) && !(r_b & 7)))) {
-    stb::WgradMaps maps;
-    if (int r = make_token_map(&maps.a, Rm, N, S, B, r_s, r_b, 64)) return r;
-    if (int r = make_token_map(&maps.b, L, R, S, B, l_s, l_b, 64)) return r;
-    int spb, rows;
-    skinny_split(B, S, N, rows, spb);
-    if (workspace && workspace_elems < (long long)spb * B * R * N)
-      return fail(STB_ERR_ARG, "skinny_tn workspace too small (stb_skinny_tn_workspace)");
-    stb::WgradParams p{};
-    p.N = N;
-    p.K = R;
-    p.chunks = (S + 63) / 64;
-    // spb splits of `rows` tokens per batch; split y is batch y / spb, slab y of the workspace
-    p.splits = spb * B;
-    p.splits_per_group = spb;
-    p.kb_per_group = p.chunks;
-    p.kb_per_split = rows / 64;
-    p.alpha = alpha;
-    p.partial = workspace;
-    p.out_f32 = out;
-    if (int r = R <= 64 ? launch_wgrad<64, stb::WGRAD_OUT_F32_RN>(maps, p, st) : launch_wgrad<128, stb::WGRAD_OUT_F32_RN>(maps, p, st))
-      return r;
-    if (workspace) {
-      const long long n = (long long)R * N;
-      stb::wgrad_reduce_slabs_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, (long long)num_sms() * 8), 256, 0, st>>>(
-          workspace, out, spb * B, n, alpha);
-      STB_LAUNCH_CHECK("wgrad_reduce_slabs");
-    }
-    return 0;
-  }
-  if (workspace) return fail(STB_ERR_UNSUPPORTED, "deterministic skinny_tn needs the tensor-core path (R % 8 == 0, R <= 128, N % 8 == 0, 16-byte aligned operands)");
-  const long long M = (long long)B * S;
-  const int col_blocks = (N / 2 + 255) / 256;
-  // enough row chunks to fill the machine ~4x
-  int chunks = std::max(1, (num_sms() * 4) / col_blocks);
-  long long mchunk = ((M + chunks - 1) / chunks + 63) / 64 * 64;
-  chunks = (int)((M + mchunk - 1) / mchunk);
-  dim3 grid(col_blocks, chunks);
-  auto LL = static_cast<const __nv_bfloat16*>(L);
-  auto RR = static_cast<const __nv_bfloat16*>(Rm);
-  switch (R) {
-    case 16: stb::skinny_tn_kernel<16><<<grid, 256, 0, st>>>(LL, l_b, l_s, RR, r_b, r_s, out, B, S, N, alpha, (int)mchunk); break;
-    case 32: stb::skinny_tn_kernel<32><<<grid, 256, 0, st>>>(LL, l_b, l_s, RR, r_b, r_s, out, B, S, N, alpha, (int)mchunk); break;
-    case 48: stb::skinny_tn_kernel<48><<<grid, 256, 0, st>>>(LL, l_b, l_s, RR, r_b, r_s, out, B, S, N, alpha, (int)mchunk); break;
-    case 64: stb::skinny_tn_kernel<64><<<grid, 256, 0, st>>>(LL, l_b, l_s, RR, r_b, r_s, out, B, S, N, alpha, (int)mchunk); break;
-    default: return fail(STB_ERR_UNSUPPORTED, "LoRA rank block R=%d not supported (16/32/48/64)", R);
-  }
-  STB_LAUNCH_CHECK("skinny_tn");
+  stb::WgradMaps maps;
+  if (int r = make_token_map(&maps.a, Rm, N, S, B, r_s, r_b, 64)) return r;
+  if (int r = make_token_map(&maps.b, L, R, S, B, l_s, l_b, 64)) return r;
+  stb::WgradParams p{};
+  p.N = N;
+  p.K = R;
+  p.chunks = (S + 63) / 64;
+  // spb splits of `rows` tokens per batch; split y is batch y / spb, slab y of the workspace
+  p.splits = spb * B;
+  p.splits_per_group = spb;
+  p.kb_per_group = p.chunks;
+  p.kb_per_split = rows / 64;
+  p.partial = workspace;
+  if (int r = R <= 64 ? launch_wgrad<64, stb::WGRAD_OUT_F32_RN>(maps, p, st) : launch_wgrad<128, stb::WGRAD_OUT_F32_RN>(maps, p, st))
+    return r;
+  const long long n = (long long)R * N;
+  stb::wgrad_reduce_slabs_kernel<<<(unsigned)std::min<long long>((n + 255) / 256, (long long)num_sms() * 8), 256, 0, st>>>(
+      workspace, out, spb * B, n, alpha);
+  STB_LAUNCH_CHECK("wgrad_reduce_slabs");
   return 0;
 }
 

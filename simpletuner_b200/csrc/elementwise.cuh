@@ -695,65 +695,6 @@ target_mse_loss_kernel(const __nv_bfloat16* __restrict__ pred_packed, const __nv
 }
 
 // ------------------------------------------------------------------------------------------------
-// LoRA weight gradients (rank r <= 64), reference: autograd through peft lora.Linear
-//   y = x W^T + s * (x A^T) B^T   =>   dA = s * (dY B)^T x ,  dB = s * dY^T (x A^T)
-// Generic "skinny" product:  Out[r, n] (+)= alpha * sum_m  L[m, r] * Rm[m, n]
-// with L = [M, R] (R <= 64, contiguous rows), Rm = [M, N].  Split over M across CTAs, fp32 atomics.
-// Each CTA: 256 threads cover 256*VEC columns of N for a chunk of MCHUNK rows.
-// ------------------------------------------------------------------------------------------------
-template <int R>
-__global__ void __launch_bounds__(256)
-skinny_tn_kernel(const __nv_bfloat16* __restrict__ L, long long l_b, long long l_s,
-                 const __nv_bfloat16* __restrict__ Rm, long long r_b, long long r_s,
-                 float* __restrict__ out /*[R, N] fp32*/, int B, int S, int N, float alpha, int mchunk) {
-  __shared__ __nv_bfloat16 sL[64][R];  // 64 rows of L at a time
-  const int n = (blockIdx.x * 256 + threadIdx.x) * 2;
-  const long long m0 = (long long)blockIdx.y * mchunk;
-  const long long Mtot = (long long)B * S;
-  const long long m1 = min(Mtot, m0 + mchunk);
-  float acc0[R], acc1[R];
-#pragma unroll
-  for (int r = 0; r < R; ++r) acc0[r] = 0.f, acc1[r] = 0.f;
-  for (long long mb = m0; mb < m1; mb += 64) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < 64 * R; i += 256) {
-      const int rr = i / R, cc = i - rr * R;
-      const long long m = mb + rr;
-      __nv_bfloat16 v = __float2bfloat16(0.f);
-      if (m < m1) {
-        const long long bb = m / S, ss = m - bb * S;
-        v = L[bb * l_b + ss * l_s + cc];
-      }
-      sL[rr][cc] = v;
-    }
-    __syncthreads();
-    if (n < N) {
-      const long long left = m1 - mb;
-      const int rows = left < 64 ? int(left) : 64;
-      for (int rr = 0; rr < rows; ++rr) {
-        const long long m = mb + rr;
-        const long long bb = m / S, ss = m - bb * S;
-        const uint32_t u = *reinterpret_cast<const uint32_t*>(Rm + bb * r_b + ss * r_s + n);
-        const float x0 = bf16_lo(u), x1 = bf16_hi(u);
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-          const float lv = __bfloat162float(sL[rr][r]);
-          acc0[r] += lv * x0;
-          acc1[r] += lv * x1;
-        }
-      }
-    }
-  }
-  if (n < N) {
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-      atomicAdd(out + (long long)r * N + n, alpha * acc0[r]);
-      if (n + 1 < N) atomicAdd(out + (long long)r * N + n + 1, alpha * acc1[r]);
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // y[b, s, :] = gate[b, :] * x[b, s, :]   (backward of `gate * linear(...)`, flux/transformer.py:464,
 // 584, 652 — the incoming gradient is scaled by the adaLN gate before the dgrad GEMM).
 // ------------------------------------------------------------------------------------------------

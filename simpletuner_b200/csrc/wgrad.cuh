@@ -7,9 +7,9 @@
 //                      past R are TMA zeros):
 //                        dA = (dY B)^T X      -> L = dY B [M, r],   Rm = X  [M, K]
 //                        dB^T = (X A^T)^T dY  -> L = X A^T [M, r],  Rm = dY [M, N]
-//                      Each token split writes a slab of `partial` with plain stores (summed in slab order by
-//                      wgrad_reduce_slabs_kernel, run-to-run reproducible), or, with `partial` null, adds alpha * D
-//                      into `out_f32` with fp32 atomics.  HBM-bound (reads Rm once).
+//                      Each token split writes its D to a slab of `partial` with plain stores;
+//                      wgrad_reduce_slabs_kernel then adds alpha * the slabs to out in slab order, so the result is
+//                      the same bit for bit from run to run.  HBM-bound (reads Rm once).
 //   WGRAD_OUT_BF16_NK  out[n, k] (bf16 [N, K]) = alpha * D (+ out[n, k]): full-rank weight gradients (full fine-tune,
 //                      BASELINE config 3; reference trainer.py:7126 `accelerator.backward`, SD3 blocks
 //                      sd3/transformer.py:145-241), A = dY and B = X.  2 * M * N * K flops (M = B*S tokens), the same
@@ -38,9 +38,8 @@ struct WgradParams {
   // g0 = (y / splits_per_group) * kb_per_group + (y % splits_per_group) * kb_per_split.  Every split is non-empty.
   int splits, splits_per_group, kb_per_group, kb_per_split;
   int col_tiles;        // ceil(K / BN)
-  float alpha;
-  float* partial;       // WGRAD_OUT_F32_RN: [splits][R][N] slabs, or nullptr = atomics into out_f32
-  float* out_f32;       // WGRAD_OUT_F32_RN: [R, N]
+  float alpha;          // WGRAD_OUT_BF16_NK (wgrad_reduce_slabs_kernel scales the LoRA slabs)
+  float* partial;       // WGRAD_OUT_F32_RN: [splits][R][N] slabs
   __nv_bfloat16* out;   // WGRAD_OUT_BF16_NK: [N, K], rows out_row_stride apart
   long long out_row_stride;
   int accumulate;       // WGRAD_OUT_BF16_NK, 1: out += (bf16 read-modify-write)
@@ -180,11 +179,7 @@ wgrad_kernel(const __grid_constant__ WgradMaps maps, const WgradParams p) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int r = u.k0 + 8 * i + 2 * (lane & 3) + e;
-              if (r < p.K) {
-                const float v = acc[4 * i + 2 * hh + e];
-                if (p.partial) p.partial[((long long)u.y * p.K + r) * p.N + n] = v;
-                else atomicAdd(p.out_f32 + (long long)r * p.N + n, p.alpha * v);
-              }
+              if (r < p.K) p.partial[((long long)u.y * p.K + r) * p.N + n] = acc[4 * i + 2 * hh + e];
             }
         } else {
           __nv_bfloat16* orow = p.out + (long long)n * p.out_row_stride;

@@ -8,7 +8,6 @@ happens inside libstb200.so.
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Optional, Sequence, Tuple
 
 import torch
@@ -522,22 +521,16 @@ def colsum2(dy, z=None, want_sum: bool = True):
     return sm, dt
 
 
-DETERMINISTIC = os.environ.get("STB_DETERMINISTIC", "1") != "0"
 # per (device, stream) reduction workspace.  A buffer that is outgrown is kept alive, never freed: a CUDA graph captured
 # while it was current still reads and writes it on replay, so its memory must not go back to an allocator pool.
 _ws_cache: dict = {}
 _ws_retired: list = []
 
 
-def set_deterministic(on: bool) -> None:
-    """LoRA weight gradients without floating-point atomics (slab partials + ordered reduction): bit-identical run to run.
-    On by default; off (or STB_DETERMINISTIC=0) accumulates the row splits with fp32 atomics instead."""
-    global DETERMINISTIC
-    DETERMINISTIC = bool(on)
-
-
 def skinny_tn(L, Rm, alpha: float = 1.0, out: Optional[torch.Tensor] = None):
-    """out[r, n] += alpha * sum_m L[m, r] * Rm[m, n].  L [B,S,R] or [M,R]; Rm [B,S,N] or [M,N]; out fp32."""
+    """out[r, n] += alpha * sum_m L[m, r] * Rm[m, n].  L [B,S,R] or [M,R]; Rm [B,S,N] or [M,N]; out fp32.
+    Per-split slabs added in index order: bit-identical from run to run.  R must be a multiple of 8 up to 128, N a
+    multiple of 8, and both operands 16-byte aligned with strides multiple of 8; anything else raises StbError."""
     L3, R3 = _as3d(L), _as3d(Rm)
     _chk(L3, "L"); _chk(R3, "Rm")
     B, S, R = L3.shape
@@ -545,19 +538,15 @@ def skinny_tn(L, Rm, alpha: float = 1.0, out: Optional[torch.Tensor] = None):
     if out is None:
         out = torch.zeros((R, N), device=L.device, dtype=torch.float32)
     assert out.dtype == torch.float32 and out.is_contiguous()
-    if DETERMINISTIC and R % 8 == 0 and R <= 128 and N % 8 == 0:
-        need = int(_lib.lib().stb_skinny_tn_workspace(B, S, R, N))
-        key = (L.device.index, _stream())
-        ws = _ws_cache.get(key)
-        if ws is None or ws.numel() < need:
-            if ws is not None:
-                _ws_retired.append(ws)
-            ws = _ws_cache[key] = torch.empty((need,), device=L.device, dtype=torch.float32)
-        check(_lib.lib().stb_skinny_tn_ws(L3.data_ptr(), L3.stride(0), L3.stride(1), R3.data_ptr(), R3.stride(0), R3.stride(1),
-                                          out.data_ptr(), B, S, R, N, alpha, ws.data_ptr(), ws.numel(), _stream()))
-        return out
-    check(_lib.lib().stb_skinny_tn(L3.data_ptr(), L3.stride(0), L3.stride(1), R3.data_ptr(), R3.stride(0),
-                                   R3.stride(1), out.data_ptr(), B, S, R, N, alpha, _stream()))
+    need = int(_lib.lib().stb_skinny_tn_workspace(B, S, R, N))
+    key = (L.device.index, _stream())
+    ws = _ws_cache.get(key)
+    if ws is None or ws.numel() < need:
+        if ws is not None:
+            _ws_retired.append(ws)
+        ws = _ws_cache[key] = torch.empty((need,), device=L.device, dtype=torch.float32)
+    check(_lib.lib().stb_skinny_tn(L3.data_ptr(), L3.stride(0), L3.stride(1), R3.data_ptr(), R3.stride(0), R3.stride(1),
+                                   out.data_ptr(), B, S, R, N, alpha, ws.data_ptr(), ws.numel(), _stream()))
     return out
 
 

@@ -1128,41 +1128,29 @@ def check_flow(B=2, Cc=16, Hh=32, Ww=48, layout=0, loss_type="l2", grad_scale=1.
                        loss_type, hc, None, grad_scale, extra)
 
 
-class _deterministic:
-    """Select the skinny_tn reduction for a block: True = slab workspace + ordered reduce, False = fp32 atomics,
-    None = leave the process setting alone.  The previous setting is restored on exit."""
-
-    def __init__(self, on):
-        self.on = on
-
-    def __enter__(self):
-        self.prev = ops.DETERMINISTIC
-        if self.on is not None:
-            ops.set_deterministic(self.on)
-
-    def __exit__(self, *exc):
-        ops.set_deterministic(self.prev)
-
-
-def check_skinny(B=2, S=300, R=16, N=3072, deterministic=None, exact=False, accumulate=False, alpha=0.5):
-    """out[r, n] += alpha sum_m L[m, r] Rm[m, n] (fp32).  deterministic: True = slab workspace + ordered reduce, False =
-    fp32 atomics; R or N not a multiple of 8 takes the CUDA-core kernel.  accumulate: out starts non-zero (N(0, 1), or
-    integers x 2^-4 with exact inputs, so that atomics in any order stay exact).  A non-power-of-two alpha (slab path
-    only with exact inputs) accepts alpha acc + out rounded once (FMA) or twice."""
-    L = _gen(B, S, R, seed=1, exact="int" if exact else None)
-    Rm = _gen(B, S, N, seed=2, exact="frac" if exact else None)
+def check_skinny(B=2, S=300, R=16, N=3072, exact=False, accumulate=False, alpha=0.5, view=False):
+    """out[r, n] += alpha sum_m L[m, r] Rm[m, n] (fp32), per-split slabs added in index order.  accumulate: out starts
+    non-zero (N(0, 1), or integers x 2^-4 with exact inputs, so that every partial sum stays exact).  A non-power-of-two
+    alpha (with exact inputs) accepts alpha acc + out rounded once (FMA) or twice.  view: L and Rm are token and column
+    windows of wider buffers, as _lora_grads passes one member's rank slice of a fused rank block and its column range of
+    the fused output; the values around the windows must not reach out."""
+    if view:
+        L = _gen(B, S + 3, R + 24, seed=1, exact="int" if exact else None)[:, 2:S + 2, 8:8 + R]
+        Rm = _gen(B, S + 5, N + 40, seed=2, exact="frac" if exact else None)[:, 3:S + 3, 16:16 + N]
+    else:
+        L = _gen(B, S, R, seed=1, exact="int" if exact else None)
+        Rm = _gen(B, S, N, seed=2, exact="frac" if exact else None)
     out0 = None
     if accumulate:
         g = torch.Generator(device="cpu").manual_seed(3)
         out0 = (torch.randint(-64, 65, (R, N), generator=g).float() / 16 if exact else torch.randn(R, N, generator=g)).to(DEV)
-    with _deterministic(deterministic):
-        out = ops.skinny_tn(L, Rm, alpha=alpha, out=out0.clone() if accumulate else None)
-        torch.cuda.synchronize()
+    out = ops.skinny_tn(L, Rm, alpha=alpha, out=out0.clone() if accumulate else None)
+    torch.cuda.synchronize()
     L2, R2 = L.double().reshape(-1, R), Rm.double().reshape(-1, N)
     acc64, mag = L2.t() @ R2, L2.abs().t() @ R2.abs()
     a32 = _f32(alpha)
     base = out0.double() if accumulate else torch.zeros_like(acc64)
-    name = f"skinny_tn_B{B}_S{S}_R{R}_N{N}_det{deterministic}" + ("_accum" if accumulate else "") + ("_exact" if exact else "")
+    name = f"skinny_tn_B{B}_S{S}_R{R}_N{N}" + ("_view" if view else "") + ("_accum" if accumulate else "") + ("_exact" if exact else "")
     if not exact:
         r = _report_acc("out", out, base + a32 * acc64, abs(a32) * mag + base.abs(), B * S, GEMM_RTOL_F32)
         return _combine(name, [r])
@@ -1176,13 +1164,12 @@ def check_skinny(B=2, S=300, R=16, N=3072, deterministic=None, exact=False, accu
 
 
 def check_skinny_repeatable(B=4, S=4608, R=48, N=9216):
-    """The slab-workspace LoRA weight gradient is bit-identical from run to run."""
+    """The LoRA weight gradient is bit-identical from run to run."""
     L = _rand(B, S, R, seed=1)
     Rm = _rand(B, S, N, seed=2)
-    with _deterministic(True):
-        a = ops.skinny_tn(L, Rm, alpha=0.5)
-        b = ops.skinny_tn(L, Rm, alpha=0.5)
-        torch.cuda.synchronize()
+    a = ops.skinny_tn(L, Rm, alpha=0.5)
+    b = ops.skinny_tn(L, Rm, alpha=0.5)
+    torch.cuda.synchronize()
     same = bool(torch.equal(a, b))
     return {"name": f"skinny_tn_repeatable_B{B}_S{S}_R{R}_N{N}", "ok": same and bool(torch.isfinite(a).all().item()),
             "max_diff": float((a - b).abs().max().item())}
@@ -1254,7 +1241,6 @@ CHECKS = {
     "skinny_r48": lambda: check_skinny(R=48, N=4096),
     "skinny_flux": lambda: check_skinny(B=4, S=4608, R=48, N=9216),
     "skinny_ragged": lambda: check_skinny(B=3, S=333, R=16, N=200),
-    "skinny_cuda_core_path": lambda: check_skinny(B=2, S=100, R=16, N=250),
 }
 # BASELINE-geometry kernel shapes (VERDICT r1 weak #1): the deepest K of the Flux step (fc2 / single-block proj_out, K = 12288 and
 # the 2-segment 3072 + 12288 `cat([attn, mlp]) @ W_out`), and the attention backward at the full joint sequence
@@ -2146,14 +2132,23 @@ CHECKS.update({
     "qk_rmsnorm_dw_hd64": lambda: check_qk_rmsnorm_dw(HD=64),
     "qk_rmsnorm_dw_hd64_norope": lambda: check_qk_rmsnorm_dw(HD=64, rope=False),
 })
-# skinny_tn tensor-core path on both reductions (slab workspace / fp32 atomics) and both kernels (rank block 64 / 128)
-for _r in (8, 64, 72, 128):
-    for _det in (True, False):
-        CHECKS[f"skinny_r{_r}_" + ("ws" if _det else "atomic")] = _case(check_skinny, B=2, S=700, R=_r, N=1536,
-                                                                         deterministic=_det)
-for _det in (True, False):   # several batches, S not a multiple of the row split
-    CHECKS["skinny_b3_split_tail_" + ("ws" if _det else "atomic")] = _case(check_skinny, B=3, S=1000, R=48, N=1024,
-                                                                          deterministic=_det)
+# skinny_tn on both kernels (rank block 64 / 128, the last padded rank below each edge), several batches whose S is not
+# a multiple of the row split (b3_split_tail), one token, a sequence shorter than one 64-token chunk, N below one 128-row
+# tile, 16 short text-length batches, the widest Flux projection, and strided windows of wider buffers; each into a zero
+# and a non-zero out, against fp64 and with exact inputs
+for _n, _kw in (("r8", dict(B=2, S=700, R=8, N=1536)), ("r56", dict(B=2, S=700, R=56, N=1536)),
+                ("r64", dict(B=2, S=700, R=64, N=1536)), ("r72", dict(B=2, S=700, R=72, N=1536)),
+                ("r120", dict(B=2, S=700, R=120, N=1536)), ("r128", dict(B=2, S=700, R=128, N=1536)),
+                ("b3_split_tail", dict(B=3, S=1000, R=48, N=1024)), ("s1", dict(B=3, S=1, R=16, N=512)),
+                ("s63", dict(B=2, S=63, R=8, N=1024)), ("n72", dict(B=2, S=300, R=16, N=72)),
+                ("b16_s77", dict(B=16, S=77, R=32, N=3072)), ("n12288", dict(B=1, S=4608, R=16, N=12288)),
+                ("view_r16", dict(B=2, S=300, R=16, N=3072, view=True)),
+                ("view_b3_r48", dict(B=3, S=333, R=48, N=1024, view=True)),
+                ("view_r128", dict(B=2, S=700, R=128, N=1536, view=True))):
+    for _acc in (False, True):
+        for _x in (False, True):
+            CHECKS[f"skinny_{_n}_ws" + ("_accum" if _acc else "") + ("_exact" if _x else "")] = _case(
+                check_skinny, **_kw, accumulate=_acc, exact=_x)
 
 
 # --------------------------------------------------------------------------------------------- run-to-run determinism
@@ -2218,11 +2213,8 @@ for _x in (False, True):
                                                       tile=(2, 128), exact=_x)
     CHECKS[f"gemm_odd_n65_bn256{_s}"] = _case(check_gemm, 200, 65, 200, B=2, bias=True, tile=(0, 256), exact=_x)
 
-    # skinny_tn into a non-zero out: slab workspace, fp32 atomics, CUDA-core kernel (N % 8 != 0)
-    CHECKS[f"skinny_ws_accum{_s}"] = _case(check_skinny, B=2, S=700, R=48, N=1536, deterministic=True, accumulate=True, exact=_x)
-    CHECKS[f"skinny_atomic_accum{_s}"] = _case(check_skinny, B=2, S=700, R=48, N=1536, deterministic=False, accumulate=True,
-                                                exact=_x)
-    CHECKS[f"skinny_cuda_core_accum{_s}"] = _case(check_skinny, B=2, S=100, R=16, N=250, accumulate=True, exact=_x)
+    # skinny_tn into a non-zero out
+    CHECKS[f"skinny_ws_accum{_s}"] = _case(check_skinny, B=2, S=700, R=48, N=1536, accumulate=True, exact=_x)
     # wgrad_full with N % 128 != 0 at both tile widths (K <= 128 forces 256; 520 gives 128 on 132 SMs)
     for _n in (200, 136):
         for _k in (120, 520):
@@ -2238,10 +2230,7 @@ CHECKS.update({
     "skinny_exact": lambda: check_skinny(exact=True),
     "skinny_flux_exact": lambda: check_skinny(B=4, S=4608, R=48, N=9216, exact=True),
     "skinny_ragged_exact": lambda: check_skinny(B=3, S=333, R=16, N=200, exact=True),
-    "skinny_r64_ws_exact": lambda: check_skinny(B=2, S=700, R=64, N=1536, deterministic=True, exact=True),
-    "skinny_r128_atomic_exact": lambda: check_skinny(B=2, S=700, R=128, N=1536, deterministic=False, exact=True),
-    "skinny_ws_accum_alpha0.3_exact": lambda: check_skinny(B=2, S=700, R=48, N=1536, deterministic=True, accumulate=True,
-                                                           alpha=0.3, exact=True),
+    "skinny_ws_accum_alpha0.3_exact": lambda: check_skinny(B=2, S=700, R=48, N=1536, accumulate=True, alpha=0.3, exact=True),
     "wgrad_full_basic_exact": lambda: check_wgrad_full(exact=True),
     "wgrad_full_strided_accum_exact": lambda: check_wgrad_full(B=3, S=231, N=384, K=200, strided=True, accumulate=True,
                                                                alpha=0.5, exact=True),

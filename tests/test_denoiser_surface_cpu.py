@@ -278,6 +278,6 @@ def test_to_and_load_state_dict_reset_every_cached_plan(kind, build):
 
 def test_denoiser_code_reads_no_environment_switch():
     pkg = ROOT / "simpletuner_b200"
-    for sub in ("flux", "sd3", "pixart", "qwen_image", "chroma"):
-        for path in (pkg / sub).glob("*.py"):
-            assert "environ" not in path.read_text(), path
+    paths = [pkg / "ops.py"] + [p for sub in ("flux", "sd3", "pixart", "qwen_image", "chroma") for p in (pkg / sub).glob("*.py")]
+    for path in paths:
+        assert "environ" not in path.read_text(), path

@@ -113,11 +113,9 @@ def test_unsupported_lora_targets_raise():
         w._denoiser().add_adapter(rank=8, target_modules=["norm1.linear"])
 
 
-def test_deterministic_mode_gives_bit_identical_lora_gradients():
-    """`ops.set_deterministic(True)` (the default): the LoRA weight-gradient kernel writes per-split slabs and a
-    second kernel adds them in index order instead of using fp32 atomics — two runs of the same step agree bit for bit, and
-    stay within the parity tolerances."""
-    from simpletuner_b200 import ops
+def test_two_runs_give_bit_identical_lora_gradients():
+    """The LoRA weight-gradient kernel writes per-split slabs and a second kernel adds them in index order, so two runs of
+    the same step agree bit for bit, and stay within the parity tolerances."""
 
     def grads():
         from oracle import flux_oracle as O
@@ -132,15 +130,6 @@ def test_deterministic_mode_gives_bit_identical_lora_gradients():
         torch.cuda.synchronize()
         return {n: p.grad.clone() for n, p in w._denoiser().named_parameters() if p.grad is not None}
 
-    prev = ops.DETERMINISTIC
-    try:
-        ops.set_deterministic(True)
-        a, b = grads(), grads()
-        ops.set_deterministic(False)
-        c = grads()      # atomics path: same values up to fp32 summation order
-    finally:
-        ops.set_deterministic(prev)
+    a, b = grads(), grads()
     assert len(a) == 22 and all(torch.equal(a[k], b[k]) for k in a)
-    for k in a:
-        assert torch.allclose(a[k].float(), c[k].float(), rtol=2e-2, atol=1e-6 + 2e-2 * float(c[k].float().abs().max())), k
     _assert(FP.run_parity(cfg=FP.small_config(layers=1, single=1), seed=21))
