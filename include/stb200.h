@@ -316,13 +316,21 @@ int stb_skinny_tn(const void* L, long long l_b, long long l_s, const void* Rm, l
  * caching/vae.py:1311; sampling caching/vae.py:1337; scaling foundation_mixins.py:68-81).
  * Activations are NHWC bf16; every 3x3 conv is a wgmma implicit GEMM (9 shifted K-segments, the halo
  * is zero-filled by TMA); 1x1 convs / attention projections are stb_gemm_bf16 over pixels.
- *   stb_conv3x3_nhwc : out[B,Ho,Wo,Co] = conv3x3(x[B,H,W,Ci]; w[Co, 9*Ci] tap-major (dy,dx,ci)) + bias (+ res)
+ *   stb_conv3x3_nhwc : out[B,Ho,Wo,Co] = conv3x3(x[B,H,W,Ci]; w[Co, 9*Cp] tap-major (dy,dx,ci)) + bias (+ res)
  *                      stride 1: padding 1;  stride 2: F.pad(x,(0,1,0,1)) then stride-2 (Downsample2D)
+ *                      Ci and Co multiples of 8; Cp = Ci rounded up to a multiple of 64, each tap's columns
+ *                      [Ci, Cp) of w zero (Cp = Ci when Ci % 64 == 0)
  *   stb_conv_in_3ch  : conv_in on the NCHW pixel tensor [B,3,H,W] (w OIHW [C,3,3,3]) -> NHWC [B,H,W,C]
  *   stb_groupnorm_nhwc : GroupNorm(G, eps, affine) (+ SiLU) over NHWC; stats = fp32 scratch [B*G*2]
  *   stb_softmax_rows : in-place softmax(scale * s) over rows of the mid-block attention scores (scale > 0)
  *   stb_gaussian_sample_scale : z = (mean + exp(.5 clamp(logvar,-30,20)) * eps - shift) * scale, NHWC moments
  *                      [B,h*w,2L] + NCHW eps [B,L,h,w] -> NCHW latents [B,L,h,w]
+ *   stb_gaussian_sample_channel_norm : the same sample, then bf16(bf16(z - shift[c]) * inv_std[c]) with bf16 [L]
+ *                      vectors (Qwen-Image latents_mean and 1 / latents_std)
+ *   stb_channel_rmsnorm_nhwc : Wan 2.1 channel RMS norm over the contiguous rows of x [rows, C]:
+ *                      F.normalize(x, dim=C, eps) * sqrt(C) * gamma (+ bias, may be NULL) (+ SiLU); C a multiple of 8
+ *                      in [8, 512], finite eps >= 0, 16-byte aligned pointers; the eager module's bf16 rounding after
+ *                      every op (csrc/vae.cuh)
  * ------------------------------------------------------------------------------------------- */
 int stb_conv3x3_nhwc(const void* x, const void* w, const void* bias, const void* res, void* out, int B, int H, int W,
                      int C_in, int C_out, int stride, void* stream);
@@ -333,6 +341,10 @@ int stb_groupnorm_nhwc(const void* x, const void* gamma, const void* beta, void*
 int stb_softmax_rows(void* s, long long row_stride, int rows, int cols, float scale, void* stream);
 int stb_gaussian_sample_scale(const void* moments, const void* eps, void* out, int B, int L, int hw, float shift,
                               float scale, int has_shift, void* stream);
+int stb_gaussian_sample_channel_norm(const void* moments, const void* eps, void* out, int B, int L, int hw,
+                                     const void* shift, const void* inv_std, void* stream);
+int stb_channel_rmsnorm_nhwc(const void* x, const void* gamma, const void* bias, void* out, long long rows, int C,
+                             float eps, int silu, void* stream);
 
 #ifdef __cplusplus
 }

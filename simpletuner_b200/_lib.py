@@ -147,6 +147,8 @@ SYMBOLS = {
     "stb_groupnorm_nhwc": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _I, _P]),
     "stb_softmax_rows": (_I, [_P, _LL, _I, _I, _F, _P]),
     "stb_gaussian_sample_scale": (_I, [_P, _P, _P, _I, _I, _I, _F, _F, _I, _P]),
+    "stb_gaussian_sample_channel_norm": (_I, [_P, _P, _P, _I, _I, _I, _P, _P, _P]),
+    "stb_channel_rmsnorm_nhwc": (_I, [_P, _P, _P, _P, _LL, _I, _F, _I, _P]),
 }
 
 _lock = threading.Lock()

@@ -946,6 +946,9 @@ template <int BN>
 static int launch_conv3x3(const void* x, const void* w, const void* bias, const void* res, void* out, int B, int H,
                           int W, int C_in, int C_out, int stride, cudaStream_t st) {
   const int H_out = stride == 1 ? H : H / 2, W_out = stride == 1 ? W : W / 2;
+  // C_in % 64 != 0: each tap's last 64-channel box runs past C_in, TMA zero-fills the activation's tail as it does the
+  // spatial halo, and w holds zeros in the same columns (a tap is C_pad = 64 cblocks wide), so the kernel is unchanged
+  const int cblocks = (C_in + 63) / 64, C_pad = 64 * cblocks;
   stb::GemmMaps maps;
   std::memset(&maps, 0, sizeof maps);
   {
@@ -957,8 +960,8 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
     if (int r = make_map_strided(&maps.a[0], x, 4, d, sb, bx, es)) return r;
   }
   {
-    unsigned long long d[2] = {(unsigned long long)9 * C_in, (unsigned long long)C_out};
-    unsigned long long sb[1] = {(unsigned long long)9 * C_in * 2ull};
+    unsigned long long d[2] = {(unsigned long long)9 * C_pad, (unsigned long long)C_out};
+    unsigned long long sb[1] = {(unsigned long long)9 * C_pad * 2ull};
     unsigned bx[2] = {64, (unsigned)BN};
     if (int r = make_map(&maps.w[0], w, 2, d, sb, bx)) return r;
   }
@@ -968,7 +971,7 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   p.num_batches = B * H_out;
   p.N = C_out;
   p.nseg = 1;
-  p.kblocks[0] = 9 * (C_in / 64);
+  p.kblocks[0] = 9 * cblocks;
   p.D = static_cast<__nv_bfloat16*>(out);
   p.d_batch_stride = (long long)W_out * C_out;
   p.d_row_stride = C_out;
@@ -979,7 +982,7 @@ static int launch_conv3x3(const void* x, const void* w, const void* bias, const 
   p.conv_h_out = H_out;
   p.conv_stride = stride;
   p.conv_pad = stride == 1 ? 1 : 0;
-  p.conv_cblocks = C_in / 64;
+  p.conv_cblocks = cblocks;
   if (res) return launch_gemm_kernel<BN, stb::EPI_ADD_RES, true>(maps, p, st, "conv3x3_nhwc");
   return launch_gemm_kernel<BN, stb::EPI_STORE, true>(maps, p, st, "conv3x3_nhwc");
 }
@@ -989,7 +992,9 @@ extern "C" {
 int stb_conv3x3_nhwc(const void* x, const void* w, const void* bias, const void* res, void* out, int B, int H, int W,
                      int C_in, int C_out, int stride, void* stream) {
   if (int r = check_device()) return r;
-  if (C_in % 64 || C_out % 8) return fail(STB_ERR_ARG, "conv3x3_nhwc needs C_in %% 64 == 0 and C_out %% 8 == 0 (got %d, %d)", C_in, C_out);
+  if (C_in < 8 || C_in % 8 || C_out < 8 || C_out % 8)
+    return fail(STB_ERR_ARG, "conv3x3_nhwc needs C_in and C_out positive multiples of 8 (got %d, %d)", C_in, C_out);
+  if (!x || !w || !out || B < 1 || H < 1 || W < 1) return fail(STB_ERR_ARG, "conv3x3_nhwc: bad arguments");
   if (stride != 1 && stride != 2) return fail(STB_ERR_ARG, "conv3x3_nhwc stride must be 1 or 2");
   if (stride == 2 && ((H | W) & 1)) return fail(STB_ERR_ARG, "stride-2 conv needs even H, W");
   if (!aligned16(x) || !aligned16(w) || !aligned16(out) || (res && !aligned16(res)) || (bias && !aligned16(bias)))
@@ -1072,8 +1077,53 @@ int stb_gaussian_sample_scale(const void* moments, const void* eps, void* out, i
   const long long total = (long long)B * L * hw;
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 8);
   stb::gaussian_sample_scale_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __nv_bfloat16*>(moments), static_cast<const __nv_bfloat16*>(eps), static_cast<__nv_bfloat16*>(out), B, L, hw, shift, scale, has_shift);
+      static_cast<const __nv_bfloat16*>(moments), static_cast<const __nv_bfloat16*>(eps), static_cast<__nv_bfloat16*>(out), B, L, hw, shift, scale, has_shift,
+      nullptr, nullptr);
   STB_LAUNCH_CHECK("gaussian_sample_scale");
+  return 0;
+}
+
+int stb_gaussian_sample_channel_norm(const void* moments, const void* eps, void* out, int B, int L, int hw,
+                                     const void* shift, const void* inv_std, void* stream) {
+  if (int r = check_device()) return r;
+  if (!moments || !eps || !out || !shift || !inv_std || B < 1 || L < 1 || hw < 1)
+    return fail(STB_ERR_ARG, "gaussian_sample_channel_norm: bad arguments");
+  const long long total = (long long)B * L * hw;
+  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)num_sms() * 8);
+  stb::gaussian_sample_scale_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const __nv_bfloat16*>(moments), static_cast<const __nv_bfloat16*>(eps), static_cast<__nv_bfloat16*>(out), B, L, hw, 0.f, 1.f, 1,
+      static_cast<const __nv_bfloat16*>(shift), static_cast<const __nv_bfloat16*>(inv_std));
+  STB_LAUNCH_CHECK("gaussian_sample_channel_norm");
+  return 0;
+}
+
+int stb_channel_rmsnorm_nhwc(const void* x, const void* gamma, const void* bias, void* out, long long rows, int C,
+                             float eps, int silu, void* stream) {
+  if (int r = check_device()) return r;
+  if (!x || !gamma || !out || rows < 1 || !(eps >= 0.f) || std::isinf(eps))
+    return fail(STB_ERR_ARG, "channel_rmsnorm_nhwc: bad arguments (rows >= 1, finite eps >= 0)");
+  if (C < 8 || C > 512 || C % 8) return fail(STB_ERR_ARG, "channel_rmsnorm_nhwc: C must be a multiple of 8 in [8, 512] (got %d)", C);
+  if (!aligned16(x) || !aligned16(out) || !aligned16(gamma) || (bias && !aligned16(bias)))
+    return fail(STB_ERR_ARG, "channel_rmsnorm_nhwc: x, out, gamma and bias must be 16-byte aligned");
+  const int nvec = C / 8;
+  const int tpr = nvec <= 1 ? 1 : nvec <= 2 ? 2 : nvec <= 4 ? 4 : nvec <= 8 ? 8 : nvec <= 16 ? 16 : 32;
+  const long long warps = (rows + 32 / tpr - 1) / (32 / tpr);
+  const int grid = (int)std::min<long long>((warps + 7) / 8, (long long)num_sms() * 16);
+  const float scale = (float)std::sqrt((double)C);
+  auto xp = static_cast<const __nv_bfloat16*>(x);
+  auto gp = static_cast<const __nv_bfloat16*>(gamma);
+  auto bp = static_cast<const __nv_bfloat16*>(bias);
+  auto op = static_cast<__nv_bfloat16*>(out);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  switch (tpr) {
+    case 1: stb::channel_rmsnorm_kernel<1><<<grid, 256, 0, st>>>(xp, gp, bp, op, rows, C, scale, eps, silu); break;
+    case 2: stb::channel_rmsnorm_kernel<2><<<grid, 256, 0, st>>>(xp, gp, bp, op, rows, C, scale, eps, silu); break;
+    case 4: stb::channel_rmsnorm_kernel<4><<<grid, 256, 0, st>>>(xp, gp, bp, op, rows, C, scale, eps, silu); break;
+    case 8: stb::channel_rmsnorm_kernel<8><<<grid, 256, 0, st>>>(xp, gp, bp, op, rows, C, scale, eps, silu); break;
+    case 16: stb::channel_rmsnorm_kernel<16><<<grid, 256, 0, st>>>(xp, gp, bp, op, rows, C, scale, eps, silu); break;
+    default: stb::channel_rmsnorm_kernel<32><<<grid, 256, 0, st>>>(xp, gp, bp, op, rows, C, scale, eps, silu); break;
+  }
+  STB_LAUNCH_CHECK("channel_rmsnorm_nhwc");
   return 0;
 }
 

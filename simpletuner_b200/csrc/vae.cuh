@@ -5,7 +5,9 @@
 //   groupnorm_stats_kernel : per (image, group) sum / sum-of-squares of x - pivot over H*W*(C/G)   (fp32 atomics)
 //   groupnorm_apply_kernel : (x - mean) * rstd * gamma + beta, optional SiLU, bf16 NHWC
 //   softmax_rows_kernel    : in-place row softmax of the mid-block attention scores (fp32 math)
-//   gaussian_sample_scale  : z = (mean + exp(0.5 clamp(logvar)) * eps - shift) * scale -> NCHW latents
+//   gaussian_sample_scale  : z = (mean + exp(0.5 clamp(logvar)) * eps - shift) * scale -> NCHW latents; shift and scale
+//                            are scalars (AutoencoderKL) or [L] vectors (Wan 2.1 / Qwen-Image latents_mean, 1 / latents_std)
+//   channel_rmsnorm_kernel : Wan 2.1 channel RMS norm F.normalize(x, dim=C) * sqrt(C) * gamma (+ bias), optional SiLU
 // reference: diffusers AutoencoderKL.encode as called at common.py:2766-2772, sampling at caching/vae.py:1337,
 // scaling at foundation_mixins.py:68-81.
 #pragma once
@@ -325,11 +327,14 @@ softmax_rows_kernel(__nv_bfloat16* __restrict__ s, long long row_stride, int col
   }
 }
 
-// moments: NHWC [B, h*w, 2L] (mean | logvar); eps: NCHW [B, L, h, w]; out: NCHW [B, L, h, w] (bf16)
+// moments: NHWC [B, h*w, 2L] (mean | logvar); eps: NCHW [B, L, h, w]; out: NCHW [B, L, h, w] (bf16).
+// shift_c / scale_c (both or neither): bf16 [L] vectors that replace the scalars, as in Qwen-Image's
+// post_vae_encode_transform_sample, bf16(bf16(z - latents_mean[c]) * (1 / latents_std)[c]).
 __global__ void __launch_bounds__(256)
 gaussian_sample_scale_kernel(const __nv_bfloat16* __restrict__ moments, const __nv_bfloat16* __restrict__ eps,
                              __nv_bfloat16* __restrict__ out, int B, int L, int hw, float shift, float scale,
-                             int has_shift) {
+                             int has_shift, const __nv_bfloat16* __restrict__ shift_c,
+                             const __nv_bfloat16* __restrict__ scale_c) {
   const long long total = (long long)B * L * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -343,8 +348,74 @@ gaussian_sample_scale_kernel(const __nv_bfloat16* __restrict__ moments, const __
     // DiagonalGaussianDistribution: std = exp(0.5 * logvar) (bf16 tensor), sample = mean + std * eps (bf16 ops)
     const float std = bf16r(__expf(0.5f * bf16r(logvar)));
     float z = bf16r(mean + bf16r(std * __bfloat162float(eps[i])));
-    z = has_shift ? bf16r(bf16r(z - shift) * scale) : bf16r(z * scale);
+    const float sh = shift_c ? __bfloat162float(shift_c[c]) : shift, sc = scale_c ? __bfloat162float(scale_c[c]) : scale;
+    z = has_shift ? bf16r(bf16r(z - sh) * sc) : bf16r(z * sc);
     out[i] = __float2bfloat16(z);
+  }
+}
+
+// Wan 2.1 channel RMS norm over the rows of x [rows, C] (NHWC pixels), C a multiple of 8 up to 512:
+// diffusers QwenImageRMS_norm, F.normalize(x, dim=C) * self.scale * self.gamma + self.bias, then (silu) the encoder's
+// separate SiLU.  Every step is a bf16 tensor in the eager module, so the kernel rounds after each one, in this order:
+//   n = bf16(sqrt(sum_c x_c^2))      the norm's fp32 sum of squares (overflows to inf as torch's does), one rounding
+//   n = max(n, bf16(eps))            clamp_min(eps) of F.normalize, eps = 1e-12 there (a NaN norm stays NaN)
+//   q = bf16(x / n)                  IEEE fp32 division
+//   s = bf16(q * scale)              scale = fp32(sqrt(C)), the Python float dim ** 0.5 as torch passes it
+//   g = bf16(s * gamma[c])
+//   y = bf16(g + bias[c])            without a bias module attribute the reference adds the Python float 0.0: y = g + 0
+//                                    (which turns -0 into +0)
+//   out = bf16(y / (1 + expf(-y)))   silu: torch's SiLU kernel, IEEE division and the accurate expf
+// Only the sum of squares is taken in another order than torch's; it moves n by at most (C + 4) 2^-24 relative before
+// the bf16 rounding.  A group of TPR lanes (the power of two >= C / 8, at most 32) owns a row; lane j holds the 8-channel
+// vector j (and j + 32 when TPR = 32), and a warp takes 32 / TPR rows at a time, so every lane of the warp takes part in the shuffles.
+template <int TPR>
+__global__ void __launch_bounds__(256)
+channel_rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ gamma,
+                       const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ out, long long rows, int C,
+                       float scale, float eps, int silu) {
+  constexpr int RPW = 32 / TPR;             // rows per warp and step
+  constexpr int VPL = TPR == 32 ? 2 : 1;     // 8-channel vectors per lane (C / 8 <= 64)
+  const int lane = threadIdx.x & 31, sub = lane / TPR, j = lane % TPR;
+  const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  const int nvec = C / 8;
+  const float n_min = bf16r(eps);           // torch casts the clamp_min scalar to the tensor's dtype
+  for (long long base = warp * RPW; base < rows; base += nwarps * RPW) {
+    const long long row = base + sub;
+    const bool live = row < rows;
+    float f[VPL][8];
+    float ss = 0.f;
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) {
+      const int c8 = j + v * TPR;
+      if (live && c8 < nvec) unpack8(*reinterpret_cast<const uint4*>(x + row * C + c8 * 8), f[v]);
+      else
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[v][e] = 0.f;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) ss += f[v][e] * f[v][e];
+    }
+#pragma unroll
+    for (int o = TPR / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    float n = bf16r(sqrtf(ss));
+    if (!(n != n)) n = fmaxf(n, n_min);      // a NaN norm stays NaN (fmaxf would return n_min)
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) {
+      const int c8 = j + v * TPR;
+      if (!live || c8 >= nvec) continue;
+      float o[8], gm[8], bs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      unpack8(__ldg(reinterpret_cast<const uint4*>(gamma + c8 * 8)), gm);
+      if (bias) unpack8(__ldg(reinterpret_cast<const uint4*>(bias + c8 * 8)), bs);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float q = bf16r(__fdiv_rn(f[v][e], n));
+        const float g = bf16r(bf16r(q * scale) * gm[e]);
+        float y = bf16r(g + bs[e]);
+        if (silu) y = __fdiv_rn(y, 1.f + expf(-y));
+        o[e] = y;
+      }
+      *reinterpret_cast<uint4*>(out + row * C + c8 * 8) = pack8(o);
+    }
   }
 }
 

@@ -432,10 +432,30 @@ def lokr_factor_grads(dW, w1, w2, scale: float):
     return dw1, dw2
 
 
-def rmsnorm_fwd(x, w, eps: float, out=None):
-    """T5LayerNorm: out = w * bf16(x * rsqrt(mean(x^2) + eps)) for a [B, S, D] view."""
+def rmsnorm_fwd(x, w, eps: float, out=None, *, normalize: bool = False, bias=None, silu: bool = False):
+    """RMS norm over the last dim of a [B, S, D] view, in one of two rounding forms:
+    T5LayerNorm (default): out = w * bf16(x * rsqrt(mean(x^2) + eps));
+    normalize=True, the Wan 2.1 VAE's channel norm: F.normalize(x, dim=-1, eps=eps) * sqrt(D) * w (+ bias) (+ SiLU),
+    rounded to bf16 after every op as the eager module is (csrc/vae.cuh); x and out contiguous, D a multiple of 8 up
+    to 512."""
     _chk(x, "x"); _chk(w, "w")
     B, S, D = x.shape
+    if normalize:
+        if bias is not None:
+            _chk(bias, "bias")
+        if out is None:
+            out = torch.empty((B, S, D), device=x.device, dtype=torch.bfloat16)
+        else:
+            _chk(out, "out")
+        if not x.is_contiguous() or not out.is_contiguous() or out.shape != x.shape:
+            raise ValueError("rmsnorm_fwd(normalize=True) needs contiguous x and out of the same shape")
+        if w.shape != (D,) or (bias is not None and bias.shape != (D,)):
+            raise ValueError(f"w and bias must be [{D}]")
+        check(_lib.lib().stb_channel_rmsnorm_nhwc(x.data_ptr(), w.data_ptr(), _ptr(bias), out.data_ptr(), B * S, D, float(eps),
+                                                  int(silu), _stream()))
+        return out
+    if bias is not None or silu:
+        raise ValueError("bias and silu belong to the normalize=True form")
     if out is None:
         out = torch.empty((B, S, D), device=x.device, dtype=torch.bfloat16)
     check(_lib.lib().stb_rmsnorm_fwd(x.data_ptr(), x.stride(0), x.stride(1), w.data_ptr(), out.data_ptr(), out.stride(0),
@@ -571,12 +591,12 @@ def note_graph_replay(n_kernels: int) -> None:
 
 # ---------------------------------------------------------------------------------------------- VAE encode
 def conv3x3_nhwc(x, w9, bias=None, res=None, stride: int = 1, out=None):
-    """x [B,H,W,Ci] NHWC contiguous; w9 [Co, 9*Ci] tap-major; returns [B,Ho,Wo,Co]."""
+    """x [B,H,W,Ci] NHWC contiguous; w9 [Co, 9*Cp] tap-major (conv_w9); returns [B,Ho,Wo,Co]."""
     _chk(x, "x"); _chk(w9, "w9")
     assert x.is_contiguous() and w9.is_contiguous()
     B, H, W, Ci = x.shape
     Co = w9.shape[0]
-    assert w9.shape[1] == 9 * Ci
+    assert w9.shape[1] == 9 * conv_tap_width(Ci)
     Ho, Wo = (H, W) if stride == 1 else (H // 2, W // 2)
     if out is None:
         out = torch.empty((B, Ho, Wo, Co), device=x.device, dtype=torch.bfloat16)
@@ -585,6 +605,22 @@ def conv3x3_nhwc(x, w9, bias=None, res=None, stride: int = 1, out=None):
     check(_lib.lib().stb_conv3x3_nhwc(x.data_ptr(), w9.data_ptr(), _ptr(bias), _ptr(res), out.data_ptr(),
                                       B, H, W, Ci, Co, stride, _stream()))
     return out
+
+
+def conv_tap_width(c_in: int) -> int:
+    """Columns per tap of a conv3x3_nhwc weight: C_in rounded up to a multiple of 64 (the kernel's channel box)."""
+    return -(-c_in // 64) * 64
+
+
+def conv_w9(w):
+    """[Co, Ci, 3, 3] -> the conv3x3_nhwc weight [Co, 9 * Cp]: tap-major (dy, dx, ci), each tap's channels zero-padded
+    from Ci to Cp = conv_tap_width(Ci)."""
+    Co, Ci = w.shape[:2]
+    t = w.detach().permute(0, 2, 3, 1)
+    Cp = conv_tap_width(Ci)
+    if Cp != Ci:
+        t = torch.nn.functional.pad(t, (0, Cp - Ci))
+    return t.reshape(Co, -1).contiguous()
 
 
 def conv_in_3ch(pixels, w, bias):
@@ -627,12 +663,21 @@ def softmax_rows_(s, scale: float):
 
 
 def gaussian_sample_scale(moments_nhwc, eps_nchw, shift, scale):
-    """moments [B, h, w, 2L] NHWC; eps [B, L, h, w]; returns scaled latents [B, L, h, w]."""
+    """moments [B, h, w, 2L] NHWC; eps [B, L, h, w]; returns scaled latents [B, L, h, w].  shift and scale are floats
+    (shift None: no shift) or both bf16 [L] tensors, bf16(bf16(z - shift[c]) * scale[c]) (Qwen-Image's latents_mean
+    and 1 / latents_std)."""
     _chk(moments_nhwc, "moments"); _chk(eps_nchw, "eps")
     B, h, w, L2 = moments_nhwc.shape
     L = L2 // 2
     assert moments_nhwc.is_contiguous() and eps_nchw.is_contiguous() and eps_nchw.shape == (B, L, h, w)
     out = torch.empty((B, L, h, w), device=moments_nhwc.device, dtype=torch.bfloat16)
+    if isinstance(shift, torch.Tensor) or isinstance(scale, torch.Tensor):
+        _chk(shift, "shift"); _chk(scale, "scale")
+        assert shift.shape == (L,) and scale.shape == (L,) and shift.is_contiguous() and scale.is_contiguous()
+        check(_lib.lib().stb_gaussian_sample_channel_norm(moments_nhwc.data_ptr(), eps_nchw.data_ptr(), out.data_ptr(), B, L,
+                                                          h * w, shift.data_ptr(), scale.data_ptr(), _stream()))
+        return out
     check(_lib.lib().stb_gaussian_sample_scale(moments_nhwc.data_ptr(), eps_nchw.data_ptr(), out.data_ptr(), B, L, h * w,
                                                float(shift or 0.0), float(scale), int(shift is not None), _stream()))
     return out
+

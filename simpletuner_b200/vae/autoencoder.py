@@ -121,17 +121,25 @@ class _MidAttention(nn.Module):
             self._qkv = (torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight], 0).detach().contiguous(),
                          torch.cat([self.to_q.bias, self.to_k.bias, self.to_v.bias], 0).detach().contiguous())
         t = ops.groupnorm_nhwc(x, self.group_norm.weight, self.group_norm.bias, self.groups, 1e-6, False).view(B, S, C)
-        qkv = ops.gemm([t], [self._qkv[0]], self._qkv[1])           # [B, S, 3C]
-        out = torch.empty((B, S, C), device=x.device, dtype=torch.bfloat16)
-        xr = x.view(B, S, C)
-        for b in range(B):  # one image at a time: the score matrix is S x S (512 MB at 1024^2)
-            q, k, v = qkv[b, :, 0:C], qkv[b, :, C:2 * C], qkv[b, :, 2 * C:]
-            s = ops.gemm([q], [k])                                   # [S, S] = q k^T
-            ops.softmax_rows_(s, C ** -0.5)
-            vt = v.t().contiguous()                                  # [C, S]: K-major "weight" for P @ V
-            o = ops.gemm([s], [vt])                                  # [S, C]
-            ops.gemm([o], [self.to_out[0].weight], self.to_out[0].bias, out=out[b], epi=ops.EPI_ADD_RES, res=xr[b])
-        return out.view(B, H, W, C)
+        return single_head_attention(t, x, self._qkv[0], self._qkv[1], self.to_out[0].weight, self.to_out[0].bias)
+
+
+def single_head_attention(t, x, w_qkv, b_qkv, w_out, b_out):
+    """x + out_proj(softmax(q k^T / sqrt(C)) v) for one head of width C over each image's pixels: t [B, S, C] is the
+    normalised input, x [B, H, W, C] the residual, w_qkv [3C, C] the q | k | v projection.  Returns [B, H, W, C]."""
+    B, H, W, C = x.shape
+    S = H * W
+    qkv = ops.gemm([t], [w_qkv], b_qkv)                              # [B, S, 3C]
+    out = torch.empty((B, S, C), device=x.device, dtype=torch.bfloat16)
+    xr = x.view(B, S, C)
+    for b in range(B):  # one image at a time: the score matrix is S x S (512 MB at 1024^2)
+        q, k, v = qkv[b, :, 0:C], qkv[b, :, C:2 * C], qkv[b, :, 2 * C:]
+        s = ops.gemm([q], [k])                                       # [S, S] = q k^T
+        ops.softmax_rows_(s, C ** -0.5)
+        vt = v.t().contiguous()                                      # [C, S]: K-major "weight" for P @ V
+        o = ops.gemm([s], [vt])                                      # [S, C]
+        ops.gemm([o], [w_out], b_out, out=out[b], epi=ops.EPI_ADD_RES, res=xr[b])
+    return out.view(B, H, W, C)
 
 
 class _MidBlock(nn.Module):
